@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the CtrLoRA denoising hot path on B200 (contract: see the task statement / DESIGN.md §Measurement).
+"""Benchmark of the CtrLoRA denoising hot path on H100 (see DESIGN.md §Measurement).
 
 Workload (BASELINE.json configs[1]): SD1.5 UNet + ControlNet (LoRA rank 128), 512x512 (latent 4x64x64), batch 4,
 DDIM with classifier-free guidance 7.5.  One "step" = one DDIM step = eps for the conditional and unconditional
@@ -8,6 +8,7 @@ offline), inputs synthetic.
 
     python bench.py [--gpus N] [--steps K] [--warmup W]            # this repo's CUDA path
     python bench.py --impl reference ...                           # the reference's algorithm on the host CPU (oracle port)
+    python bench.py --dump-outputs DIR ...                         # also write the last timed step's outputs as DIR/*.npy
 
 N > 1 (torchrun): sampling does not exchange anything between images, so ranks are independent replicas
 ("replicas only", DESIGN.md §Multi-GPU); value = N * K steps / max-over-ranks time.
@@ -28,6 +29,26 @@ sys.path.insert(0, ROOT)
 BATCH, LATENT, CTX_TOKENS, CTX_DIM, CFG_SCALE = 4, 64, 77, 768, 7.5
 CONFIG = os.path.join(ROOT, "configs", "ctrlora_finetune_sd15_rank128.yaml")
 GF_PER_IMAGE_PASS = 1103.4  # algorithmic forward GFLOP of ControlNet(r=128) + UNet per image (BASELINE.md §2)
+
+
+DUMP_SAMPLE = 1 << 20  # elements kept of an output larger than this
+
+
+def dump_outputs(directory, arrays):
+    """Write each tensor as <directory>/<name>.npy in float32.  A tensor above DUMP_SAMPLE elements is reduced to
+    DUMP_SAMPLE of its flattened elements at a fixed stride from a seeded offset (the choice depends only on the size),
+    so two builds compare 1:1 and the selection costs no index array of the full size."""
+    if not directory:
+        return
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    for name, t in arrays.items():
+        t = t.detach().float()
+        if t.numel() > DUMP_SAMPLE:
+            stride = t.numel() // DUMP_SAMPLE
+            offset = int(torch.randint(stride, (1,), generator=torch.Generator().manual_seed(12345)))
+            t = t.reshape(-1)[offset::stride][:DUMP_SAMPLE]
+        np.save(os.path.join(directory, f"{name}.npy"), t.cpu().numpy())
 
 
 def dist_env():
@@ -64,7 +85,7 @@ def build_model(device, seed=0, config=None):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -97,24 +118,12 @@ class ClockSampler(threading.Thread):
                 "samples": len(self.rows), "reasons": sorted(reasons)}
 
 
-def ncu_gemm_traffic():
-    """DRAM bytes of the GEMM family per DDIM step from the committed ncu launch list of this same workload
-    (profiles/r2_shares_ddim_step.json, written by tools/launch_shares.py from `ncu --metrics ...dram__bytes...` over
-    tools/profile_step.py); None when the capture is absent."""
-    path = os.path.join(ROOT, "profiles", "r2_shares_ddim_step.json")
-    try:
-        fam = json.load(open(path))["families"]["gemm_tcgen05"]
-        return fam["dram_bytes"] if fam["dram_bytes"] > 0 else None, os.path.relpath(path, ROOT)
-    except Exception:
-        return None, None
-
-
 def measured_peaks():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         d = json.load(open(path))
-        return d.get("bf16_tflops_sustained", 1412.1), d.get("hbm_gbs", 6569.6), "measured (MEASURED_PEAKS.json)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+        return d.get("bf16_tflops_sustained", 989.0), d.get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json)"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense fp16, HBM3)"
 
 
 def cpu_reference_pass(model_state, threads, n_images=1, seed=1):
@@ -214,16 +223,15 @@ def cpu_reference_step(model_state, seed=1):
 
 
 def run_reference(args, rank, world):
-    """--impl reference: the reference's CPU implementation of the path (oracle port; /root/reference is a Python tree that
-    cannot travel to the GPU box), same config / metric / unit.  One 'step' = one full DDIM step of the workload (two
-    batch-4 apply_model passes + the update), not an extrapolated sample; the step count is cut to fit a few minutes."""
+    """--impl reference: the reference's CPU implementation of the path (oracle port of the reference's Python tree),
+    same config / metric / unit.  One 'step' = one full DDIM step of the workload (two batch-4 apply_model passes + the
+    update), not an extrapolated sample; exactly --steps timed steps after one warm-up step (each takes seconds)."""
     if rank != 0:
         return
     sd = cpu_state_dict()
     threads, cores, probe = pick_cpu_threads(sd)
-    budget_s = 240.0
-    t_first = cpu_reference_step(sd)  # warm-up (also sizes the run)
-    steps = max(3, min(args.steps, int(budget_s / t_first) - 1))
+    cpu_reference_step(sd)  # warm-up
+    steps = args.steps
     times = sorted(cpu_reference_step(sd) for _ in range(steps))
     t_step = times[len(times) // 2]  # median: the arm has to be reproducible, a single stalled step must not move it
     value = 1.0 / t_step
@@ -241,7 +249,7 @@ def run_reference(args, rank, world):
 
 def run_reference_gpu(args, rank, world):
     """--impl reference-gpu: the library comparator SURVEY.md §8(d) asks for -- the reference's algorithm (oracle port: plain
-    torch ops = cuDNN / cuBLAS / ATen eager, N x N attention matrix materialised like the reference) on the SAME B200, in
+    torch ops = cuDNN / cuBLAS / ATen eager, N x N attention matrix materialised like the reference) on the same GPU, in
     fp32 and under bf16 autocast.  Two sequential batch-4 passes per step like the reference's sampler.  Not a product path."""
     if rank != 0:
         return
@@ -288,7 +296,7 @@ def workload_config(n):
                         "(latent 4x64x64), 77x768 context; cond+uncond batched as one batch-8 pass",
             "batch_per_gpu": BATCH, "cfg_scale": CFG_SCALE, "ddim_steps_schedule": 50,
             "parallelism": f"replicas x{n}" if n > 1 else "single GPU",
-            "l2": "no flush needed: 2.7 GB of fp16 weights stream through the 126 MB L2 every step"}
+            "l2": "no flush needed: 2.7 GB of fp16 weights stream through the 50 MB L2 every step"}
 
 
 TRAIN_BATCH = 16
@@ -335,6 +343,8 @@ def run_train(args, rank, local_rank, world, device):
     e1.record()
     barrier()
     ms_dev = e0.elapsed_time(e1)
+    if rank == 0:  # the loss of the last timed step and the trainable parameters it produced
+        dump_outputs(getattr(args, "dump_outputs", None), {"train_loss": loss.reshape(1), "train_params": trainer.G.flat_p})
     loss_host = torch.empty(1).pin_memory()
     h2d = sum(host[k].numel() * host[k].element_size() for k in order)
     for _ in range(2):
@@ -418,6 +428,8 @@ def run_pretrain(args, rank, local_rank, world, device):
     e1.record()
     barrier()
     ms_dev = e0.elapsed_time(e1)
+    if rank == 0:
+        dump_outputs(args.dump_outputs, {"pretrain_loss": loss.reshape(1), "pretrain_params": trainer.G.flat_p})
     loss_host = torch.empty(1).pin_memory()
     h2d = sum(host[k].numel() * host[k].element_size() for k in order)
     for _ in range(2):
@@ -498,10 +510,14 @@ def main():
     ap.add_argument("--lora-rank", type=int, default=128, choices=[32, 64, 128, 256, 512],
                     help="training workload only: BASELINE.json configs[4] rank sweep (default: the rank-128 headline)")
     ap.add_argument("--train-batch", type=int, default=TRAIN_BATCH, help="training workload: images per GPU per step")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the arrays the timed path returned in its last step as DIR/<name>.npy")
     ap.add_argument("--workload", default="sample+train", choices=["sample", "train", "sample+train", "pretrain"],
                     help="sample: configs[1] DDIM step (the headline line); train: configs[2] finetune step; default: both, "
                          "the training result rides in the line's 'train' key")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     rank, local_rank, world = dist_env()
     args.warmup = max(args.warmup, 3)
     if args.impl == "reference":
@@ -587,7 +603,7 @@ def main():
 
     # The module tree (3 000 modules, ~10^6 Python objects) is static from here on: move it out of the cyclic collector's
     # reach, as a serving process would -- a generation-2 pass over it costs ~100 ms and, landing inside the 20-step
-    # end-to-end loop, moved that figure between 49 and 64 steps/s from run to run (tools/debug_e2e.py: 15.54 ms/step steady).
+    # end-to-end loop, moves that figure from run to run.
     import gc
     gc.collect()
     gc.freeze()
@@ -601,11 +617,13 @@ def main():
     x = dev["x"]
     with sampler.run_mode():  # the K steps of a sampling run share their conditioning (as in DDIMSampler.sample)
         for i in range(args.steps):
-            x, _ = step(i, x)
+            x, pred_x0 = step(i, x)
     e1.record()
     barrier()
     ms_dev = e0.elapsed_time(e1)
     clk = clocks.stop()
+    if rank == 0:
+        dump_outputs(args.dump_outputs, {"sample_x_prev": x, "sample_pred_x0": pred_x0})
 
     # ---- (2) end to end through the public API with host buffers: H2D of the step's inputs, D2H of its result
     out_host = torch.empty(BATCH, 4, LATENT, LATENT).pin_memory()
@@ -634,7 +652,7 @@ def main():
     barrier()
     ms_e2e = f0.elapsed_time(f1)
 
-    # ---- roofline of the dominant kernel (tcgen05 implicit GEMM): the step's GEMM launches are recorded on an
+    # ---- roofline of the dominant kernel (wgmma implicit GEMM): the step's GEMM launches are recorded on an
     # un-graphed step, then replayed back to back from one CUDA graph between two CUDA events (ops.replay_gemms)
     gemm_stats = ops.replay_gemms(one_step_in_run, sampler)
     attn_stats = attention_roofline(device)
@@ -662,12 +680,10 @@ def main():
                 "gpu_launches": launches_per_step * args.steps,
                 "images_per_sec": value * BATCH,
                 "model_tflops": value / world * 2 * BATCH * GF_PER_IMAGE_PASS / 1e3,
-                "roofline": {"kernel": "gemm_tcgen05_kernel (all convs + linears of one step, replayed back to back from a CUDA graph)",
+                "roofline": {"kernel": "gemm_wgmma_kernel (all convs + linears of one step, replayed back to back from a CUDA graph)",
                              "bound": "tensor",
                              "achieved": ach, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach / peak_tf,
-                             "peak_source": peak_src + ", sustained bf16/fp16 dense", "traffic": ncu_gemm_traffic()[0],
-                             "traffic_unit": "DRAM bytes per step, all GEMM launches (ncu dram__bytes_read+write)",
-                             "traffic_source": ncu_gemm_traffic()[1],
+                             "peak_source": peak_src + ", sustained bf16/fp16 dense",
                              "launches": gemm_stats["launches"], "gflop_per_step": gemm_stats["flops"] / 1e9,
                              "share_of_step": gemm_stats["ms"] / (ms_dev / args.steps)}}
         # second kernel of the step (19 % of it): the d_head-40 self-attention of the 64x64 level, bound by exp2 throughput
@@ -675,7 +691,7 @@ def main():
         peak_exp = 16.0 * torch.cuda.get_device_properties(device).multi_processor_count * sm_mhz * 1e6 / 1e12
         a_ach = attn_stats["exps"] / (attn_stats["us"] * 1e-6) / 1e12
         line["roofline_attention"] = {
-            "kernel": "attention_stream64s_kernel (7 launches per step: 8 img x 8 heads x 4096 x 4096, d = 40)",
+            "kernel": "attention_kernel<48> (7 launches per step: 8 img x 8 heads x 4096 x 4096, d = 40)",
             "bound": "mufu (16 ex2 per clock per SM at the sampled SM clock)", "achieved": a_ach, "peak": peak_exp,
             "unit": "Texp/s", "frac": a_ach / peak_exp, "us_per_launch": attn_stats["us"],
             "tensor_tflops": attn_stats["flops"] / (attn_stats["us"] * 1e-6) / 1e12,

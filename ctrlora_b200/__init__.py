@@ -1,4 +1,4 @@
-"""ctrlora_b200 — B200-native (sm_100a) implementation of CtrLoRA's denoising hot path.
+"""ctrlora_b200 — H100-native (sm_90a) implementation of CtrLoRA's denoising hot path.
 
 `ctrlora_b200.csrc`     hand-written CUDA kernels + the C ABI (include/ctrlora_b200.h)
 `ctrlora_b200.ops`      tensor-level wrappers over the C ABI

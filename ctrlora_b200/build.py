@@ -1,4 +1,4 @@
-"""Builds ctrlora_b200/lib/libctrlora_b200.so (sm_100a only) with nvcc; no torch headers are involved.
+"""Builds ctrlora_b200/lib/libctrlora_b200.so (sm_90a only) with nvcc; no torch headers are involved.
 
 The library is in-tree so that it travels to the GPU box with the repo snapshot.  `build()` is idempotent: it
 recompiles only when a source is newer than the library.
@@ -15,7 +15,7 @@ LIB_PATH = os.path.join(LIB_DIR, "libctrlora_b200.so")
 OBJ_DIR = os.path.join(ROOT, "build")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xptxas", "-v", "-I", CSRC, "-I", INCLUDE,
 ]
 
@@ -53,7 +53,7 @@ def build(force=False, verbose=False):
             sys.stderr.write(out)
     if rebuilt or not os.path.exists(LIB_PATH):
         cmd = [nvcc, "-shared", "-o", LIB_PATH] + objs + ["-cudart", "static",
-               "-gencode", "arch=compute_100a,code=sm_100a"]
+               "-gencode", "arch=compute_90a,code=sm_90a"]
         r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}")

@@ -1,5 +1,5 @@
-// Shared device helpers for the sm_100a kernels: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 / TMEM wrappers.
-// Everything here is inline PTX for sm_100a; there is no fallback for other architectures.
+// Shared device helpers for the sm_90a kernels: mbarrier, TMA (cp.async.bulk.tensor), wgmma operand descriptors.
+// Everything here is inline PTX for sm_90a; there is no fallback for other architectures.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -87,59 +87,30 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
         : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---------------------------------------------------------------- wgmma shared-memory operand descriptors
+// Operand tiles are what a TMA box with CU_TENSOR_MAP_SWIZZLE_128B produces: rows of 128 bytes (64 fp16), 8-row
+// groups of 1024 B, the 16-byte chunks of row r XOR-permuted by (r & 7).  Tile bases must be 1024-byte aligned.
+// K-major (contraction dimension contiguous): SBO = 1024 between 8-row groups, LBO unused; a k16 step is +32 B.
+__device__ __forceinline__ uint64_t wgmma_desc_kmajor(uint32_t smem_addr) {
+    uint64_t d = 0;
+    d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
+    d |= static_cast<uint64_t>(1) << 16;
+    d |= static_cast<uint64_t>(1024 >> 4) << 32;
+    d |= static_cast<uint64_t>(1) << 62;  // SWIZZLE_128B
+    return d;
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+// MN-major (the M / N dimension contiguous, e.g. a [tokens][features] tile contracted over tokens): 64-element atoms
+// `lbo_bytes` apart along M / N, 8-row groups 1024 B apart along K; a k16 step is +2048 B.
+__device__ __forceinline__ uint64_t wgmma_desc_mnmajor(uint32_t smem_addr, uint32_t lbo_bytes) {
+    uint64_t d = 0;
+    d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
+    d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
+    d |= static_cast<uint64_t>(1024 >> 4) << 32;
+    d |= static_cast<uint64_t>(1) << 62;
+    return d;
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]; kind::f16 covers fp16 and bf16 operands with fp32 accumulation.
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                         uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp receives row (lane base + i).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t* v) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t* v) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x1(uint32_t taddr, uint32_t& v) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(v) : "r"(taddr) : "memory");
+__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 __device__ __forceinline__ float max3f(float a, float b, float c) {
     float r;
@@ -151,29 +122,9 @@ __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
     asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
     return r;
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major operand tile in shared memory, rows of 128 bytes, SWIZZLE_128B (what a TMA box with
-// CU_TENSOR_MAP_SWIZZLE_128B produces): 8-row groups are 1024 B apart (SBO), LBO is 1 for swizzled K-major,
-// descriptor version 1 (Blackwell), layout type 2.  The tile base must be 1024-byte aligned.
-__device__ __forceinline__ uint64_t umma_desc_kmajor_sw128(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
-    d |= static_cast<uint64_t>(1) << 16;            // leading byte offset (unused for swizzled K-major)
-    d |= static_cast<uint64_t>(1024 >> 4) << 32;    // stride byte offset between 8-row groups
-    d |= static_cast<uint64_t>(1) << 46;            // version
-    d |= static_cast<uint64_t>(2) << 61;            // SWIZZLE_128B
-    return d;
-}
-// Instruction descriptor for kind::f16: fp32 accumulate, A and B K-major. fmt: 0 = fp16, 1 = bf16.
-__device__ __host__ __forceinline__ uint32_t umma_idesc_f16(int m, int n, int fmt) {
-    return (1u << 4) | (static_cast<uint32_t>(fmt) << 7) | (static_cast<uint32_t>(fmt) << 10) |
-           (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
-}
-
 // ---------------------------------------------------------------- programmatic dependent launch (PDL)
 // Every hot kernel starts with launch_dependents (the next kernel in the stream may begin its prologue: barrier init,
-// TMEM allocation, descriptor prefetch) and executes wait before its first global-memory access.
+// descriptor prefetch) and executes wait before its first global-memory access.
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
@@ -296,10 +247,8 @@ __device__ __forceinline__ float gelu_erf_f(float x) {
 
 }  // namespace ctrl
 
-// ---------------------------------------------------------------- 2-CTA (cta_group::2) helpers
+// ---------------------------------------------------------------- clusters
 namespace ctrl {
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;  // clears the CTA-rank bit of a shared::cluster address -> the pair's CTA 0
-
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -307,47 +256,6 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 }
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// TMA loads issued by either CTA of the pair; the transaction bytes land on CTA 0's mbarrier
-__device__ __forceinline__ void tma_load_3d_2cta(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(
-            smem_u32(dst)),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2cta(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], "
-        "[%2];" ::"r"(smem_u32(dst)),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-__device__ __forceinline__ void umma_f16_2cta(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on the same-offset mbarrier of both CTAs once the issued MMAs have completed
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                     smem_u32(bar)),
-                 "h"(static_cast<uint16_t>(3))
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// arrive on CTA 0's copy of `bar` (local arrive when executed by CTA 0)
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask) : "memory");
 }
 // ---------------------------------------------------------------- raw shared-address variants for single-thread hot loops
 // (the generic->shared conversion and pointer arithmetic are hoisted out of the loop by the caller)
@@ -379,43 +287,8 @@ __device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity) {
 __device__ __forceinline__ void mbar_expect_tx_a(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
-template <bool TWO_CTA>
-__device__ __forceinline__ void tma_load_3d_a(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2) {
-    if (TWO_CTA)
-        asm volatile(
-            "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
-            "l"(reinterpret_cast<uint64_t>(m)), "r"(bar & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2)
-            : "memory");
-    else
-        asm volatile(
-            "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
-            "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-            : "memory");
-}
-template <bool TWO_CTA>
-__device__ __forceinline__ void tma_load_4d_a(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2, int c3) {
-    if (TWO_CTA)
-        asm volatile(
-            "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(dst),
-            "l"(reinterpret_cast<uint64_t>(m)), "r"(bar & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-            : "memory");
-    else
-        asm volatile(
-            "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(dst),
-            "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-            : "memory");
-}
-template <bool TWO_CTA>
-__device__ __forceinline__ void umma_commit_a(uint32_t bar) {
-    if (TWO_CTA)
-        asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-                     "h"(static_cast<uint16_t>(3))
-                     : "memory");
-    else
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// (elect_one above) lets the compiler keep the surrounding loop in warp-uniform control flow so that TMA / tcgen05
-// operands live in uniform registers; a `lane == 0` branch costs an ELECT + R2UR waterfall per instruction.
+// (elect_one above) lets the compiler keep the surrounding loop in warp-uniform control flow so that TMA operands live
+// in uniform registers; a `lane == 0` branch costs an ELECT + R2UR waterfall per instruction.
 __device__ __forceinline__ int uniform_warp_idx() { return __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0); }
 // ---------------------------------------------------------------- TMA stores (shared -> global, bulk async-group completion)
 __device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2, int c3) {
@@ -430,16 +303,6 @@ template <int N>
 __device__ __forceinline__ void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 template <int N>
 __device__ __forceinline__ void bulk_wait_group() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
-// 32 lanes x 16 consecutive fp32 columns, registers -> TMEM (the mirror of tmem_ld_32x16)
-__device__ __forceinline__ void tmem_st_32x16(uint32_t taddr, const uint32_t* v) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-        "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]),
-        "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 // Spin on mbarrier.test_wait (no hardware suspend): lowest wake-up latency, for waits that sit on a per-tile critical chain.
 __device__ __forceinline__ void mbar_wait_spin(uint64_t* bar, uint32_t parity) {
     const uint32_t a = smem_u32(bar);
@@ -476,22 +339,6 @@ __device__ __forceinline__ float4 lds128f(uint32_t addr) {
     return v;
 }
 __device__ __forceinline__ void sts32f(uint32_t addr, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory"); }
-// D[tmem] (+)= A[tmem] * B[smem]: the A operand ([128 lanes] x [K/2 32-bit columns], two fp16 per column, written with
-// tcgen05.st by the thread that owns the lane) never touches shared memory: no 4 KiB-per-MMA smem A read (the SS form
-// costs max(N/2, 32 + N/4) cycles per K=16 step, this one N/2 -- tools/microbench/mma_issue.cu).
-__device__ __forceinline__ void umma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x8(uint32_t taddr, const uint32_t* v) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(v[0]), "r"(v[1]),
-                 "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-                 : "memory");
-}
 // exp2 on the FMA pipe (Cody-Waite split + degree-3 minimax on [-0.5, 0.5], max relative error 1.1e-4: below fp16's
 // half-ulp). The softmax / backward row math is MUFU-bound (16 ex2 per clock per SM); evaluating every fourth
 // exponential this way moves a quarter of that load to the otherwise idle FMA pipe (the FlashAttention-4 trick).

@@ -1,4 +1,4 @@
-// CUDA-core twin of the tcgen05 implicit GEMM (same argument block, same epilogue semantics).  It exists to bisect
+// CUDA-core twin of the wgmma implicit GEMM (same argument block, same epilogue semantics).  It exists to bisect
 // tensor-core / TMA descriptor bugs on the GPU box; the product path never calls it.
 #include "common.cuh"
 #include "ctrlora_b200.h"

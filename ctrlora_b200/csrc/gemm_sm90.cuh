@@ -1,0 +1,53 @@
+// Kernel-side parameter block of the wgmma implicit-GEMM kernel (see gemm_sm90.cu).
+#pragma once
+#include "common.cuh"
+
+namespace ctrl {
+
+constexpr int GEMM_BM = 128;            // two consumer warpgroups x wgmma M = 64
+constexpr int GEMM_BK = 64;             // 64 fp16 = 128 B = one SWIZZLE_128B row
+constexpr int GEMM_MAX_BN = 128;        // wgmma N of one tile (GEGLU: value half + gate half); 64 accumulators per thread
+constexpr int GEMM_MAX_STAGES = 8;
+constexpr int GEMM_A_BYTES = GEMM_BM * GEMM_BK * 2;   // 16 KiB
+constexpr int GEMM_THREADS = 384;       // warpgroup 0: TMA producer (one thread), warpgroups 1-2: wgmma + epilogue
+constexpr int GEMM_CONSUMERS = 256;
+constexpr int GEMM_SMEM_DATA = 192 * 1024;            // operand ring; the epilogue stages the fp32 tile over it
+constexpr int GEMM_STAGE_LD = GEMM_MAX_BN + 4;        // fp32 row pitch of the epilogue staging tile
+constexpr int GEMM_SMEM_BYTES = GEMM_SMEM_DATA + 1024 /*align slack*/ + 256 /*barriers*/ + 2048 /*bias staging*/;
+
+struct GemmKParams {
+    // tile geometry over the (B, H, W) pixel grid; a plain [M, K] matrix is B=1, H=1, W=M
+    int W, H, Bn;
+    int bw, bh, nb;                 // TMA box of one 128-row tile: nb * bh * bw == 128
+    int tiles_w, tiles_h, tiles_b;  // ceil-div of the dims above by the box
+    int N;                          // output columns
+    int BN;                         // wgmma N of one tile (GEGLU: value half + gate half)
+    int n_tiles;
+    int taps, kw, pad;              // filter taps (1 or 9), filter width, zero padding
+    int kchunks;                    // ceil(Cin / 64) per tap
+    int kchunks2;                   // extra 1x1 segment from the second operand pair (0 = none)
+    int geglu;                      // 1: weights are [2N, K]; out = value * gelu(gate)
+    int stages, stage_bytes;        // TMA ring: stage = A tile (16 KiB) + B tile (BN * 128 B, 1 KiB aligned)
+    int splits, kiters_per_split;   // split-K: partial sums meet in `ws` (fp32, self-cleaning), last CTA runs the epilogue
+    float* ws;
+    unsigned int* counters;
+    // epilogue
+    void* out[3];
+    int seg_width;                  // 0: single output; else column n goes to out[n / seg_width]
+    int transposed[3];              // store segment as [img, head, d, tok_pad] (V^T for attention)
+    int ldc;
+    int out_f32;
+    const float* bias;              // [N] (GEGLU: [2N])
+    const float* rowbias;           // [images, rowbias_ld]  per-image additive term (time embedding)
+    int rows_per_img;
+    int rowbias_ld;
+    int residual_f32;
+    const __half* residual;         // [M, ldr]
+    int ldr;
+    float out_scale;
+    int head_dim, tok_pad;
+    __half* dup_out;               // transposed segments are ALSO stored row-major here (training keeps natural V)
+    int dup_ld;
+};
+
+}  // namespace ctrl

@@ -397,7 +397,7 @@ extern "C" int ctrlora_colsum(const void* x, int x_is_f32, long long ld, long lo
     if (!x || !out) return CTRLORA_ERR_ARG;
     if (!x_is_f32 && cols % 8 == 0 && ld % 8 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {
         const int vecs = cols / 8, xb = (vecs + 31) / 32;
-        long long ys = (2 * 148 + xb - 1) / xb;  // about two blocks per SM
+        long long ys = (2 * 132 + xb - 1) / xb;  // about two blocks per SM of an H100
         if (ys > rows / 64) ys = rows / 64;
         if (ys < 1) ys = 1;
         launch_pdl(colsum_vec_kernel, dim3(xb, (unsigned)ys), dim3(256), (size_t)0, STREAM(stream),
@@ -474,7 +474,7 @@ extern "C" int ctrlora_adamw_begin(int* step_counter, const int* skip_flag, floa
 extern "C" int ctrlora_nonfinite_flag_f32(const float* x, long long n, int* flag, void* stream) {
     if (!x || !flag || (reinterpret_cast<uintptr_t>(x) & 15)) return CTRLORA_ERR_ARG;
     long long blocks = (n / 4 + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     if (blocks < 1) blocks = 1;
     nonfinite_flag_kernel<<<static_cast<unsigned>(blocks), 256, 0, STREAM(stream)>>>(x, n, flag);
     return LAUNCH_OK();

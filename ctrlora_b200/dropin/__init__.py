@@ -3,7 +3,7 @@
 `ctrlora_b200/dropin` is a directory of top-level packages named like the reference's (`cldm`, `ldm`): put it first
 on sys.path (see `activate()`) and `cldm.model.create_model`, the YAML `target:` strings, `cldm.lora`,
 `cldm.ddim_hacked.DDIMSampler`, `ldm.modules.attention`, `ldm.modules.diffusionmodules.openaimodel` resolve to the
-B200-native implementation.  INTEGRATION.md shows the file-level overlay onto a reference checkout.
+H100-native implementation.  INTEGRATION.md shows the file-level overlay onto a reference checkout.
 """
 import os
 import sys

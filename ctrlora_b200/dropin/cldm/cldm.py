@@ -1,7 +1,7 @@
 """Drop-in for the reference's `cldm/cldm.py`: `ControlledUnetModel`, `ControlNet`, `ControlLDM`.
 
 Data flow of one `apply_model` (reference :329-344 and cldm_ctrlora_finetune.py:67-82):
-    ControlNet: 12 input blocks, each followed by its 1x1 zero-conv (a tcgen05 GEMM), middle block, middle_block_out
+    ControlNet: 12 input blocks, each followed by its 1x1 zero-conv (a wgmma GEMM), middle block, middle_block_out
     -> 13 residuals (pixel-major fp16, returned as logical-NCHW views)
     UNet: encoder + middle, then for each decoder block the next ResBlock's GroupNorm kernel reads
     [h (+ s*c_mid) | hs_i + s_i*c_i] in place: the residual adds, the control_scales multiply and torch.cat of the
@@ -267,5 +267,5 @@ class ControlLDM(LatentDiffusion):
         return torch.optim.AdamW(params, lr=lr)
 
     def low_vram_shift(self, is_diffusing):
-        """Kept for API compatibility (reference :428-438): a 180 GB B200 holds every stage at once, nothing moves."""
+        """Kept for API compatibility (reference :428-438): an 80 GB H100 holds every stage at once, nothing moves."""
         return None

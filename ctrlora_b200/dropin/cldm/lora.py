@@ -4,7 +4,7 @@ state-dict keys (`<linear>.lora_layer.{down,up}.weight`).
 
 At run time the reference evaluates `W x + b + scale * up(down(x))` as three GEMMs and an add per call
 (lora.py:285-291).  Here the low-rank delta is folded into the fp16 kernel copy of the weight
-(`ctrlora_b200.prepare.lora_folded_weight`, one tcgen05 GEMM per weight version), so a LoRA linear costs exactly one
+(`ctrlora_b200.prepare.lora_folded_weight`, one wgmma GEMM per weight version), so a LoRA linear costs exactly one
 GEMM per call; the fp32 master parameters (`weight`, `lora_layer.down/up.weight`) stay separate and trainable.
 """
 from typing import Optional

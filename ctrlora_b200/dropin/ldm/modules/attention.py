@@ -1,5 +1,5 @@
 """Drop-in for the reference's `ldm/modules/attention.py`: same class names, constructor signatures, attribute tree
-and state-dict keys; the arithmetic runs in the sm_100a kernels.
+and state-dict keys; the arithmetic runs in the sm_90a kernels.
 
 Kernel sequence of one SpatialTransformer (reference :321-340 and :271-275), all on pixel-major fp16 so the
 'b c h w -> b (h w) c' rearranges (:330,:337) cost nothing:

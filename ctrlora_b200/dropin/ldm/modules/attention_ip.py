@@ -5,8 +5,8 @@
     out = to_out( softmax(q k^T) v  +  ip_scale * softmax(q k_ip^T) v_ip )
 
 Here the second stream reuses the projected queries, runs the single-tile attention kernel over the (4 .. 16) image
-tokens, and its output enters `to_out` as the SECOND OPERAND PAIR of the same tcgen05 GEMM
-(o @ Wo^T + o_ip @ (ip_scale Wo)^T accumulate in one TMEM tile): no separate add pass, no extra rounding of the sum.
+tokens, and its output enters `to_out` as the SECOND OPERAND PAIR of the same wgmma GEMM
+(o @ Wo^T + o_ip @ (ip_scale Wo)^T accumulate in one register tile): no separate add pass, no extra rounding of the sum.
 """
 import torch
 import torch.nn as nn

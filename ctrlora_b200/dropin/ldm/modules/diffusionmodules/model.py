@@ -1,13 +1,13 @@
 """Drop-in for the reference's `ldm/modules/diffusionmodules/model.py`: the first-stage VAE's `Encoder` / `Decoder`
 (and their `ResnetBlock`, `AttnBlock`, `Downsample`, `Upsample`) with the reference's constructor kwargs, attribute tree
-and state-dict keys, evaluated on the same sm_100a kernels as the UNet (SURVEY.md §8 rows f1 / f3).
+and state-dict keys, evaluated on the same sm_90a kernels as the UNet (SURVEY.md §8 rows f1 / f3).
 
 Why it is on the path: every CtrLoRA `apply_model` starts with `0.18215 * VAE.encode(hint).sample()`
 (cldm/cldm_ctrlora_finetune.py:76-77) -- 1117 GFLOP per 512x512 image, more than the ControlNet + UNet pass it feeds.
 
 Kernel sequence (all pixel-major fp16, fp32 accumulation / statistics):
     ResnetBlock   groupnorm(eps 1e-6)+swish -> conv3x3 implicit GEMM -> groupnorm+swish -> conv3x3 (+ identity residual, or the
-                  1x1 nin_shortcut accumulated into the same TMEM tile)                        reference :129-149
+                  1x1 nin_shortcut accumulated into the same accumulator tile)                        reference :129-149
     Downsample    F.pad(0,1,0,1) + conv3x3 stride 2 = right/bottom-padded stride-2 gather + plain GEMM      :80-84
     Upsample      nearest x2 + conv3x3                                                                       :61-65
     AttnBlock     groupnorm -> one [q|k|v] GEMM (V stored transposed) -> per image: fp32 logits GEMM (q k^T), row softmax,

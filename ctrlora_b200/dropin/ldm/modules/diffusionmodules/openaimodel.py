@@ -3,7 +3,7 @@ Down/Upsample and UNetModel with the reference's constructor kwargs, attribute t
 
 Kernel sequence of one ResBlock (reference ResBlock._forward :254-274):
     groupnorm+SiLU -> conv3x3 implicit GEMM (+bias + time-embedding row term) -> groupnorm+SiLU ->
-    conv3x3 implicit GEMM (+bias + skip: residual read, or the 1x1 skip conv accumulated into the same TMEM tile)
+    conv3x3 implicit GEMM (+bias + skip: residual read, or the 1x1 skip conv accumulated into the same accumulator tile)
 Decoder blocks take their `cat([h, hs.pop() + control.pop()], 1)` input as a CatSpec: the first GroupNorm reads the
 pieces in place.
 """
@@ -51,7 +51,7 @@ class TimestepEmbedSequential(nn.Sequential, TimestepBlock):
 
 
 class _Conv(nn.Conv2d):
-    """nn.Conv2d parameter holder whose forward is the tcgen05 implicit GEMM (3x3 pad 1 / 1x1, stride 1)."""
+    """nn.Conv2d parameter holder whose forward is the wgmma implicit GEMM (3x3 pad 1 / 1x1, stride 1)."""
 
     def _cache(self):
         c = self.__dict__.get("_prep")

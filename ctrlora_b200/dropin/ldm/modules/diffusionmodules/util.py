@@ -1,6 +1,6 @@
 """Primitives of the denoising path, mirroring the names exported by the reference's
 `ldm/modules/diffusionmodules/util.py`.  Schedules are host-side numpy (as in the reference); everything that touches
-activations runs in the sm_100a kernels (ctrlora_b200.ops) — there is no torch/CPU fallback for those.
+activations runs in the sm_90a kernels (ctrlora_b200.ops) — there is no torch/CPU fallback for those.
 """
 import math
 
@@ -126,5 +126,5 @@ def zero_module(module):
 
 def checkpoint(func, inputs, params, flag):
     """The reference recomputes the forward inside backward (util.py:102-151) to save memory; results are identical
-    (dropout p = 0).  A B200 keeps the activations, so this is a plain call."""
+    (dropout p = 0).  An 80 GB H100 keeps the activations, so this is a plain call."""
     return func(*inputs)

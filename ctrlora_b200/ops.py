@@ -122,7 +122,7 @@ def _ptr(t):
 def _require_cuda(*ts):
     for t in ts:
         if t is not None and not t.is_cuda:
-            raise _lib.CtrloraError("ctrlora_b200 ops need CUDA tensors (sm_100a); there is no CPU path")
+            raise _lib.CtrloraError("ctrlora_b200 ops need CUDA tensors (sm_90a); there is no CPU path")
 
 
 def _as_bhwc(a):

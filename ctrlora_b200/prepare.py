@@ -87,7 +87,7 @@ def conv_weight(weight, pad_in=None, pad_out=None):
 def lora_folded_weight(weight, down, up, scale=1.0, out=None):
     """W' = W + scale * up @ down as fp16 [N, 1, K]  (cldm/lora.py:250 `_fuse_lora`, evaluated in fp32 accumulate).
 
-    One tcgen05 GEMM: A = up [N, r], B = down^T [K, r], epilogue adds the fp32 master W.  Cost 2*N*K*r flop, once per
+    One wgmma GEMM: A = up [N, r], B = down^T [K, r], epilogue adds the fp32 master W.  Cost 2*N*K*r flop, once per
     weight version (per optimizer step in training, once per checkpoint in sampling) instead of two skinny GEMMs and an
     add per forward call (cldm/lora.py:285-291)."""
     n, k = weight.shape

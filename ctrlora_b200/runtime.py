@@ -15,7 +15,7 @@ def pixel_major(x, c_pad=None):
     if x.dim() != 4:
         raise ValueError(f"expected a [B,C,H,W] tensor, got {tuple(x.shape)}")
     if not x.is_cuda:
-        raise RuntimeError("ctrlora_b200 runs on CUDA (sm_100a) only: move the model and inputs to the GPU")
+        raise RuntimeError("ctrlora_b200 runs on CUDA (sm_90a) only: move the model and inputs to the GPU")
     if x.dtype == torch.float16:
         v = x.permute(0, 2, 3, 1)
         if v.is_contiguous() and c_pad in (None, x.shape[1]):

@@ -1,4 +1,4 @@
-"""CtrLoRA finetune training step on the sm_100a kernels: forward with saved activations, hand-scheduled backward,
+"""CtrLoRA finetune training step on the sm_90a kernels: forward with saved activations, hand-scheduled backward,
 flat-buffer NCCL all-reduce of the trainable gradients and fused AdamW.
 
 reference call stack (SURVEY.md §3.1): LatentDiffusion.p_losses (ldm/models/diffusion/ddpm.py:885-920) ->
@@ -11,7 +11,7 @@ reaches (385 M ControlNet + UNet decoder weights it never uses).  Here only what
   * activation gradients through the ControlNet,
   * weight gradients for LoRA down/up (factored: dUp = dY^T (X Down^T), dDown = (dY Up)^T X), zero-convs, and the
     'norm'-named GroupNorm / LayerNorm affine parameters.
-The reference's activation checkpointing (util.py:102-151) is replaced by simply keeping the activations (180 GB HBM).
+The reference's activation checkpointing (util.py:102-151) is replaced by simply keeping the activations (they fit the 80 GB of an H100).
 The M = batch time-embedding MLP (time_embed, emb_layers: 12 tiny LoRA linears) is differentiated with torch fp32
 matmuls on [B, 1280] tensors -- negligible work, documented in DESIGN.md.
 """
@@ -800,11 +800,9 @@ class FinetuneTrainer:
 
     def _cuts(self):
         """Backward stages after which a gradient bucket is closed and its all-reduce started (CTRLORA_ALLREDUCE_CUTS, comma
-        separated subset of middle,ib9,ib6,ib3; empty = one all-reduce after the backward).  Default: EMPTY.  Measured on
-        8 x B200 (profiles/r2_scaling_experiments.txt): no cut 74.77 ms/step, one cut after input_blocks.3 (89 % of the
-        buffer reduced under the three 64x64 blocks' backward) 75.07 ms, all four cuts 75.14 ms -- every cut splits the CUDA
-        graph, and NCCL's CTAs take SMs away from the persistent one-CTA-per-SM GEMMs they overlap with, which costs more
-        than the ~1 ms of all-reduce it hides.  The machinery stays for longer collectives (more ranks, multi-node)."""
+        separated subset of middle,ib9,ib6,ib3; empty = one all-reduce after the backward).  Default: EMPTY: every cut splits
+        the CUDA graph and the collective's CTAs compete with the backward it overlaps, which pays only for collectives
+        longer than the finetune step's (more ranks, multi-node)."""
         import os
         cuts = getattr(self, "allreduce_cuts", None)
         if cuts is None:
@@ -1035,9 +1033,8 @@ class PretrainTrainer(FinetuneTrainer):
     def _overlap_cuts(self):
         """Backward stages that close a bucket whose all-reduce then runs under the rest of the backward
         (CTRLORA_PRETRAIN_ALLREDUCE_CUTS, default all four: middle,ib9,ib6,ib3; empty = one exchange after the backward).
-        The dense gradient buffer is 1.5 GB; measured on 2 x B200 (profiles/r2_scaling_experiments.txt): one exchange after
-        the backward 53.2 ms/step, cuts ib9 52.6, ib9+ib6 52.1-52.7, all four 52.0 -- about a third of the 3.4 ms exchange is
-        hidden; the rest is lost to the collective's CTAs and HBM traffic competing with the backward it overlaps."""
+        The dense gradient buffer is 1.5 GB, so part of its exchange can hide under the backward; the rest is lost to the
+        collective's CTAs and HBM traffic competing with the backward it overlaps."""
         import os
         cuts = getattr(self, "allreduce_cuts", None)
         if cuts is None:

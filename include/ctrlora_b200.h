@@ -1,7 +1,7 @@
 /* ctrlora_b200 C ABI — the drop-in boundary underneath the reference's Python module contract.
  *
  * The reference (xyfJASON/ctrlora) has no FFI of its own: its hot path is torch calls (SURVEY.md §8b).  Every entry
- * point below replaces one group of those torch call sites with a hand-written sm_100a kernel; the reference file:line
+ * point below replaces one group of those torch call sites with a hand-written sm_90a kernel; the reference file:line
  * each one stands in for is cited on the declaration.  Conventions: plain pointers and sizes, device pointers unless
  * stated, no allocation inside (workspaces are passed in), the launch goes on `stream` (a cudaStream_t passed as
  * void*), the return value is a status code (0 = ok), no exceptions cross the boundary.
@@ -33,7 +33,7 @@ const char* ctrlora_last_cuda_error(void);
 int ctrlora_memset_zero(void* ptr, long long bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
- * Implicit GEMM on the 5th-gen tensor cores (tcgen05, accumulators in TMEM, operands staged by TMA):
+ * Implicit GEMM on the Hopper tensor cores (wgmma, accumulators in registers, operands staged by TMA):
  *   out[m, n] = epilogue( sum_{tap, c} A[pixel(m) + tap_offset, c] * W[n, tap, c]  (+ sum_c A2[pixel(m), c] * W2[n, c]) )
  * replaces  nn.Linear / F.linear              ldm/modules/attention.py:154-161,52,72; cldm/lora.py:287-290
  *           nn.Conv2d 1x1 and 3x3 stride 1    ldm/modules/diffusionmodules/openaimodel.py:196,228-240,729; cldm/cldm.py:281-282
@@ -78,7 +78,7 @@ typedef struct ctrlora_gemm_args {
     int splitk_counters_len;
     void* dup_out;          /* optional: transposed segments are also stored row-major here (fp16, row stride dup_ld) */
     int dup_ld;
-    int force_single_cta;   /* 1: never use the 2-CTA (cta_group::2) tile pairs (tests / bisecting) */
+    int force_single_cta;   /* accepted for ABI compatibility; every tile is one CTA */
 } ctrlora_gemm_args;
 
 int ctrlora_gemm_f16(const ctrlora_gemm_args* args, void* stream);

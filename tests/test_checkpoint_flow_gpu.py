@@ -16,6 +16,7 @@ GOLD = os.path.join(ROOT, "tests", "golden")
 pytestmark = pytest.mark.gpu
 
 from tolerances import TOL  # noqa: E402
+from golden_io import load_golden  # noqa: E402
 
 
 def rel(a, b):
@@ -47,7 +48,7 @@ def test_extract_combine_load_flow_reproduces_the_pretrained_tasks():
     from cldm.lora import LoRACompatibleLinear
     from cldm.model import create_model
     from oracle import synth
-    g = torch.load(os.path.join(GOLD, "tiny_variants_golden.pt"), weights_only=False)
+    g = load_golden(os.path.join(GOLD, "tiny_variants_golden.pt"))
     seed = g["seed"]
     pre = create_model(os.path.join(GOLD, "tiny_pretrain.yaml"), init_weights=False)
     assert isinstance(pre, ControlPretrainLDM)

@@ -1,5 +1,5 @@
 """N > 1 host logic on CPU (gloo, world_size 2): the flat trainable-gradient buffer, its single all-reduce and the
-replica consistency of the parameter set.  No kernels run here (they need sm_100a); the GPU-side arithmetic is covered
+replica consistency of the parameter set.  No kernels run here (they need sm_90a); the GPU-side arithmetic is covered
 by tests/test_train_gpu.py."""
 import os
 import sys

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 implicit GEMM (ctrlora_gemm_f16) against torch fp32 on the same fp16-rounded operands.
+"""GPU parity of the wgmma implicit GEMM (ctrlora_gemm_f16) against torch fp32 on the same fp16-rounded operands.
 
 Tolerance: fp16 output rounding (2^-11 relative) + fp32 accumulation-order differences -> 2e-3 * max|ref| absolute.
 """

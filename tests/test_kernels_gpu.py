@@ -86,7 +86,7 @@ def _attn_ref(q, k, v, B, H, Nq, Nk, d):
     (1, 4, 64, 520, 8),
     (2, 4, 256, 256, 32),
     (1, 2, 130, 129, 64),
-    (1, 8, 600, 700, 40),     # ragged multi-tile: masked last key tile with P in TMEM and the ones-row row sums
+    (1, 8, 600, 700, 40),     # ragged multi-tile: masked last key tile (keys beyond Nk masked)
     (1, 2, 300, 1000, 24),    # d16 = 32 < DPAD = 48
     (1, 2, 384, 640, 48),     # d a multiple of 16: row sums through the P x ones product
 ])

@@ -14,6 +14,7 @@ GOLD = os.path.join(ROOT, "tests", "golden")
 pytestmark = pytest.mark.gpu
 
 from tolerances import TOL  # noqa: E402
+from golden_io import load_golden  # noqa: E402
 
 
 def rel(a, b):
@@ -28,7 +29,7 @@ def setup():
     from cldm.model import create_model
     from ctrlora_b200.train import PretrainTrainer
     from oracle import synth
-    g = torch.load(os.path.join(GOLD, "tiny_variants_golden.pt"), weights_only=False)
+    g = load_golden(os.path.join(GOLD, "tiny_variants_golden.pt"))
     model = create_model(os.path.join(GOLD, "tiny_pretrain.yaml"), init_weights=False)
     model.control_model.load_state_dict(synth.synth_state_dict(g["pretrain_control_shapes"], g["seed"], "control_model."))
     model.model.diffusion_model.load_state_dict(synth.synth_state_dict(g["unet_shapes"], g["seed"], "model.diffusion_model."))

@@ -13,6 +13,7 @@ GOLD = os.path.join(ROOT, "tests", "golden")
 pytestmark = pytest.mark.gpu
 
 from tolerances import TOL  # noqa: E402
+from golden_io import load_golden  # noqa: E402
 
 
 def rel(a, b):
@@ -134,7 +135,7 @@ def test_sd15_training_step_vs_reference_golden():
     from cldm.model import create_model
     from ctrlora_b200.train import FinetuneTrainer
     from oracle import synth
-    g = torch.load(os.path.join(GOLD, "sd15_rank128_train_golden.pt"), weights_only=False)
+    g = load_golden(os.path.join(GOLD, "sd15_rank128_train_golden.pt"))
     gs = torch.load(os.path.join(GOLD, "sd15_rank128_golden.pt"), weights_only=False)
     model = create_model(os.path.join(ROOT, "configs", "ctrlora_finetune_sd15_rank128.yaml"), init_weights=False)
     model.control_model.load_state_dict(synth.synth_state_dict(gs["control_shapes"], g["seed"], "control_model."))

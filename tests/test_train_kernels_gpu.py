@@ -20,7 +20,7 @@ def _rand(*shape, s=1.0):
 @pytest.mark.parametrize("M,P,Q", [(4096, 320, 128), (1000, 128, 320), (16384, 1280, 128), (300, 64, 64), (2048, 640, 640),
                                    (8192, 128, 2560), (77 * 4, 8, 768)])
 def test_wgrad_tn(M, P, Q):
-    """dW = A^T B over the token dim (LoRA up/down grads, zero-conv grads): MN-major UMMA operands."""
+    """dW = A^T B over the token dim (LoRA up/down grads, zero-conv grads): MN-major wgmma operands."""
     from ctrlora_b200 import ops
     torch.manual_seed(0)
     a, b = _rand(M, P), _rand(M, Q, s=M ** -0.5)
@@ -142,7 +142,7 @@ def test_mse_loss_and_adamw():
 
 @pytest.mark.parametrize("B,H,Nq,Nk,d", [(2, 8, 512, 512, 40), (1, 8, 1024, 1024, 80), (2, 8, 256, 256, 160), (2, 8, 256, 77, 40),
                                          (2, 4, 200, 300, 16), (1, 8, 64, 64, 160), (2, 8, 1024, 77, 80), (1, 4, 130, 129, 32),
-                                         (1, 8, 600, 700, 40), (1, 2, 520, 1000, 24), (1, 2, 640, 576, 48)])  # all-TMEM kernels, ragged
+                                         (1, 8, 600, 700, 40), (1, 2, 520, 1000, 24), (1, 2, 640, 576, 48)])  # ragged
 def test_attention_backward(B, H, Nq, Nk, d):
     """dQ, dK, dV of the fused attention against torch autograd on the same fp16-rounded inputs."""
     from ctrlora_b200 import ops

@@ -1,5 +1,5 @@
 """First-stage VAE parity (SURVEY.md §8 rows f1 / f3): the drop-in AutoencoderKL (encoder, decoder, posterior) on the
-sm_100a kernels against outputs of the unmodified reference (ldm/models/autoencoder.py:82-91,
+sm_90a kernels against outputs of the unmodified reference (ldm/models/autoencoder.py:82-91,
 ldm/modules/diffusionmodules/model.py:452-654; fixtures from `tools/make_golden.py --vae / --vae-full`)."""
 import os
 import sys

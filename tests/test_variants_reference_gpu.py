@@ -21,6 +21,7 @@ GOLD = os.path.join(ROOT, "tests", "golden")
 pytestmark = pytest.mark.gpu
 
 from tolerances import TOL  # noqa: E402
+from golden_io import load_golden  # noqa: E402
 
 
 def rel(got, ref):
@@ -30,7 +31,7 @@ def rel(got, ref):
 
 @pytest.fixture(scope="module")
 def g():
-    return torch.load(os.path.join(GOLD, "tiny_variants_golden.pt"), weights_only=False)
+    return load_golden(os.path.join(GOLD, "tiny_variants_golden.pt"))
 
 
 def build(kind, g, control_shapes):

@@ -18,6 +18,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from oracle import synth  # noqa: E402
 from tools import ref_shims  # noqa: E402
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+from golden_io import save_golden  # noqa: E402
 
 GOLD = os.path.join(ROOT, "tests", "golden")
 
@@ -143,7 +145,7 @@ def tiny(seed=0):
     g["lora"] = {"shapes": {k: tuple(v.shape) for k, v in lsd.items()}, "y": y_unfused, "w_fused_0.7": w_fused,
                  "y_fused_0.7": y_fused, "w_unfused": w_unfused}
     out = os.path.join(GOLD, "tiny_finetune_golden.pt")
-    torch.save(g, out)
+    save_golden(g, out)
     print("wrote", out, os.path.getsize(out) // 1024, "KiB")
 
 
@@ -177,7 +179,7 @@ def full(seed=0):
         g["control_0_slice"] = control[0][:, :8].clone()
         g["eps"] = unet(x=x, timesteps=t, context=ctx, control=[c.clone() for c in control], only_mid_control=False)
     out = os.path.join(GOLD, "sd15_rank128_golden.pt")
-    torch.save(g, out)
+    save_golden(g, out)
     print("wrote", out, os.path.getsize(out) // 1024, "KiB", "in", time.time() - t0, "s")
 
 
@@ -306,7 +308,7 @@ def variants(seed=0):
     g["midonly_train"] = {"loss": loss.detach().clone(), "eps": eps.detach().clone(),
                           "grad_norms": {n: (gr[n].grad.norm().item() if gr[n].grad is not None else 0.0) for n in names}}
     out = os.path.join(GOLD, "tiny_variants_golden.pt")
-    torch.save(g, out)
+    save_golden(g, out)
     print("wrote", out, os.path.getsize(out) // 1024, "KiB")
 
 
@@ -355,7 +357,7 @@ def full_train(seed=0):
                                                "time_embed.0.lora_layer.up"))]
     g["grads"] = {n: grads[n].grad.clone() for n in keep}
     out = os.path.join(GOLD, "sd15_rank128_train_golden.pt")
-    torch.save(g, out)
+    save_golden(g, out)
     print("wrote", out, os.path.getsize(out) // 1024, "KiB", "in", time.time() - t0, "s")
 
 
@@ -405,7 +407,7 @@ def vae(seed=0, full=False):
         with torch.no_grad():
             g["roundtrip"] = m.decode(post.mode()).clone()
     out = os.path.join(GOLD, "sd_vae_golden.pt" if full else "tiny_vae_golden.pt")
-    torch.save(g, out)
+    save_golden(g, out)
     print("wrote", out, os.path.getsize(out) // 1024, "KiB")
 
 
@@ -439,7 +441,7 @@ def ranks(seed=0):
                          "grad_norms": {n: gr[n].grad.norm().item() for n in names}}
         g["unet_shapes"] = shapes_of(model.model.diffusion_model)
     out = os.path.join(GOLD, "tiny_ranks_golden.pt")
-    torch.save(g, out)
+    save_golden(g, out)
     print("wrote", out, os.path.getsize(out) // 1024, "KiB")
 
 
@@ -528,7 +530,7 @@ def style(seed=0):
         g["eps_no_ip"] = model.apply_model(x, t, [{"c_crossattn": [ctx], "c_concat": [hint]}])
         g["eps_no_hint"] = model.apply_model(x, t, [{"c_crossattn": [ctx], "c_concat": [None], "c_ip": [ip]}])
     out = os.path.join(GOLD, "tiny_style_golden.pt")
-    torch.save(g, out)
+    save_golden(g, out)
     print("wrote", out, os.path.getsize(out) // 1024, "KiB")
 
 

@@ -1,14 +1,14 @@
 """Error-vs-cost curve for closing the fp16 parity gap with a selective two-term (hi + lo) operand split.
 
-Input: profiles/r2_precision_attribution.json (tools/precision_attribution.py: err_g = end-to-end error when ONLY block g
+Input: precision_attribution.json (tools/precision_attribution.py: err_g = end-to-end error when ONLY block g
 rounds to fp16; the squares add up to the measured end-to-end error^2 within 13 %).  A block whose GEMM operands are split
-(A_hi W_hi + A_lo W_hi + A_hi W_lo, three tcgen05 passes instead of one) stops contributing its operand-rounding error;
+(A_hi W_hi + A_lo W_hi + A_hi W_lo, three GEMM passes instead of one) stops contributing its operand-rounding error;
 its cost is 2 extra passes over its GEMM flops at the measured GEMM-family rate of the bench line.  Blocks are taken in
 order of error^2 removed per extra flop.  (Attention-internal roundings inside a block are not removed by the split, so
 the curve is optimistic by the attention share of each block.)
 """
 import json, sys
-src = sys.argv[1] if len(sys.argv) > 1 else "profiles/r2_precision_attribution.json"
+src = sys.argv[1] if len(sys.argv) > 1 else "precision_attribution.json"
 rate_tflops = float(sys.argv[2]) if len(sys.argv) > 2 else 829.0    # measured GEMM-family TFLOP/s of the DDIM step
 passes_per_step = 8                                                  # batch 4 x (cond, uncond)
 step_ms = 15.36
@@ -31,4 +31,4 @@ for i, gname in enumerate(items, 1):
 first = next(r for r in rows if r["err"] <= 1.0e-3)
 print("first point at or below 1e-3:", first)
 json.dump({"source": src, "gemm_rate_tflops": rate_tflops, "baseline_err": d["all"], "curve": rows, "first_below_1e-3": first},
-          open("profiles/r2_precision_curve.json", "w"), indent=1)
+          open("precision_curve.json", "w"), indent=1)

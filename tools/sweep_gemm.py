@@ -7,7 +7,24 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from ctrlora_b200 import ops  # noqa: E402
-from tools.profile_kernels import rnd, timeit  # noqa: E402
+
+
+def rnd(*s, scale=1.0):
+    return (torch.randn(*s, device="cuda") * scale).half()
+
+
+def timeit(fn, n=10):
+    """Mean seconds per call over n calls after 3 warm-up calls (CUDA events)."""
+    for _ in range(3):
+        fn()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(n):
+        fn()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / n * 1e-3
+
 
 import os as _os
 SHAPES_SMALL = [(8, 8, 8, 1280, 1280, 3), (8, 8, 8, 2560, 1280, 3), (8, 8, 8, 1280, 1280, 1), (8, 16, 16, 1280, 1280, 3), (8, 16, 16, 1280, 1280, 1)]
@@ -25,9 +42,7 @@ if __name__ == "__main__":
         print(f"--- {ks}x{ks} {h}x{w} {c}->{n} (M={b * h * w}), {fl / 1e9:.0f} GF")
         auto = timeit(lambda: ops.gemm(a, wt, ksize=ks, bias=bias, residual=res, out=out))
         print(f"  auto: {auto * 1e3:7.1f} us {fl / auto / 1e9:6.0f} TF/s")
-        for bn in (256, 160, 128, 80, 64, 48, 32):
-            if n % bn and bn not in (48,):
-                continue
+        for bn in (128, 64, 32):  # the wgmma tile widths of ctrlora_gemm_f16
             row = []
             for s in (1, 2, 4, 6, 8, 12):
                 try:
