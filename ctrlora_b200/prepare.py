@@ -4,6 +4,8 @@ re-derived whenever a source parameter changes (torch's `_version` counter / a n
 The fp32 nn.Parameters keep the reference's names and shapes, so `load_state_dict(strict=True)`, the optimizer
 filters and the checkpoint tooling (SURVEY.md §5) see the reference's state dict; these copies are derived data.
 """
+import contextlib
+
 import torch
 
 from . import ops
@@ -35,6 +37,24 @@ def _ver(*params):
                  if p is not None else None for p in params)
 
 
+# While a list is installed here, every PrepCache.get appends (cache, key, params, builder) to it: a trainer that
+# accumulates gradients records which weight copies a micro-batch reads, so it can rebuild them in a graph of their own.
+# A builder re-run that way must read its inputs from parameters or through other get() calls, never from a tensor it
+# closed over, or it would rebuild from stale data.
+RECORD = None
+
+
+@contextlib.contextmanager
+def record_builds():
+    global RECORD
+    log, prev = [], RECORD
+    RECORD = log
+    try:
+        yield log
+    finally:
+        RECORD = prev
+
+
 class PrepCache:
     """`get(key, params, builder)` returns builder() and re-runs it only when one of `params` changed."""
 
@@ -42,6 +62,8 @@ class PrepCache:
         self._store = {}
 
     def get(self, key, params, builder):
+        if RECORD is not None:
+            RECORD.append((self, key, params, builder))
         ver = _ver(*params)
         hit = self._store.get(key)
         if hit is not None and hit[0] == ver:

@@ -14,7 +14,13 @@ reaches (385 M ControlNet + UNet decoder weights it never uses).  Here only what
 The reference's activation checkpointing (util.py:102-151) is replaced by simply keeping the activations (they fit the 80 GB of an H100).
 The M = batch time-embedding MLP (time_embed, emb_layers: 12 tiny LoRA linears) is differentiated with torch fp32
 matmuls on [B, 1280] tensors -- negligible work, documented in DESIGN.md.
+
+Gradient accumulation (the train scripts' --gradacc, Lightning's accumulate_grad_batches = k): step() takes one
+micro-batch; k calls form a window whose gradients add into the flat buffer and are exchanged once, by the last
+micro-batch, before one AdamW step with grad_scale 1 / (world * loss scale * k).  flush() applies a partial window.
 """
+import numbers
+
 import torch
 import torch.nn as nn
 
@@ -419,8 +425,10 @@ def down_bwd(ds, s, d_out, G=None):
     b, h, w, c = s["shape"]
     if G is not None:
         dense_conv_grads(ds.op, None, pixel_major(d_out), G, col=s["col"])
-    wk = _cache(ds).get("w", [ds.op.weight], lambda: prepare.conv_weight(ds.op.weight).view(ds.out_channels, 1, 9 * c))
-    wt = _cache(ds).get("wT", [ds.op.weight], lambda: prepare.weight_T(wk))
+    # builders read their inputs through the caches (never a tensor fetched earlier): a recorded builder re-run inside a
+    # preparation graph (FinetuneTrainer._capture_window) must derive from the current parameters
+    wk = lambda: _cache(ds).get("w", [ds.op.weight], lambda: prepare.conv_weight(ds.op.weight).view(ds.out_channels, 1, 9 * c))
+    wt = _cache(ds).get("wT", [ds.op.weight], lambda: prepare.weight_T(wk()))
     d_col = ops.gemm(pixel_major(d_out), wt)  # [B, h/2, w/2, 9*C]
     return nchw_view(ops.im2col_s2_bwd(d_col, h, w))
 
@@ -675,7 +683,8 @@ class FinetuneTrainer:
     """One data-parallel CtrLoRA finetune step per call (configs ctrlora_finetune_sd15_rank*.yaml)."""
 
     def __init__(self, model, lr=1e-5, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.01, process_group=None,
-                 loss_scale=None, dynamic_loss_scale=True):
+                 loss_scale=None, dynamic_loss_scale=True, accumulate_grad_batches=1):
+        self._init_window(accumulate_grad_batches)
         self.model = model
         self.cn = model.control_model
         self.unet = model.model.diffusion_model
@@ -691,6 +700,7 @@ class FinetuneTrainer:
             torch.distributed.broadcast(self.G.flat_p, src=0, group=process_group)
             prepare.bump_train_version()
         self.step_count = 0
+        self.seg_steps = {}        # per-segment AdamW step counts
         # Loss scaling (the backward's activation gradients are fp16; the reference trains in fp32 and needs none):
         # d(loss)/d(eps) = 2 (eps - noise) / numel is ~1e-5 at batch 16 x 4 x 64 x 64 -- below fp16's normal range.  The
         # default scale makes it (eps - noise) / LOSS_SCALE_DIV independent of the batch shape; the AdamW kernel divides
@@ -704,6 +714,16 @@ class FinetuneTrainer:
 
     LOSS_SCALE_DIV = 8.0
     CHECK_OVERFLOW_EVERY = 16   # host polls the device-side skipped-steps counter this often (no per-step sync)
+
+    def _init_window(self, k):
+        """Gradient accumulation (Lightning's accumulate_grad_batches): k consecutive step() calls form one window, one
+        optimizer step.  micro_step = micro-batches already in the current window."""
+        if isinstance(k, bool) or not isinstance(k, numbers.Integral) or k < 1:
+            raise ValueError(f"accumulate_grad_batches must be an integer >= 1, got {k!r}")
+        self.accumulate_grad_batches = int(k)
+        self.micro_step = 0
+        self._window_tasks = []
+        self._accum = None         # graphs of the accumulating path (capture with k > 1)
 
     def _init_step_state(self, dev):
         """AdamW's step counter lives on the device (ops.adamw_begin): a step skipped for a non-finite gradient does not
@@ -737,12 +757,15 @@ class FinetuneTrainer:
     def _scale_for(self, numel):
         return float(self.loss_scale) if self.loss_scale is not None else numel / (2.0 * self.LOSS_SCALE_DIV)
 
-    def loss_and_grads(self, x0, hint_latent, context, t, noise):
-        """q_sample -> apply_model -> MSE -> backward into the flat gradient buffer.  Returns the loss (fp32 tensor)."""
+    def loss_and_grads(self, x0, hint_latent, context, t, noise, accumulate=False):
+        """q_sample -> apply_model -> MSE -> backward into the flat gradient buffer.  Returns the loss (fp32 tensor).
+        accumulate: add to the gradients already in the buffer (a continuing micro-batch of a window) and keep the window's
+        loss scale and overflow flag; otherwise the buffer and the flag are zeroed first."""
         m = self.model
-        self.G.zero()
-        self.overflow_flag.zero_()
-        self._scale_used = self._scale_for(x0.numel())
+        if not accumulate:
+            self.G.zero()
+            self.overflow_flag.zero_()
+            self._scale_used = self._scale_for(x0.numel())
         ops.stats_arena_begin(x0.device)  # one memset for all GroupNorm forward / backward statistics of the step
         try:
             x_noisy = m.q_sample(x_start=x0, t=t, noise=noise)
@@ -855,8 +878,11 @@ class FinetuneTrainer:
     # -- CUDA-graph replay of forward + backward (≈3 000 launches per step; Python cannot enqueue them fast enough)
     def capture(self, x0, hint_latent, context, t, noise, warmup=2):
         """Capture loss_and_grads for these shapes.  The LoRA folds / transposes of the trainable parameters are part
-        of the graph (they must re-run every step), the frozen-weight copies are built during warm-up and are not."""
+        of the graph (they must re-run every step), the frozen-weight copies are built during warm-up and are not.
+        With accumulate_grad_batches > 1 the graphs of the accumulating path are captured instead (_capture_window)."""
         self._static = [v.clone() for v in (x0, hint_latent, context, t, noise)]
+        if self.accumulate_grad_batches > 1:
+            return self._capture_window([None], warmup)
         cur = torch.cuda.current_stream()
         side = torch.cuda.Stream()
         side.wait_stream(cur)
@@ -916,6 +942,10 @@ class FinetuneTrainer:
         return self._static_loss
 
     def step(self, x0, hint_latent, context, t, noise):
+        """One micro-batch; every accumulate_grad_batches-th call also exchanges the gradients and runs AdamW.  Returns
+        this micro-batch's loss (its own mean, not divided by k)."""
+        if self.accumulate_grad_batches > 1:
+            return self._micro_batch((x0, hint_latent, context, t, noise), None)
         overlapped = False
         if getattr(self, "_graph", None) is not None:
             loss = self.loss_and_grads_graphed(x0, hint_latent, context, t, noise)
@@ -935,24 +965,241 @@ class FinetuneTrainer:
             torch.cuda.current_stream().wait_stream(self._comm)  # every bucket reduced before the overflow check / AdamW
         else:
             self.reduce_gradients()
-        ops.nonfinite_flag(self.G.flat_g, self.overflow_flag)  # after the all-reduce: every rank takes the same decision
-        step_dev, bc = self._seg_state("all")
-        ops.adamw_begin(step_dev, self.overflow_flag, self.betas, bc, self._skipped_dev)
-        ops.adamw_step(self.G.flat_p, self.G.flat_g, self.G.exp_avg, self.G.exp_avg_sq, 0, lr=self.lr,
-                       betas=self.betas, eps=self.eps, weight_decay=self.wd,
-                       grad_scale=1.0 / (self.world * self._scale_used), skip_flag=self.overflow_flag, bc_dev=bc)
+        self._update(self.window_segments([None]))
+        return loss
+
+    def _update(self, segs):
+        """Overflow check and AdamW over the exchanged gradients of the segments `segs` ([(offset, numel, key)]): the end
+        of a window.  The window's 1/k enters AdamW's grad_scale, not the fp16 loss gradient."""
+        G = self.G
+        for off, n, _ in segs:
+            ops.nonfinite_flag(G.flat_g[off:off + n], self.overflow_flag)  # after the all-reduce: every rank decides the same
+        for i, (off, n, key) in enumerate(segs):
+            step_dev, bc = self._seg_state(key)
+            ops.adamw_begin(step_dev, self.overflow_flag, self.betas, bc, self._skipped_dev if i == 0 else None)
+            ops.adamw_step(G.flat_p[off:off + n], G.flat_g[off:off + n], G.exp_avg[off:off + n], G.exp_avg_sq[off:off + n], 0,
+                           lr=self.lr, betas=self.betas, eps=self.eps, weight_decay=self.wd,
+                           grad_scale=1.0 / (self.world * self._scale_used * self.accumulate_grad_batches),
+                           skip_flag=self.overflow_flag, bc_dev=bc)
+            self.seg_steps[key] = self.seg_steps.get(key, 0) + 1
         prepare.bump_train_version()
         self.step_count += 1
+        self.micro_step = 0
         if self._poll_overflow():
-            # GradScaler semantics: the updates were skipped on the device; the scale is halved (re-capturing the graph, whose
-            # loss kernel has the scale baked in)
-            self.step_count = int(step_dev.item())
-            if getattr(self, "_graph", None) is not None:
-                self.capture(*self._static, warmup=1)
-        return loss
+            # GradScaler semantics: the updates were skipped on the device; the scale is halved (re-capturing the graphs,
+            # whose loss kernel has the scale baked in)
+            self.seg_steps = {k: int(v.item()) for k, v in self._step_dev.items()}
+            self.step_count = self.seg_steps[segs[0][2]]
+            self._recapture()
+
+    def _recapture(self):
+        if getattr(self, "_graph", None) is not None or self._accum is not None:
+            self.capture(*self._static, warmup=1)
 
     def _overflowed(self):
         return bool(self.overflow_flag.item())
+
+    # -- gradient accumulation (accumulate_grad_batches = k > 1) ------------------------------------------------------
+    # A window of k micro-batches: the first zeroes the gradient buffer (and the overflow flag) and fixes the loss scale;
+    # every micro-batch's backward adds into the buffer (every gradient write of the backward accumulates); the trainable
+    # weight copies (LoRA folds, fp16 / transposed / dgrad copies) are built once per window: the caches are keyed on the
+    # train version, which moves only when AdamW runs.  Only the last micro-batch exchanges the gradients.
+    def window_segments(self, tasks):
+        """[(offset, numel, key)] a window's update touches, given this rank's micro-batch tasks: the whole buffer."""
+        return [(0, self.G.numel, "all")]
+
+    def begin_micro_batch(self, task=None):
+        """Window bookkeeping of one micro-batch, host only: records its task, and when it is the window's last one
+        returns the window's segments (window_segments, which exchanges the used tasks across ranks).  Returns
+        (window_start, first_use_of_task, segments or None)."""
+        start = self.micro_step == 0
+        if start:
+            self._window_tasks = []
+        first_use = task not in self._window_tasks
+        self._window_tasks.append(task)
+        self.micro_step += 1
+        final = self.micro_step == self.accumulate_grad_batches
+        return start, first_use, (self.window_segments(self._window_tasks) if final else None)
+
+    def _run(self, args, task, accumulate):
+        return self.loss_and_grads(*args, accumulate=accumulate)
+
+    def _window_plan(self, segs, bucket_ranges):
+        """ranges to all-reduce after each backward bucket of the window's last micro-batch"""
+        return bucket_ranges
+
+    def _reduce_window(self, segs):
+        self.reduce_gradients([(off, n) for off, n, _ in segs])
+
+    def _segmented(self):
+        """capture the accumulating path's compute graph as one graph per gradient bucket (overlapped exchange)"""
+        return self.world > 1 and self._overlap()
+
+    def _after_cut(self):
+        """hook while capturing the segment that follows a bucket cut"""
+
+    def _micro_batch(self, args, task):
+        start, first_use, segs = self.begin_micro_batch(task)
+        final = segs is not None
+        overlapped = False
+        if self._accum is not None:
+            for dst, src in zip(self._static, args):
+                if dst.data_ptr() != src.data_ptr():
+                    dst.copy_(src, non_blocking=True)
+            if task is not None:
+                self.cn.switch_lora(task)  # host-side pointers follow the graphs
+                self.task = task
+            prep, compute = self._accum["prep"], self._accum["compute"]
+            if task not in compute:
+                raise KeyError(f"no graph captured for task {task!r}: pass it to capture()")
+            if start:
+                prep[None].replay()       # zero the buffer and the overflow flag, rebuild the task-independent copies
+            if first_use and task is not None and task in prep:
+                prep[task].replay()       # the task's LoRA folds, once per window
+            g, static_loss, self._scale_used = compute[task]
+            if isinstance(g, list):
+                plan = self._window_plan(segs, [r for _, r in g]) if final else [None] * len(g)
+                for (graph, _), ranges in zip(g, plan):
+                    graph.replay()
+                    if final:
+                        self._reduce_ranges(ranges)
+                overlapped = final and self.world > 1
+            else:
+                g.replay()
+            loss = static_loss.clone()    # the next micro-batch's graphs may reuse the captured loss's memory
+        elif final and self.world > 1 and self._overlap():
+            merged = self.merged_buckets()
+            plan = dict(zip([st for st, _ in merged], self._window_plan(segs, [r for _, r in merged])))
+            self._on_stage = lambda name: self._reduce_ranges(plan.get(name))
+            try:
+                loss = self._run(args, task, not start)
+            finally:
+                self._on_stage = None
+            self._reduce_ranges(plan["final"])
+            overlapped = True
+        else:
+            loss = self._run(args, task, not start)
+        if final:
+            if overlapped:
+                torch.cuda.current_stream().wait_stream(self._comm)
+            else:
+                self._reduce_window(segs)
+            self._update(segs)
+        return loss
+
+    def flush(self):
+        """Apply a partial window (fewer than k micro-batches, e.g. at the end of an epoch) with the same 1/k factor, as
+        Lightning does on an epoch's last batch.  Nothing happens on an empty window."""
+        if self.micro_step == 0:
+            return
+        segs = self.window_segments(self._window_tasks)
+        self._reduce_window(segs)
+        self._update(segs)
+
+    def _capture_window(self, tasks, warmup):
+        """CUDA graphs of the accumulating path, for the shapes of self._static:
+          * prep[None]: zero the gradient buffer and the overflow flag, rebuild every trainable-weight copy that does not
+            depend on a task's LoRA set -- replayed at a window's start;
+          * prep[task] (pretraining): rebuild the copies that depend on the task's LoRA set -- replayed on the task's first
+            micro-batch in a window (a window mixes tasks, so not every fold can be built at its start);
+          * compute[task]: forward + backward adding into the buffer, reading the copies above (one graph, or one per
+            gradient bucket when the exchange overlaps the backward).
+        Which copies a micro-batch reads is recorded from an eager run.  Each prep graph has a memory pool of its own, so
+        no other graph's scratch can overwrite the copies it keeps; the compute graphs share one pool (one is in flight)."""
+        static = self._static
+        cur = torch.cuda.current_stream()
+        side = torch.cuda.Stream()
+        side.wait_stream(cur)
+        logs = {}
+        with torch.cuda.stream(side):
+            for task in tasks:
+                for _ in range(warmup - 1):
+                    self._run(static, task, False)
+                prepare.bump_train_version()
+                with prepare.record_builds() as log:
+                    self._run(static, task, False)
+                logs[task] = log
+        cur.wait_stream(side)
+        torch.cuda.synchronize()
+        builds, seen = {None: []}, set()
+        for task in tasks:
+            own = self._task_param_ids(task)
+            builds.setdefault(task, [])
+            for entry in logs[task]:
+                cache, key, params, _ = entry
+                ps = [p for p in params if p is not None]
+                if not any(getattr(p, "_ctrlora_trainable", False) for p in ps):
+                    continue  # frozen copies are built once and never change
+                owner = task if any(id(p) in own for p in ps) else None
+                if (owner, id(cache), key) not in seen:
+                    seen.add((owner, id(cache), key))
+                    builds[owner].append(entry)
+
+        def rebuild(entries):
+            for cache, key, params, builder in entries:
+                cache.get(key, params, builder)
+
+        prepare.bump_train_version()  # every recorded copy is rebuilt inside its prep graph
+        prep, compute, pool = {}, {}, None
+        for owner, entries in builds.items():
+            if owner is not None and not entries:
+                continue
+            if owner is not None:
+                self.cn.switch_lora(owner)
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                if owner is None:
+                    self.G.zero()
+                    self.overflow_flag.zero_()
+                rebuild(entries)
+            prep[owner] = g
+        for task in tasks:
+            g, loss, pool = self._capture_compute(lambda: self._run(static, task, True), pool)
+            compute[task] = (g, loss, self._scale_used)
+        self._accum = {"prep": prep, "compute": compute}
+        return self
+
+    def _task_param_ids(self, task):
+        return set()
+
+    def _capture_compute(self, run, pool):
+        """graph of run() (one continuing micro-batch) in `pool`; one graph per gradient bucket when _segmented()"""
+        kw = {} if pool is None else {"pool": pool}
+        if not self._segmented():
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, **kw):
+                loss = run()
+            return g, loss, g.pool() if pool is None else pool
+        buckets = dict(self.merged_buckets())
+        cur = torch.cuda.current_stream()
+        segs, state = [], {"pool": pool}
+        stream = torch.cuda.Stream()
+        stream.wait_stream(cur)
+        with torch.cuda.stream(stream):
+            state["g"] = torch.cuda.CUDAGraph()
+            state["g"].capture_begin(**kw)
+
+            def on_stage(name):
+                if name not in buckets:
+                    return
+                state["g"].capture_end()
+                state["pool"] = state["pool"] or state["g"].pool()
+                segs.append((state["g"], buckets[name]))
+                self._after_cut()
+                state["g"] = torch.cuda.CUDAGraph()
+                state["g"].capture_begin(pool=state["pool"])
+
+            self._on_stage = on_stage
+            try:
+                loss = run()
+            finally:
+                self._on_stage = None
+                ops.set_sm_limit(0)
+            state["g"].capture_end()
+            state["pool"] = state["pool"] or state["g"].pool()
+            segs.append((state["g"], buckets["final"]))
+        cur.wait_stream(stream)
+        return segs, loss, state["pool"]
 
 
 
@@ -989,7 +1236,8 @@ class PretrainTrainer(FinetuneTrainer):
     ControlNetFinetune(ft_with_lora=False) (full-parameter finetuning, cldm_ctrlora_finetune.py:101-104)."""
 
     def __init__(self, model, lr=1e-5, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.01, process_group=None,
-                 loss_scale=None, dynamic_loss_scale=True):
+                 loss_scale=None, dynamic_loss_scale=True, accumulate_grad_batches=1):
+        self._init_window(accumulate_grad_batches)
         self.model = model
         self.cn = model.control_model
         self.unet = model.model.diffusion_model
@@ -1022,11 +1270,14 @@ class PretrainTrainer(FinetuneTrainer):
         self._graphs, self._pool, self._static, self._static_loss = {}, None, None, {}
         self.task = self.tasks[0] if self.tasks else None
 
-    def loss_and_grads(self, x0, hint_latent, context, t, noise, task=None):
+    def loss_and_grads(self, x0, hint_latent, context, t, noise, task=None, accumulate=False):
         if task is not None and self.tasks:
             self.cn.switch_lora(task)
             self.task = task
-        return super().loss_and_grads(x0, hint_latent, context, t, noise)
+        return super().loss_and_grads(x0, hint_latent, context, t, noise, accumulate=accumulate)
+
+    def _run(self, args, task, accumulate):
+        return self.loss_and_grads(*args, task=task, accumulate=accumulate)
 
     # -- one CUDA graph per task (the attached LoRA set is baked into the captured kernels' pointers); the graphs share one
     # memory pool: only one of them is ever in flight
@@ -1055,6 +1306,8 @@ class PretrainTrainer(FinetuneTrainer):
     def capture(self, x0, hint_latent, context, t, noise, tasks=None, warmup=2):
         if self._static is None:
             self._static = [v.clone() for v in (x0, hint_latent, context, t, noise)]
+        if self.accumulate_grad_batches > 1:
+            return self._capture_window(list(tasks or self.tasks or [None]), warmup)
         overlap = self.world > 1 and bool(self._overlap_cuts())
         for task in (tasks or self.tasks or [None]):
             cur = torch.cuda.current_stream()
@@ -1126,6 +1379,36 @@ class PretrainTrainer(FinetuneTrainer):
     def segments_for(self, task):
         return active_segments(self.layout, self._tasks_on_ranks(task)) if self.tasks else [(0, self.G.numel, "base")]
 
+    def window_segments(self, tasks):
+        """Segments of a window whose micro-batches on this rank trained `tasks`: the ControlNet plus every LoRA set that
+        any rank used in any micro-batch of the window.  The ranks exchange their used-task masks once per window (one
+        all-reduce)."""
+        if not self.tasks:
+            return [(0, self.G.numel, "base")]
+        used = sorted({self.tasks.index(t) for t in tasks})
+        if self.world > 1:
+            mask = torch.zeros(len(self.tasks), device=self.G.flat_p.device, dtype=torch.int32)
+            mask[used] = 1
+            torch.distributed.all_reduce(mask, group=self.pg)
+            used = [i for i, v in enumerate(mask.tolist()) if v]
+        return active_segments(self.layout, [self.tasks[i] for i in used])
+
+    def _window_plan(self, segs, bucket_ranges):
+        return self.exchange_plan(segs, bucket_ranges)
+
+    def _reduce_window(self, segs):
+        self.reduce_gradients(segs)
+
+    def _segmented(self):
+        return self.world > 1 and bool(self._overlap_cuts())
+
+    def _after_cut(self):
+        ops.set_sm_limit(max(2, torch.cuda.get_device_properties(self.G.flat_p.device).multi_processor_count
+                             - self._sm_reserve()))
+
+    def _task_param_ids(self, task):
+        return {id(p) for n, p in zip(self.G.names, self.G.params) if n.startswith(f"loras_dict.{task}.")}
+
     def exchange_plan(self, segs, bucket_ranges):
         """Ranges to all-reduce after each backward bucket: the bucket's part of the ControlNet segment; the LoRA sets live
         behind it in the flat buffer and travel with the LAST bucket, and only the sets some rank trained this step (`segs`,
@@ -1147,6 +1430,8 @@ class PretrainTrainer(FinetuneTrainer):
 
     def step(self, x0, hint_latent, context, t, noise, task=None):
         task = task if task is not None else self.task
+        if self.accumulate_grad_batches > 1:
+            return self._micro_batch((x0, hint_latent, context, t, noise), task)
         segs = self.segments_for(task)  # (ranks exchange their task index first: known before the backward starts)
         overlapped = False
         if task in self._graphs:
@@ -1171,23 +1456,13 @@ class PretrainTrainer(FinetuneTrainer):
             torch.cuda.current_stream().wait_stream(self._comm)  # every bucket reduced before the overflow check / AdamW
         else:
             self.reduce_gradients(segs)
-        for off, n, _ in segs:
-            ops.nonfinite_flag(self.G.flat_g[off:off + n], self.overflow_flag)
-        G = self.G
-        for i, (off, n, key) in enumerate(segs):
-            step_dev, bc = self._seg_state(key)
-            ops.adamw_begin(step_dev, self.overflow_flag, self.betas, bc, self._skipped_dev if i == 0 else None)
-            ops.adamw_step(G.flat_p[off:off + n], G.flat_g[off:off + n], G.exp_avg[off:off + n], G.exp_avg_sq[off:off + n], 0,
-                           lr=self.lr, betas=self.betas, eps=self.eps, weight_decay=self.wd,
-                           grad_scale=1.0 / (self.world * self._scale_used), skip_flag=self.overflow_flag, bc_dev=bc)
-            self.seg_steps[key] = self.seg_steps.get(key, 0) + 1
-        prepare.bump_train_version()
-        self.step_count += 1
-        if self._poll_overflow():
-            self.seg_steps = {k: int(v.item()) for k, v in self._step_dev.items()}
-            self.step_count = self.seg_steps.get("base", self.step_count)
-            if self._graphs:
-                tasks = list(self._graphs)
-                self._graphs.clear()
-                self.capture(*self._static, tasks=tasks, warmup=1)
+        self._update(segs)
         return loss
+
+    def _recapture(self):
+        if self._accum is not None:
+            self.capture(*self._static, tasks=list(self._accum["compute"]), warmup=1)
+        elif self._graphs:
+            tasks = list(self._graphs)
+            self._graphs.clear()
+            self.capture(*self._static, tasks=tasks, warmup=1)

@@ -2,6 +2,7 @@
 
     python tools/make_golden.py            # tiny config (committed fixture, ~300 KB)
     python tools/make_golden.py --full     # SD1.5-size eps for one image (committed fixture, ~70 KB; takes minutes)
+    python tools/make_golden.py --accum    # gradient accumulation windows, finetune and pretrain (tiny config)
 
 The reference cannot travel to the GPU box; these fixtures can.  Weights/inputs are regenerated from names by
 oracle/synth.py, so the fixtures hold only key/shape lists and outputs.
@@ -534,8 +535,90 @@ def style(seed=0):
     print("wrote", out, os.path.getsize(out) // 1024, "KiB")
 
 
+ACCUM_FT_KEEP = ("zero_convs.0.", "middle_block_out", "input_blocks.1.1.norm",
+                 "input_blocks.1.1.transformer_blocks.0.attn1.to_q.lora_layer", "time_embed.0.lora_layer",
+                 "middle_block.1.transformer_blocks.0.ff.net.2.lora_layer", "input_blocks.4.0.emb_layers.1.lora_layer")
+ACCUM_PT_KEEP = ("input_blocks.0.0.weight", "input_blocks.1.0.in_layers.2.weight", "input_blocks.4.1.proj_in.weight",
+                 "input_blocks.4.1.transformer_blocks.0.attn1.to_q.weight", "middle_block.1.proj_out.weight",
+                 "time_embed.0.weight", "zero_convs.3.0.weight", "middle_block_out.0.bias",
+                 "loras_dict.canny.0.down.weight", "loras_dict.canny.5.up.weight",
+                 "loras_dict.depth.0.down.weight", "loras_dict.depth.5.up.weight")
+
+
+def accum(seed=0, lr=1e-3):
+    """Gradient accumulation as Lightning 1.5 runs it (accumulate_grad_batches = k), emulated explicitly with the
+    reference's modules: per micro-batch the p_losses arithmetic (ddpm.py:885-920), loss / k, .backward() (gradients add
+    into .grad), then ONE torch.optim.AdamW step, which skips parameters whose .grad is None.
+      finetune (tiny_finetune.yaml): 3 micro-batches of batch 2, the optimizer set of cldm_ctrlora_finetune.py:88-100;
+      pretrain (tiny_pretrain.yaml): a window with tasks [canny, depth, canny], switch_lora per micro-batch inside
+      apply_model (cldm_ctrlora_pretrain.py:104), AdamW over control_model.parameters() (:174-182)."""
+    B, H = 2, 16
+    ts = [[981, 21], [500, 250], [37, 760]]
+
+    def micro(i):
+        mk = lambda n, s: synth.synth_input(f"{n}_acc{i}", s, seed)
+        return dict(x=mk("x", (B, 4, H, H)), hint=mk("hint", (B, 4, H, H)), ctx=mk("ctx", (B, 77, 64)),
+                    noise=mk("noise", (B, 4, H, H)), t=torch.tensor(ts[i], dtype=torch.long))
+
+    def window(model, params, tasks):
+        k = len(tasks)
+        model.encode_first_stage = lambda h: h
+        model.get_first_stage_encoding = lambda h: h
+        for p in model.parameters():
+            p.grad = None
+        losses = []
+        for i, task in enumerate(tasks):
+            d = micro(i)
+            cond = {"c_crossattn": [d["ctx"]], "c_concat": [d["hint"]]}
+            if task is not None:
+                cond["task"] = task
+            x_noisy = model.q_sample(x_start=d["x"], t=d["t"], noise=d["noise"])
+            eps = model.apply_model(x_noisy, d["t"], cond)
+            loss = model.get_loss(eps, d["noise"], mean=False).mean([1, 2, 3]).mean()
+            (loss / k).backward()
+            losses.append(loss.detach().clone())
+        opt = torch.optim.AdamW(params, lr=lr)
+        return torch.stack(losses), opt
+
+    g = {"seed": seed, "B": B, "H": H, "t": torch.tensor(ts), "lr": lr}
+    # ---------------- finetune
+    model = build_reference(os.path.join(GOLD, "tiny_finetune.yaml"), seed)
+    cn = model.control_model
+    names = [n for n, _ in cn.named_parameters()
+             if "lora_layer" in n or "zero_convs" in n or "middle_block_out" in n or "norm" in n]
+    named = dict(cn.named_parameters())
+    params = [named[n] for n in names]
+    losses, opt = window(model, params, [None, None, None])
+    keep = [n for n in names if n.startswith(ACCUM_FT_KEEP)]
+    ft = {"control_shapes": shapes_of(cn), "unet_shapes": shapes_of(model.model.diffusion_model), "losses": losses,
+          "trainable_names": names, "grad_norms": {n: named[n].grad.norm().item() for n in names},
+          "grads": {n: named[n].grad.clone() for n in keep}, "before": {n: named[n].detach().clone() for n in keep}}
+    opt.step()
+    ft["after"] = {n: named[n].detach().clone() for n in keep}
+    g["finetune"] = ft
+    # ---------------- pretrain
+    model = build_reference(os.path.join(GOLD, "tiny_pretrain.yaml"), seed)
+    cn = model.control_model
+    named = [(n, p) for n, p in cn.named_parameters(remove_duplicate=False) if ".lora_layer." not in n]
+    by_name = dict(named)
+    tasks = ["canny", "depth", "canny"]
+    shapes = shapes_of(cn)  # before switch_lora attaches a set (its aliases would join the state dict)
+    losses, opt = window(model, list(cn.parameters()), tasks)
+    pt = {"control_shapes": shapes, "tasks": tasks, "losses": losses, "param_names": [n for n, _ in named],
+          "grad_norms": {n: (p.grad.norm().item() if p.grad is not None else None) for n, p in named},
+          "grads": {n: by_name[n].grad.clone() for n in ACCUM_PT_KEEP},
+          "before": {n: by_name[n].detach().clone() for n in ACCUM_PT_KEEP}}
+    opt.step()
+    pt["after"] = {n: by_name[n].detach().clone() for n in ACCUM_PT_KEEP}
+    g["pretrain"] = pt
+    out = os.path.join(GOLD, "tiny_accum_golden.pt")
+    save_golden(g, out)
+    print("wrote", out, os.path.getsize(out) // 1024, "KiB")
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
+    ap.add_argument("--accum", action="store_true")
     ap.add_argument("--full", action="store_true")
     ap.add_argument("--variants", action="store_true")
     ap.add_argument("--full-train", action="store_true")
@@ -562,5 +645,7 @@ if __name__ == "__main__":
         vae(full=True)
     elif a.style:
         style()
+    elif a.accum:
+        accum()
     else:
         tiny()
