@@ -3,9 +3,11 @@
 //   * every 1x1 / 3x3 stride-1 Conv2d in NHWC    (reference: ldm/modules/diffusionmodules/openaimodel.py:162-274)
 // D[M, N] = sum_taps A_shifted[M, Cin] * W[N, tap, Cin]^T  (+ optional second 1x1 operand pair: the ResBlock skip conv)
 // A tiles are TMA boxes over the (C, W, H, B) activation tensor: a filter tap is a coordinate shift and the conv zero
-// padding is the TMA out-of-bounds fill, so no im2col buffer exists in HBM.  One CTA owns one 128 x BN output tile: a
-// producer thread fills a ring of TMA stages, two consumer warpgroups (64 rows each) run wgmma with accumulators in
-// registers, then stage the fp32 tile in shared memory for a row-per-thread epilogue.
+// padding is the TMA out-of-bounds fill, so no im2col buffer exists in HBM.  The grid is persistent: each CTA walks a
+// static list of 128 x BN output tiles (BN up to 256), a producer thread fills a ring of TMA stages, and two consumer
+// warpgroups (64 rows each) run wgmma with accumulators in registers, then run a row-per-thread epilogue through a
+// staging buffer of their own while the producer already loads the next tile.  Tiles of a last, partial wave may be
+// split along K.
 #include "gemm_sm90.cuh"
 #include "wgmma.cuh"
 #include "ctrlora_b200.h"
@@ -19,69 +21,53 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
     return *reinterpret_cast<uint32_t*>(&h);
 }
 
-// One 32-column chunk of the epilogue for one accumulator row: bias, GEGLU, time-embedding row term, scale, residual,
-// then the store (row-major fp16 / fp32, or the transposed V^T layout).  v = value columns, g = gate columns (GEGLU).
-template <bool GEGLU>
-__device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, float* v, const float* g, int c, int bn_out, int n0,
-                                               bool row_ok, long long m, int img, int tok, const float* sb,
-                                               const uint4* rpre = nullptr) {
+// One CW-column chunk (CW = 16 or 32) of the epilogue for one output row, after bias (and GEGLU): time-embedding row
+// term, scale, residual, then the store (row-major fp16 / fp32, or the transposed V^T layout).
+template <int CW>
+__device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, float* v, int c, int bn_out, int n0, bool row_ok,
+                                               long long m, int img, int tok) {
     const int nbase = n0 + c;
-    const bool full_chunk = (c + 32 <= bn_out) && (nbase + 32 <= p.N);
-    // sb: this tile's bias staged in shared memory (zeros where there is no bias / beyond N): broadcast 16-byte reads
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-        const float4 b4 = lds128f(smem_u32(sb + c + 4 * q));
-        v[4 * q] += b4.x; v[4 * q + 1] += b4.y; v[4 * q + 2] += b4.z; v[4 * q + 3] += b4.w;
-    }
-    if (GEGLU) {
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-            const float4 b4 = lds128f(smem_u32(sb + 256 + c + 4 * q));
-            v[4 * q] *= gelu_erf_f(g[4 * q] + b4.x);
-            v[4 * q + 1] *= gelu_erf_f(g[4 * q + 1] + b4.y);
-            v[4 * q + 2] *= gelu_erf_f(g[4 * q + 2] + b4.z);
-            v[4 * q + 3] *= gelu_erf_f(g[4 * q + 3] + b4.w);
-        }
-    }
+    const bool full_chunk = (c + CW <= bn_out) && (nbase + CW <= p.N);
     if (!row_ok) return;
     if (p.rowbias) {
         const float* rb = p.rowbias + static_cast<long long>(img) * p.rowbias_ld + nbase;
         if (full_chunk && (p.rowbias_ld & 3) == 0) {
 #pragma unroll
-            for (int q = 0; q < 8; ++q) {
+            for (int q = 0; q < CW / 4; ++q) {
                 const float4 b4 = __ldg(reinterpret_cast<const float4*>(rb) + q);
                 v[4 * q] += b4.x; v[4 * q + 1] += b4.y; v[4 * q + 2] += b4.z; v[4 * q + 3] += b4.w;
             }
         } else {
 #pragma unroll
-            for (int j = 0; j < 32; ++j)
+            for (int j = 0; j < CW; ++j)
                 if (nbase + j < p.N) v[j] += __ldg(rb + j);
         }
     }
     if (p.out_scale != 1.0f) {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] *= p.out_scale;
+        for (int j = 0; j < CW; ++j) v[j] *= p.out_scale;
     }
     if (p.residual && p.residual_f32) {
         const float* rp = reinterpret_cast<const float*>(p.residual) + m * p.ldr + nbase;
         if (full_chunk && (p.ldr & 3) == 0) {  // LoRA folds: W (fp32 master) + s * up . down
 #pragma unroll
-            for (int q = 0; q < 8; ++q) {
+            for (int q = 0; q < CW / 4; ++q) {
                 const float4 r4 = __ldg(reinterpret_cast<const float4*>(rp) + q);
                 v[4 * q] += r4.x; v[4 * q + 1] += r4.y; v[4 * q + 2] += r4.z; v[4 * q + 3] += r4.w;
             }
         } else {
-            for (int j = 0; j < 32; ++j)
+#pragma unroll
+            for (int j = 0; j < CW; ++j)
                 if (c + j < bn_out && nbase + j < p.N) v[j] += rp[j];
         }
     } else if (p.residual) {
         const __half* rp = p.residual + m * p.ldr + nbase;
         if (full_chunk && (p.ldr & 7) == 0) {
-            uint4 u[4];
+            uint4 u[CW / 8];
 #pragma unroll
-            for (int q = 0; q < 4; ++q) u[q] = rpre ? rpre[q] : __ldg(reinterpret_cast<const uint4*>(rp) + q);
+            for (int q = 0; q < CW / 8; ++q) u[q] = __ldg(reinterpret_cast<const uint4*>(rp) + q);
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
+            for (int q = 0; q < CW / 8; ++q) {
                 const __half2* h = reinterpret_cast<const __half2*>(&u[q]);
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
@@ -91,7 +77,8 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, float* v, c
                 }
             }
         } else {
-            for (int j = 0; j < 32; ++j)
+#pragma unroll
+            for (int j = 0; j < CW; ++j)
                 if (c + j < bn_out && nbase + j < p.N) v[j] += __half2float(rp[j]);
         }
     }
@@ -99,28 +86,31 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, float* v, c
     if (p.seg_width > 0) { seg = nbase / p.seg_width; nloc = nbase - seg * p.seg_width; }
     if (p.transposed[seg]) {
         __half* o = reinterpret_cast<__half*>(p.out[seg]) + (static_cast<long long>(img) * p.seg_width + nloc) * p.tok_pad + tok;
-        for (int j = 0; j < 32; ++j)
+#pragma unroll
+        for (int j = 0; j < CW; ++j)
             if (c + j < bn_out && nbase + j < p.N) o[static_cast<long long>(j) * p.tok_pad] = __float2half_rn(v[j]);
         if (p.dup_out) {
             __half* o2 = p.dup_out + m * p.dup_ld + nloc;
-            for (int j = 0; j < 32; ++j)
+#pragma unroll
+            for (int j = 0; j < CW; ++j)
                 if (c + j < bn_out && nbase + j < p.N) o2[j] = __float2half_rn(v[j]);
         }
     } else if (p.out_f32) {
         float* o = reinterpret_cast<float*>(p.out[seg]) + m * p.ldc + nloc;
         if (full_chunk && (p.ldc & 3) == 0) {
 #pragma unroll
-            for (int q = 0; q < 8; ++q)
+            for (int q = 0; q < CW / 4; ++q)
                 reinterpret_cast<float4*>(o)[q] = make_float4(v[q * 4], v[q * 4 + 1], v[q * 4 + 2], v[q * 4 + 3]);
         } else {
-            for (int j = 0; j < 32; ++j)
+#pragma unroll
+            for (int j = 0; j < CW; ++j)
                 if (c + j < bn_out && nbase + j < p.N) o[j] = v[j];
         }
     } else {
         __half* o = reinterpret_cast<__half*>(p.out[seg]) + m * p.ldc + nloc;
         if (full_chunk && (p.ldc & 7) == 0) {
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
+            for (int q = 0; q < CW / 8; ++q) {
                 uint4 u;
                 u.x = pack_h2(v[q * 8 + 0], v[q * 8 + 1]);
                 u.y = pack_h2(v[q * 8 + 2], v[q * 8 + 3]);
@@ -129,25 +119,58 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, float* v, c
                 reinterpret_cast<uint4*>(o)[q] = u;
             }
         } else {
-            for (int j = 0; j < 32; ++j)
+#pragma unroll
+            for (int j = 0; j < CW; ++j)
                 if (c + j < bn_out && nbase + j < p.N) o[j] = __float2half_rn(v[j]);
         }
     }
 }
 
+// One work unit: an output tile (m tile, n tile) and its k-iteration range.  `slot` >= 0 marks a split tile: its
+// workspace slices and arrival counter.
+struct GemmUnit {
+    int mt, nt, it0, it1, ks, slot;
+};
+__device__ __forceinline__ GemmUnit gemm_unit(const GemmKParams& p, int u, int m_tiles, int k_iters) {
+    GemmUnit w;
+    int tile;
+    if (u < p.tiles_whole) {
+        tile = u;
+        w.ks = 0; w.slot = -1; w.it0 = 0; w.it1 = k_iters;
+    } else {
+        const int v = u - p.tiles_whole;
+        w.slot = v / p.splits;
+        w.ks = v - w.slot * p.splits;
+        tile = p.tiles_whole + w.slot;
+        w.it0 = w.ks * p.kiters_per_split;
+        w.it1 = min(k_iters, w.it0 + p.kiters_per_split);
+    }
+    w.mt = tile % m_tiles;  // M fastest: CTAs that run at the same time share the B (weight) tile
+    w.nt = tile / m_tiles;
+    return w;
+}
+
+// fp32 epilogue slab of one warpgroup: [64 rows][64 columns], 16-byte chunk j of row r stored at chunk j ^ (r & 7)
+__device__ __forceinline__ uint32_t epi_addr(uint32_t base, int r, int col) {
+    return base + static_cast<uint32_t>(r * (GEMM_EPI_COLS * 4) + ((((col >> 2) ^ (r & 7)) << 4) | ((col & 3) << 2)));
+}
+
+// Persistent: CTA b runs work units b, b + gridDim.x, ...  The producer thread walks the same sequence, so it fills
+// the ring for the next unit while the consumers run the epilogue of the current one; the ring position (stage,
+// phase) carries across units.  CTAs never wait on each other, so correctness does not depend on co-residency.
 template <bool GEGLU, int BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
                   const __grid_constant__ GemmKParams p) {
-    constexpr int LD = BN + 4;  // fp32 pitch of the staged tile (float4-aligned rows)
+    constexpr int BN_OUT = GEGLU ? BN / 2 : BN;
+    constexpr int NACC = BN / 2;  // fp32 accumulators per consumer thread (64 rows x BN per warpgroup)
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + GEMM_SMEM_DATA);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + GEMM_SMEM_DATA + GEMM_EPI_BYTES);
     uint64_t* full = bars;
     uint64_t* empty = bars + GEMM_MAX_STAGES;
     volatile int* last_flag = reinterpret_cast<volatile int*>(bars + 2 * GEMM_MAX_STAGES);
-    float* sb = reinterpret_cast<float*>(smem + GEMM_SMEM_DATA + 256);  // [value 256 | gate 256]
 
     pdl_launch_dependents();
     const int warp = uniform_warp_idx();
@@ -172,150 +195,168 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_b;
     const int main_iters = p.taps * p.kchunks;
     const int k_iters = main_iters + p.kchunks2;
-    const int bn_out = GEGLU ? (BN >> 1) : BN;
-    // tile -> (m tile, split, n tile); the k range of a split is [ks * kiters_per_split, ...)
-    const int mt = static_cast<int>(blockIdx.x) % m_tiles;
-    const int rest = static_cast<int>(blockIdx.x) / m_tiles;
-    const int ks = rest % p.splits, nt = rest / p.splits;
-    const int tw = mt % p.tiles_w, th = (mt / p.tiles_w) % p.tiles_h, tb = mt / (p.tiles_w * p.tiles_h);
-    const int n0 = nt * bn_out;
-    const int it0 = ks * p.kiters_per_split, it1 = min(k_iters, it0 + p.kiters_per_split);
-    const int nit = it1 - it0;
 
     if (warp < 4) {
         // ---------------------------------------------------- TMA producer: one thread of warpgroup 0
+        setmaxnreg_dec<GEMM_PRODUCER_REGS>();
         if (warp == 0 && elect_one()) {
-            const int w0 = tw * p.bw - p.pad, h0 = th * p.bh - p.pad, b0 = tb * p.nb;
             const uint32_t tx_bytes = GEMM_A_BYTES + BN * 128;
-            for (int j = 0; j < nit; ++j) {
-                const int it = it0 + j, s = j % nstages;
-                mbar_wait(&empty[s], ((j / nstages) & 1) ^ 1);
-                uint8_t* dst = smem + s * p.stage_bytes;
-                mbar_expect_tx(&full[s], tx_bytes);
-                if (it < main_iters) {
-                    const int tap = it / p.kchunks, kc = it - tap * p.kchunks, ky = tap / p.kw, kx = tap - ky * p.kw;
-                    tma_load_4d(dst, &tmA, &full[s], kc * GEMM_BK, w0 + kx, h0 + ky, b0);
-                    tma_load_3d(dst + GEMM_A_BYTES, &tmB, &full[s], kc * GEMM_BK, tap, n0);
-                    if (GEGLU) tma_load_3d(dst + GEMM_A_BYTES + bn_out * 128, &tmB, &full[s], kc * GEMM_BK, tap, p.N + n0);
-                } else {  // second operand pair (fused 1x1 skip convolution)
-                    const int c0 = (it - main_iters) * GEMM_BK;
-                    tma_load_4d(dst, &tmA2, &full[s], c0, w0 + p.pad, h0 + p.pad, b0);
-                    tma_load_3d(dst + GEMM_A_BYTES, &tmB2, &full[s], c0, 0, n0);
-                }
-            }
-        }
-        return;  // the consumers synchronise among themselves only (named barrier 1)
-    }
-
-    // -------------------------------------------------------- consumers: wgmma main loop, rows [64 wg, 64 wg + 64)
-    const int ct = threadIdx.x - 128;  // 0..255
-    const int wg = ct >> 7;
-    float acc[BN / 2];
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    const uint32_t smem0 = smem_u32(smem);
-    for (int j = 0; j < nit; ++j) {
-        const int s = j % nstages;
-        mbar_wait(&full[s], (j / nstages) & 1);
-        const uint32_t a_base = smem0 + s * p.stage_bytes + wg * 64 * 128;
-        const uint32_t b_base = smem0 + s * p.stage_bytes + GEMM_A_BYTES;
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < GEMM_BK / 16; ++k)
-            WgmmaSS<BN, 0, 0>::mma(acc, wgmma_desc_kmajor(a_base + 32 * k), wgmma_desc_kmajor(b_base + 32 * k), (j | k) ? 1u : 0u);
-        wgmma_commit();
-        wgmma_wait<1>();  // the previous stage's MMAs have finished reading it
-        if (j > 0) mbar_arrive(&empty[(j - 1) % nstages]);
-    }
-    wgmma_wait<0>();
-    wgmma_fence_regs<BN / 2>(acc);
-
-    // ---- stage the fp32 tile over the (now idle) operand ring, and this tile's bias
-    named_bar_sync(1, GEMM_CONSUMERS);  // both warpgroups are done reading the ring
-    float* stg = reinterpret_cast<float*>(smem);
-    {
-        const int r0 = wg * 64 + ((ct & 127) >> 5) * 16 + (lane >> 2), cq = 2 * (lane & 3);
-#pragma unroll
-        for (int i = 0; i < BN / 8; ++i) {
-            *reinterpret_cast<float2*>(stg + r0 * LD + 8 * i + cq) = make_float2(acc[4 * i], acc[4 * i + 1]);
-            *reinterpret_cast<float2*>(stg + (r0 + 8) * LD + 8 * i + cq) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
-        }
-        float bv = 0.f, bg = 0.f;
-        if (p.bias && ct < bn_out && n0 + ct < p.N) {
-            bv = __ldg(p.bias + n0 + ct);
-            if (GEGLU) bg = __ldg(p.bias + p.N + n0 + ct);
-        }
-        sb[ct] = bv;
-        sb[256 + ct] = bg;
-    }
-    named_bar_sync(1, GEMM_CONSUMERS);
-
-    // ---- epilogue: thread = row, the two threads of a row take alternate 32-column chunks
-    const int r = ct & 127, half = ct >> 7;
-    const int iw = r % p.bw, ih = (r / p.bw) % p.bh, ib = r / (p.bw * p.bh);
-    const int gw = tw * p.bw + iw, gh = th * p.bh + ih, gb = tb * p.nb + ib;
-    const bool row_ok = gw < p.W && gh < p.H && gb < p.Bn;
-    const long long m = (static_cast<long long>(gb) * p.H + gh) * p.W + gw;
-    const int img = row_ok ? static_cast<int>(m / p.rows_per_img) : 0;
-    const int tok = row_ok ? static_cast<int>(m % p.rows_per_img) : 0;
-    const float* srow = stg + r * LD;
-    if (p.splits == 1) {
-        for (int c = 32 * half; c < bn_out; c += 64) {
-            float v[32], g[GEGLU ? 32 : 1];
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-                const float4 x = *reinterpret_cast<const float4*>(srow + c + 4 * q);
-                v[4 * q] = x.x; v[4 * q + 1] = x.y; v[4 * q + 2] = x.z; v[4 * q + 3] = x.w;
-                if (GEGLU) {
-                    const float4 y = *reinterpret_cast<const float4*>(srow + bn_out + c + 4 * q);
-                    g[4 * q] = y.x; g[4 * q + 1] = y.y; g[4 * q + 2] = y.z; g[4 * q + 3] = y.w;
-                }
-            }
-            epilogue_chunk<GEGLU>(p, v, g, c, bn_out, n0, row_ok, m, img, tok, sb);
-        }
-    } else {
-        // ---- split-K: park this split's partial tile in its own fp32 workspace slice (plain stores)
-        const int tile_mn = nt * m_tiles + mt;
-        const long long slice = static_cast<long long>(GEMM_BM) * BN;
-        // slice layout [BN / 4][128 rows][4 floats]: thread = row, so the 32 lanes of a warp touch 32 consecutive
-        // 16-byte slots (512 contiguous bytes per instruction) both when parking and when reducing
-        float* wrow0 = p.ws + static_cast<long long>(tile_mn) * p.splits * slice + static_cast<long long>(r) * 4;
-        float* wrow = wrow0 + ks * slice;
-        auto wofs = [](int col) { return static_cast<long long>(col >> 2) * (GEMM_BM * 4); };
-        for (int c = 32 * half; c < BN; c += 64) {
-#pragma unroll
-            for (int q = 0; q < 8; ++q)
-                __stcg(reinterpret_cast<float4*>(wrow + wofs(c + 4 * q)), *reinterpret_cast<const float4*>(srow + c + 4 * q));
-        }
-        __threadfence();
-        named_bar_sync(1, GEMM_CONSUMERS);
-        if (ct == 0) {
-            const unsigned int old = atomicAdd(&p.counters[tile_mn], 1u);
-            const int last = (old == static_cast<unsigned int>(p.splits - 1));
-            if (last) p.counters[tile_mn] = 0;  // self-cleaning: ready for the next launch
-            *last_flag = last;
-        }
-        named_bar_sync(1, GEMM_CONSUMERS);
-        if (*last_flag) {
-            __threadfence();
-            for (int c = 32 * half; c < bn_out; c += 64) {
-                float v[32], g[32];
-#pragma unroll
-                for (int q = 0; q < 8; ++q) {
-                    float4 t4 = make_float4(0.f, 0.f, 0.f, 0.f), g4 = t4;
-                    for (int sl = 0; sl < p.splits; ++sl) {  // fixed order: deterministic sums
-                        const float4 x4 = __ldcg(reinterpret_cast<const float4*>(wrow0 + sl * slice + wofs(c + 4 * q)));
-                        t4.x += x4.x; t4.y += x4.y; t4.z += x4.z; t4.w += x4.w;
-                        if (GEGLU) {
-                            const float4 y4 = __ldcg(reinterpret_cast<const float4*>(wrow0 + sl * slice + wofs(bn_out + c + 4 * q)));
-                            g4.x += y4.x; g4.y += y4.y; g4.z += y4.z; g4.w += y4.w;
-                        }
+            int s = 0;
+            uint32_t phase = 0;
+            for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+                const GemmUnit w = gemm_unit(p, u, m_tiles, k_iters);
+                const int tw = w.mt % p.tiles_w, th = (w.mt / p.tiles_w) % p.tiles_h, tb = w.mt / (p.tiles_w * p.tiles_h);
+                const int w0 = tw * p.bw - p.pad, h0 = th * p.bh - p.pad, b0 = tb * p.nb, n0 = w.nt * BN_OUT;
+                for (int it = w.it0; it < w.it1; ++it) {
+                    mbar_wait_nocall(&empty[s], phase ^ 1);
+                    uint8_t* dst = smem + s * p.stage_bytes;
+                    mbar_expect_tx(&full[s], tx_bytes);
+                    if (it < main_iters) {
+                        const int tap = it / p.kchunks, kc = it - tap * p.kchunks, ky = tap / p.kw, kx = tap - ky * p.kw;
+                        tma_load_4d(dst, &tmA, &full[s], kc * GEMM_BK, w0 + kx, h0 + ky, b0);
+                        tma_load_3d(dst + GEMM_A_BYTES, &tmB, &full[s], kc * GEMM_BK, tap, n0);
+                        if (GEGLU) tma_load_3d(dst + GEMM_A_BYTES + BN_OUT * 128, &tmB, &full[s], kc * GEMM_BK, tap, p.N + n0);
+                    } else {  // second operand pair (fused 1x1 skip convolution)
+                        const int c0 = (it - main_iters) * GEMM_BK;
+                        tma_load_4d(dst, &tmA2, &full[s], c0, w0 + p.pad, h0 + p.pad, b0);
+                        tma_load_3d(dst + GEMM_A_BYTES, &tmB2, &full[s], c0, 0, n0);
                     }
-                    v[4 * q] = t4.x; v[4 * q + 1] = t4.y; v[4 * q + 2] = t4.z; v[4 * q + 3] = t4.w;
-                    g[4 * q] = g4.x; g[4 * q + 1] = g4.y; g[4 * q + 2] = g4.z; g[4 * q + 3] = g4.w;
+                    if (++s == nstages) { s = 0; phase ^= 1; }
                 }
-                epilogue_chunk<GEGLU>(p, v, g, c, bn_out, n0, row_ok, m, img, tok, sb);
             }
+        }
+        return;  // the consumers synchronise among themselves only (named barriers 1-3)
+    }
+
+    // -------------------------------------------------------- consumers: rows [64 wg, 64 wg + 64) of every tile
+    setmaxnreg_inc<GEMM_CONSUMER_REGS>();
+    const int ct = threadIdx.x - 128;  // 0..255
+    const int wg = ct >> 7, t = ct & 127;
+    const uint32_t smem0 = smem_u32(smem);
+    const uint32_t stg = smem0 + GEMM_SMEM_DATA + wg * (64 * GEMM_EPI_COLS * 4);
+    const int fr = ((t >> 5) << 4) + (lane >> 2), cq = 2 * (lane & 3);  // accumulator fragment: rows fr, fr + 8
+    const int er = t & 63, eh = t >> 6;                                  // epilogue: row er, 32-column half eh of a slab
+    const long long slice = static_cast<long long>(GEMM_BM) * BN;       // floats of one split-K workspace slice
+    int s = 0;
+    uint32_t phase = 0;
+    for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+        const GemmUnit w = gemm_unit(p, u, m_tiles, k_iters);
+        float acc[NACC];
+#pragma unroll
+        for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+        int prev = -1;
+        for (int it = w.it0; it < w.it1; ++it) {
+            mbar_wait_nocall(&full[s], phase);
+            const uint32_t a_base = smem0 + s * p.stage_bytes + wg * 64 * 128;
+            const uint32_t b_base = smem0 + s * p.stage_bytes + GEMM_A_BYTES;
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < GEMM_BK / 16; ++k)
+                WgmmaSS<BN, 0, 0>::mma(acc, wgmma_desc_kmajor(a_base + 32 * k), wgmma_desc_kmajor(b_base + 32 * k),
+                                       (it > w.it0 || k > 0) ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<1>();  // the previous stage's MMAs have finished reading it
+            if (prev >= 0) mbar_arrive(&empty[prev]);
+            prev = s;
+            if (++s == nstages) { s = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        wgmma_fence_regs<NACC>(acc);
+        mbar_arrive(&empty[prev]);  // the producer may refill the ring for the next unit during this epilogue
+
+        if (w.slot >= 0) {
+            // ---- split-K: park this split's partial tile in its own fp32 workspace slice in fragment order (each
+            // warp stores 512 contiguous bytes per instruction); the last CTA to arrive sums the slices in slice order
+            float* frag0 = p.ws + static_cast<long long>(w.slot) * p.splits * slice + ct * 4;
+#pragma unroll
+            for (int i = 0; i < NACC / 4; ++i)
+                __stcg(reinterpret_cast<float4*>(frag0 + w.ks * slice + i * (GEMM_CONSUMERS * 4)),
+                       make_float4(acc[4 * i], acc[4 * i + 1], acc[4 * i + 2], acc[4 * i + 3]));
+            __threadfence();
+            named_bar_sync(1, GEMM_CONSUMERS);
+            if (ct == 0) {
+                const unsigned int old = atomicAdd(&p.counters[w.slot], 1u);
+                const int last = (old == static_cast<unsigned int>(p.splits - 1));
+                if (last) p.counters[w.slot] = 0;  // self-cleaning: ready for the next launch
+                *last_flag = last;
+            }
+            named_bar_sync(1, GEMM_CONSUMERS);
+            if (!*last_flag) continue;
+            __threadfence();
+#pragma unroll
+            for (int i = 0; i < NACC / 4; ++i) {
+                float4 t4 = make_float4(0.f, 0.f, 0.f, 0.f);
+                for (int sl = 0; sl < p.splits; ++sl) {  // fixed order: deterministic sums
+                    const float4 x4 = __ldcg(reinterpret_cast<const float4*>(frag0 + sl * slice + i * (GEMM_CONSUMERS * 4)));
+                    t4.x += x4.x; t4.y += x4.y; t4.z += x4.z; t4.w += x4.w;
+                }
+                acc[4 * i] = t4.x; acc[4 * i + 1] = t4.y; acc[4 * i + 2] = t4.z; acc[4 * i + 3] = t4.w;
+            }
+        }
+
+        // ---- bias and GEGLU on the fragment: a thread holds value column c and its gate column c + BN_OUT
+        const int n0 = w.nt * BN_OUT;
+#pragma unroll
+        for (int i = 0; i < BN_OUT / 8; ++i) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int n = n0 + 8 * i + cq + e;
+                float bv = 0.f, bg = 0.f;
+                if (p.bias && n < p.N) {
+                    bv = __ldg(p.bias + n);
+                    if (GEGLU) bg = __ldg(p.bias + p.N + n);
+                }
+                acc[4 * i + e] += bv;
+                acc[4 * i + 2 + e] += bv;
+                if (GEGLU) {
+                    acc[4 * i + e] *= gelu_erf_f(acc[4 * (i + BN_OUT / 8) + e] + bg);
+                    acc[4 * i + 2 + e] *= gelu_erf_f(acc[4 * (i + BN_OUT / 8) + 2 + e] + bg);
+                }
+            }
+        }
+
+        // ---- the rest of the epilogue, one 64-column slab at a time through this warpgroup's staging buffer
+        const int tw = w.mt % p.tiles_w, th = (w.mt / p.tiles_w) % p.tiles_h, tb = w.mt / (p.tiles_w * p.tiles_h);
+        const int r = wg * 64 + er;
+        const int iw = r % p.bw, ih = (r / p.bw) % p.bh, ib = r / (p.bw * p.bh);
+        const int gw = tw * p.bw + iw, gh = th * p.bh + ih, gb = tb * p.nb + ib;
+        const bool row_ok = gw < p.W && gh < p.H && gb < p.Bn;
+        const long long m = (static_cast<long long>(gb) * p.H + gh) * p.W + gw;
+        const int img = row_ok ? static_cast<int>(m / p.rows_per_img) : 0;
+        const int tok = row_ok ? static_cast<int>(m % p.rows_per_img) : 0;
+        constexpr int NSLAB = (BN_OUT + GEMM_EPI_COLS - 1) / GEMM_EPI_COLS;
+#pragma unroll
+        for (int sl = 0; sl < NSLAB; ++sl) {
+            const int s0 = sl * GEMM_EPI_COLS;
+#pragma unroll
+            for (int j = 0; j < GEMM_EPI_COLS / 8; ++j) {
+                const int i = sl * (GEMM_EPI_COLS / 8) + j;
+                if (i >= BN_OUT / 8) break;
+                const int col = 8 * j + cq;
+                asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(epi_addr(stg, fr, col)), "f"(acc[4 * i]), "f"(acc[4 * i + 1])
+                             : "memory");
+                asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(epi_addr(stg, fr + 8, col)), "f"(acc[4 * i + 2]),
+                             "f"(acc[4 * i + 3])
+                             : "memory");
+            }
+            named_bar_sync(2 + wg, 128);
+            // a thread takes 32 columns of its row, in chunks of CW (16 with 256-column tiles: the accumulators of the
+            // later slabs are still live)
+            constexpr int CW = BN_OUT > 128 ? 16 : 32;
+#pragma unroll
+            for (int c1 = 0; c1 < 32; c1 += CW) {
+                const int c = s0 + 32 * eh + c1;
+                if (c < BN_OUT) {
+                    float v[CW];
+#pragma unroll
+                    for (int q = 0; q < CW / 4; ++q) {
+                        const float4 x = lds128f(epi_addr(stg, er, 32 * eh + c1 + 4 * q));
+                        v[4 * q] = x.x; v[4 * q + 1] = x.y; v[4 * q + 2] = x.z; v[4 * q + 3] = x.w;
+                    }
+                    epilogue_chunk<CW>(p, v, c, BN_OUT, n0, row_ok, m, img, tok);
+                }
+            }
+            named_bar_sync(2 + wg, 128);  // the slab is free for the next one
         }
     }
 }
@@ -374,7 +415,15 @@ static int pow2_floor(int x) {
 }
 
 static int g_num_sms = 0;
-static int g_sm_limit = 0;  // > 0: SM budget the tile-size model plans with (ctrlora_set_sm_limit)
+static int g_sm_limit = 0;  // > 0: SM budget of the persistent grid and the tile model (ctrlora_set_sm_limit)
+
+// constants of the tile model (cycles of one SM): estimates from the data-sheet rates, not yet fitted to a sweep;
+// tools/sweep_gemm.py times every (block_n, split_k) of the step's shapes against the model's choice
+constexpr double GEMM_L2_BPC = 40.0;          // operand bytes per cycle an SM streams from L2 with all SMs busy
+constexpr double GEMM_EPI_FIXED = 600.0;      // per tile: drain, row setup
+constexpr double GEMM_EPI_PER_COL = 12.0;     // per output column of a tile (128 rows: stores, residual reads)
+constexpr double GEMM_SPLIT_PER_COL = 12.0;   // per accumulator column and slice moved through the workspace (512 B)
+constexpr int GEMM_MAX_AUTO_SPLIT = 8;
 static bool g_attr_set = false;
 
 template <bool GEGLU, int BN>
@@ -422,45 +471,55 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
     const int sms = g_sm_limit > 0 && g_sm_limit < g_num_sms ? g_sm_limit : g_num_sms;
     const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_b;
     const int k_iters = p.taps * p.kchunks + p.kchunks2;
-    // ---- pick the N tile (wgmma N = 32, 64 or 128 output columns; GEGLU tiles carry value + gate) and the K split with
-    // a per-tile cycle model: a k-step costs max(MMA = BN cycles for 128 x BN x 64 at the dense fp16 rate of one SM,
-    // operand bytes / 64 B/clk from L2); a launch costs waves x (k-steps + epilogue).
-    int bn_out = a->block_n, splits = a->split_k > 0 ? a->split_k : 1;
+    // ---- pick the N tile (wgmma N = 32 ... 256 columns; GEGLU tiles carry value + gate) and the split of the tail with
+    // a cycle model of the persistent schedule over `sms` CTAs.  A k-step of a 128 x BN tile costs max(MMA: 4 BN cycles
+    // at the dense fp16 rate of one SM, operand bytes / GEMM_L2_BPC from L2); a tile adds its epilogue.  Full waves of
+    // tiles run whole; the tiles of the last, partial wave may be split along K so that their work units fill it.
+    // A plan that does not fit the split-K workspace or counters is not considered.  An explicit block_n / split_k
+    // overrides the model (split_k then splits every tile).
+    const bool explicit_split = a->split_k > 0;
     const int max_out = p.geglu ? GEMM_MAX_BN / 2 : GEMM_MAX_BN;
-    if (bn_out <= 0) {
-        double best_cost = -1;
-        for (int cand = max_out; cand >= 32; cand /= 2) {
-            if (a->seg_width > 0 && a->seg_width % cand != 0) continue;
-            const int bnt = p.geglu ? 2 * cand : cand;
-            const int nt = (p.N + cand - 1) / cand;
-            const long tiles_mn = (long)m_tiles * nt;
-            const double waste = (double)nt * cand / p.N;  // columns computed beyond N
-            const int S = a->split_k > 0 ? a->split_k : 1;  // only an explicit request splits K
-            const int kps = (k_iters + S - 1) / S;
-            const int s_eff = (k_iters + kps - 1) / kps;
-            const long tiles = tiles_mn * s_eff;
-            const long waves = (tiles + sms - 1) / sms;
-            const double t_mma = kps * (double)bnt;
-            const double t_load = kps * (double)(GEMM_A_BYTES + bnt * 128) / 64.0;
-            double t_tile = (t_mma > t_load ? t_mma : t_load) + 600.0 + cand * 8.0;
-            if (s_eff > 1) t_tile += bnt * 12.0;
-            const double cost = waves * t_tile * (0.5 + 0.5 * waste);
-            if (best_cost < 0 || cost < best_cost) { best_cost = cost; bn_out = cand; splits = s_eff; }
+    auto plan = [&](int cand, int S, int* s_eff, int* whole) -> double {
+        const int bnt = p.geglu ? 2 * cand : cand;
+        const long long tiles = (long long)m_tiles * ((p.N + cand - 1) / cand);
+        const int kps = (k_iters + S - 1) / S;
+        *s_eff = (k_iters + kps - 1) / kps;
+        long long w = *s_eff == 1 ? tiles : explicit_split ? 0 : (tiles / sms) * sms;
+        const long long tail = tiles - w;
+        if (*s_eff > 1 && (!a->splitk_ws || !a->splitk_counters || tail == 0 ||
+                           tail * *s_eff * GEMM_BM * bnt * 4 > a->splitk_ws_bytes || tail > a->splitk_counters_len))
+            return -1.0;
+        *whole = (int)w;
+        const double step = fmax(4.0 * bnt, (double)(GEMM_A_BYTES + bnt * 128) / GEMM_L2_BPC);
+        const double epi = GEMM_EPI_FIXED + GEMM_EPI_PER_COL * cand;
+        const double t_whole = k_iters * step + epi;
+        const double t_split = kps * step + epi + GEMM_SPLIT_PER_COL * bnt * (1 + *s_eff);
+        return (double)((w + sms - 1) / sms) * t_whole + (double)((tail * *s_eff + sms - 1) / sms) * t_split;
+    };
+    int bn_out = 0, splits = 1, tiles_whole = 0;
+    double best_cost = -1;
+    for (int cand = max_out; cand >= 32; cand /= 2) {
+        if (a->block_n > 0 && cand != a->block_n) continue;
+        if (a->seg_width > 0 && a->seg_width % cand != 0) continue;
+        for (int S = explicit_split ? a->split_k : 1; S <= (explicit_split ? a->split_k : GEMM_MAX_AUTO_SPLIT); ++S) {
+            int s_eff, whole;
+            const double cost = plan(cand, S, &s_eff, &whole);
+            if (cost < 0) continue;
+            if (best_cost < 0 || cost < best_cost) { best_cost = cost; bn_out = cand; splits = s_eff; tiles_whole = whole; }
         }
-        if (bn_out <= 0) return CTRLORA_ERR_ARG;  // no tile width divides seg_width
     }
-    if (bn_out != 32 && bn_out != 64 && bn_out != 128) return CTRLORA_ERR_ARG;
-    if (bn_out > max_out) return CTRLORA_ERR_ARG;
-    if (a->seg_width > 0 && a->seg_width % bn_out != 0) return CTRLORA_ERR_ARG;
+    if (bn_out <= 0) {
+        // no tile width divides seg_width, the explicit width is not a wgmma width, or an explicit split does not fit
+        // the workspace
+        return CTRLORA_ERR_ARG;
+    }
     p.BN = p.geglu ? 2 * bn_out : bn_out;
     p.n_tiles = (p.N + bn_out - 1) / bn_out;
     p.kiters_per_split = (k_iters + splits - 1) / splits;
     p.splits = (k_iters + p.kiters_per_split - 1) / p.kiters_per_split;
+    p.tiles_whole = tiles_whole;
+    p.units = tiles_whole + (m_tiles * p.n_tiles - tiles_whole) * p.splits;
     if (p.splits > 1) {
-        const long long tiles_mn = (long long)m_tiles * p.n_tiles;
-        if (!a->splitk_ws || !a->splitk_counters || tiles_mn * p.splits * GEMM_BM * p.BN * 4 > a->splitk_ws_bytes ||
-            tiles_mn > a->splitk_counters_len)
-            return CTRLORA_ERR_ARG;
         p.ws = a->splitk_ws;
         p.counters = a->splitk_counters;
     }
@@ -511,22 +570,26 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
     }
     if (!g_attr_set) {
         if (!set_smem_attr<false, 32>() || !set_smem_attr<false, 64>() || !set_smem_attr<false, 128>() ||
-            !set_smem_attr<true, 64>() || !set_smem_attr<true, 128>())
+            !set_smem_attr<false, 256>() || !set_smem_attr<true, 64>() || !set_smem_attr<true, 128>() ||
+            !set_smem_attr<true, 256>())
             return CTRLORA_ERR_CUDA;
         g_attr_set = true;
     }
-    const dim3 grid((unsigned)((long long)m_tiles * p.n_tiles * p.splits));
+    const dim3 grid((unsigned)(p.units < sms ? p.units : sms));
     cudaError_t lrc;
-    if (p.geglu) lrc = p.BN == 64 ? launch_gemm<true, 64>(grid, stream, tmA, tmB, tmA2, tmB2, p)
-                                  : launch_gemm<true, 128>(grid, stream, tmA, tmB, tmA2, tmB2, p);
-    else lrc = p.BN == 32 ? launch_gemm<false, 32>(grid, stream, tmA, tmB, tmA2, tmB2, p)
-             : p.BN == 64 ? launch_gemm<false, 64>(grid, stream, tmA, tmB, tmA2, tmB2, p)
-                          : launch_gemm<false, 128>(grid, stream, tmA, tmB, tmA2, tmB2, p);
+    if (p.geglu) lrc = p.BN == 64  ? launch_gemm<true, 64>(grid, stream, tmA, tmB, tmA2, tmB2, p)
+                     : p.BN == 128 ? launch_gemm<true, 128>(grid, stream, tmA, tmB, tmA2, tmB2, p)
+                                   : launch_gemm<true, 256>(grid, stream, tmA, tmB, tmA2, tmB2, p);
+    else lrc = p.BN == 32  ? launch_gemm<false, 32>(grid, stream, tmA, tmB, tmA2, tmB2, p)
+             : p.BN == 64  ? launch_gemm<false, 64>(grid, stream, tmA, tmB, tmA2, tmB2, p)
+             : p.BN == 128 ? launch_gemm<false, 128>(grid, stream, tmA, tmB, tmA2, tmB2, p)
+                           : launch_gemm<false, 256>(grid, stream, tmA, tmB, tmA2, tmB2, p);
     if (lrc != cudaSuccess) return CTRLORA_ERR_CUDA;
     return cudaGetLastError() == cudaSuccess ? CTRLORA_OK : CTRLORA_ERR_CUDA;
 }
 
-// The tile-size model of ctrlora_gemm_f16 plans with at most `limit` SMs (0 = all).  A communication kernel that runs
+// The persistent grid of ctrlora_gemm_f16 uses at most `limit` CTAs, one per SM, and its tile model plans with that
+// many SMs (0 = all).  A communication kernel that runs
 // next to the backward (the overlapped gradient all-reduce) owns a few SMs.  The limit is read at launch time, i.e. it
 // is baked into a CUDA graph at capture.
 extern "C" int ctrlora_set_sm_limit(int limit) {

@@ -6,14 +6,17 @@ namespace ctrl {
 
 constexpr int GEMM_BM = 128;            // two consumer warpgroups x wgmma M = 64
 constexpr int GEMM_BK = 64;             // 64 fp16 = 128 B = one SWIZZLE_128B row
-constexpr int GEMM_MAX_BN = 128;        // wgmma N of one tile (GEGLU: value half + gate half); 64 accumulators per thread
+constexpr int GEMM_MAX_BN = 256;        // wgmma N of one tile (GEGLU: value half + gate half); 128 accumulators per thread
 constexpr int GEMM_MAX_STAGES = 8;
 constexpr int GEMM_A_BYTES = GEMM_BM * GEMM_BK * 2;   // 16 KiB
 constexpr int GEMM_THREADS = 384;       // warpgroup 0: TMA producer (one thread), warpgroups 1-2: wgmma + epilogue
 constexpr int GEMM_CONSUMERS = 256;
-constexpr int GEMM_SMEM_DATA = 192 * 1024;            // operand ring; the epilogue stages the fp32 tile over it
-constexpr int GEMM_STAGE_LD = GEMM_MAX_BN + 4;        // fp32 row pitch of the epilogue staging tile
-constexpr int GEMM_SMEM_BYTES = GEMM_SMEM_DATA + 1024 /*align slack*/ + 256 /*barriers*/ + 2048 /*bias staging*/;
+constexpr int GEMM_PRODUCER_REGS = 40;  // setmaxnreg split: 128 * 40 + 256 * 232 <= 64 K registers
+constexpr int GEMM_CONSUMER_REGS = 232;
+constexpr int GEMM_SMEM_DATA = 192 * 1024;            // operand ring (the producer fills it during the epilogue)
+constexpr int GEMM_EPI_COLS = 64;                     // epilogue slab: 64 rows x 64 fp32 columns per consumer warpgroup
+constexpr int GEMM_EPI_BYTES = 2 * 64 * GEMM_EPI_COLS * 4;  // 32 KiB, 16-byte chunks XOR-swizzled by row
+constexpr int GEMM_SMEM_BYTES = GEMM_SMEM_DATA + GEMM_EPI_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 
 struct GemmKParams {
     // tile geometry over the (B, H, W) pixel grid; a plain [M, K] matrix is B=1, H=1, W=M
@@ -28,7 +31,11 @@ struct GemmKParams {
     int kchunks2;                   // extra 1x1 segment from the second operand pair (0 = none)
     int geglu;                      // 1: weights are [2N, K]; out = value * gelu(gate)
     int stages, stage_bytes;        // TMA ring: stage = A tile (16 KiB) + B tile (BN * 128 B, 1 KiB aligned)
-    int splits, kiters_per_split;   // split-K: partial sums meet in `ws` (fp32, self-cleaning), last CTA runs the epilogue
+    // persistent schedule: work unit u < tiles_whole is output tile u over the whole K range; the units after it are
+    // the remaining tiles split `splits` ways along K (partial sums meet in `ws`, fp32; the self-cleaning counter of
+    // the tile picks the last-arriving CTA, which sums the slices in slice order and runs the epilogue)
+    int units, tiles_whole;
+    int splits, kiters_per_split;
     float* ws;
     unsigned int* counters;
     // epilogue
