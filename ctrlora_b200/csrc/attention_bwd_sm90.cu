@@ -151,11 +151,11 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     float dq[DP / 2];
 #pragma unroll
     for (int i = 0; i < DP / 2; ++i) dq[i] = 0.f;
-    mbar_wait(&bars[0], 0);
+    mbar_wait_nocall(&bars[0], 0);
     for (int t = 0; t < n_tiles; ++t) {
         const int st = t & 1;
         const uint32_t sK = s0 + L::OWN + st * L::STAGE, sV = sK + L::TILE;
-        mbar_wait(&bars[1 + st], (t >> 1) & 1);
+        mbar_wait_nocall(&bars[1 + st], (t >> 1) & 1);
         float s[32], dp[32];
         wgmma_fence();
         ab_dot<DP>(s, s0, sK);
@@ -239,7 +239,7 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
         if (DO_K) dk[i] = 0.f;
         if (DO_V) dv[i] = 0.f;
     }
-    mbar_wait(&bars[0], 0);
+    mbar_wait_nocall(&bars[0], 0);
     for (int t = 0; t < n_tiles; ++t) {
         const int st = t & 1;
         const uint32_t sQ = s0 + L::OWN + st * L::STAGE, sDO = sQ + L::TILE;
@@ -249,7 +249,7 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
             sl[tid] = q < p.Nq ? (tid < 64 ? p.lse[stat + q] : p.delta[stat + q]) : 0.f;
         }
         __syncthreads();
-        mbar_wait(&bars[1 + st], (t >> 1) & 1);
+        mbar_wait_nocall(&bars[1 + st], (t >> 1) & 1);
         float s[32], dp[DO_K ? 32 : 1];
         wgmma_fence();
         ab_dot<DP>(s, s0, sQ);

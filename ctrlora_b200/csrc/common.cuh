@@ -126,6 +126,9 @@ __device__ __forceinline__ uint64_t wgmma_desc_mnmajor(uint32_t smem_addr, uint3
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
+    asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 __device__ __forceinline__ float max3f(float a, float b, float c) {
     float r;
     asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));

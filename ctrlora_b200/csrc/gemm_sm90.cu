@@ -415,7 +415,18 @@ static int pow2_floor(int x) {
 }
 
 static int g_num_sms = 0;
-static int g_sm_limit = 0;  // > 0: SM budget of the persistent grid and the tile model (ctrlora_set_sm_limit)
+static int g_sm_limit = 0;  // > 0: SM budget of the persistent grids and the tile model (ctrlora_set_sm_limit)
+
+// SMs a persistent grid may occupy: the device's count, capped by ctrlora_set_sm_limit; 0 if the count is unavailable
+int persistent_sms() {
+    if (g_num_sms == 0) {
+        int dev = 0;
+        cudaGetDevice(&dev);
+        cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
+        if (g_num_sms <= 0) return 0;
+    }
+    return g_sm_limit > 0 && g_sm_limit < g_num_sms ? g_sm_limit : g_num_sms;
+}
 
 // constants of the tile model (cycles of one SM): estimates from the data-sheet rates, not yet fitted to a sweep;
 // tools/sweep_gemm.py times every (block_n, split_k) of the step's shapes against the model's choice
@@ -462,13 +473,8 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
     p.kchunks = (a->a_c + GEMM_BK - 1) / GEMM_BK;
     p.kchunks2 = a->a2 ? (a->a2_c + GEMM_BK - 1) / GEMM_BK : 0;
     p.geglu = a->geglu;
-    if (g_num_sms == 0) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-        if (g_num_sms <= 0) return CTRLORA_ERR_CUDA;
-    }
-    const int sms = g_sm_limit > 0 && g_sm_limit < g_num_sms ? g_sm_limit : g_num_sms;
+    const int sms = persistent_sms();
+    if (sms <= 0) return CTRLORA_ERR_CUDA;
     const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_b;
     const int k_iters = p.taps * p.kchunks + p.kchunks2;
     // ---- pick the N tile (wgmma N = 32 ... 256 columns; GEGLU tiles carry value + gate) and the split of the tail with

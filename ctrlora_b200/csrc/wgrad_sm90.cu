@@ -65,7 +65,7 @@ wgrad_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         if (warp == 0 && elect_one()) {
             for (int j = 0; j < nit; ++j) {
                 const int s = j % p.stages, tok = (it0 + j) * WG_BK;
-                mbar_wait(&empty[s], ((j / p.stages) & 1) ^ 1);
+                mbar_wait_nocall(&empty[s], ((j / p.stages) & 1) ^ 1);
                 uint8_t* dst = smem + s * p.stage_bytes;
                 mbar_expect_tx(&full[s], WG_A_BYTES + p.q_atoms * WG_BK * 128);
                 tma_load_2d(dst, &tmA, &full[s], pt * 128, tok);
@@ -83,7 +83,7 @@ wgrad_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     const uint32_t smem0 = smem_u32(smem);
     for (int j = 0; j < nit; ++j) {
         const int s = j % p.stages;
-        mbar_wait(&full[s], (j / p.stages) & 1);
+        mbar_wait_nocall(&full[s], (j / p.stages) & 1);
         const uint32_t a_base = smem0 + s * p.stage_bytes + wg * WG_BK * 128;
         const uint32_t b_base = smem0 + s * p.stage_bytes + WG_A_BYTES;
         wgmma_fence();

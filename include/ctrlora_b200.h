@@ -164,7 +164,7 @@ int ctrlora_transpose_f16(const void* src, void* dst, long long batch, int rows,
  * rebuilt every step in pretraining, where the conv weights train (cldm/cldm_ctrlora_pretrain.py:88-96). */
 int ctrlora_conv_dgrad_weight_f16(const void* src, void* dst, int cout, int taps, int cin, void* stream);
 
-/* Persistent GEMM grids use at most `limit` SMs from now on (0 = all of them): the gradient all-reduce that overlaps the
+/* Persistent GEMM and attention-forward grids use at most `limit` SMs from now on (0 = all of them): the gradient all-reduce that overlaps the
  * ControlNet backward (the reference's DDP does the same overlap by buckets, pytorch_lightning strategy "ddp",
  * train_ctrlora_pretrain.py) owns a few SMs, and a 148-CTA persistent grid would wait for them.  Read at launch time. */
 int ctrlora_set_sm_limit(int limit);
