@@ -4,7 +4,7 @@
 // D[M, N] = sum_taps A_shifted[M, Cin] * W[N, tap, Cin]^T  (+ optional second 1x1 operand pair: the ResBlock skip conv)
 // A tiles are TMA boxes over the (C, W, H, B) activation tensor: a filter tap is a coordinate shift and the conv zero
 // padding is the TMA out-of-bounds fill, so no im2col buffer exists in HBM.  The grid is persistent: each CTA walks a
-// static list of 128 x BN output tiles (BN up to 256), a producer thread fills a ring of TMA stages, and two consumer
+// static list of 128 x BN output tiles (BN up to 320), a producer thread fills a ring of TMA stages, and two consumer
 // warpgroups (64 rows each) run wgmma with accumulators in registers, then run a row-per-thread epilogue through a
 // staging buffer of their own while the producer already loads the next tile.  Tiles of a last, partial wave may be
 // split along K.
@@ -165,6 +165,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                   const __grid_constant__ GemmKParams p) {
     constexpr int BN_OUT = GEGLU ? BN / 2 : BN;
     constexpr int NACC = BN / 2;  // fp32 accumulators per consumer thread (64 rows x BN per warpgroup)
+    constexpr int BOX = GEGLU || BN > 256 ? BN / 2 : BN;  // rows of one B TMA box: a tile is one box or two
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + GEMM_SMEM_DATA + GEMM_EPI_BYTES);
@@ -215,11 +216,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                         const int tap = it / p.kchunks, kc = it - tap * p.kchunks, ky = tap / p.kw, kx = tap - ky * p.kw;
                         tma_load_4d(dst, &tmA, &full[s], kc * GEMM_BK, w0 + kx, h0 + ky, b0);
                         tma_load_3d(dst + GEMM_A_BYTES, &tmB, &full[s], kc * GEMM_BK, tap, n0);
-                        if (GEGLU) tma_load_3d(dst + GEMM_A_BYTES + BN_OUT * 128, &tmB, &full[s], kc * GEMM_BK, tap, p.N + n0);
+                        if (BOX < BN)  // GEGLU: the gate rows start at N
+                            tma_load_3d(dst + GEMM_A_BYTES + BOX * 128, &tmB, &full[s], kc * GEMM_BK, tap, GEGLU ? p.N + n0 : n0 + BOX);
                     } else {  // second operand pair (fused 1x1 skip convolution)
                         const int c0 = (it - main_iters) * GEMM_BK;
                         tma_load_4d(dst, &tmA2, &full[s], c0, w0 + p.pad, h0 + p.pad, b0);
                         tma_load_3d(dst + GEMM_A_BYTES, &tmB2, &full[s], c0, 0, n0);
+                        if (BOX < BN) tma_load_3d(dst + GEMM_A_BYTES + BOX * 128, &tmB2, &full[s], c0, 0, n0 + BOX);
                     }
                     if (++s == nstages) { s = 0; phase ^= 1; }
                 }
@@ -251,9 +254,16 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             const uint32_t b_base = smem0 + s * p.stage_bytes + GEMM_A_BYTES;
             wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < GEMM_BK / 16; ++k)
-                WgmmaSS<BN, 0, 0>::mma(acc, wgmma_desc_kmajor(a_base + 32 * k), wgmma_desc_kmajor(b_base + 32 * k),
-                                       (it > w.it0 || k > 0) ? 1u : 0u);
+            for (int k = 0; k < GEMM_BK / 16; ++k) {
+                const uint32_t sc = (it > w.it0 || k > 0) ? 1u : 0u;
+                if constexpr (BN > 256) {  // columns [0, 160) and [160, 320): the fragment stays in column order
+                    WgmmaSS<BN / 2, 0, 0>::mma(acc, wgmma_desc_kmajor(a_base + 32 * k), wgmma_desc_kmajor(b_base + 32 * k), sc);
+                    WgmmaSS<BN / 2, 0, 0>::mma(acc + NACC / 2, wgmma_desc_kmajor(a_base + 32 * k),
+                                               wgmma_desc_kmajor(b_base + (BN / 2) * 128 + 32 * k), sc);
+                } else {
+                    WgmmaSS<BN, 0, 0>::mma(acc, wgmma_desc_kmajor(a_base + 32 * k), wgmma_desc_kmajor(b_base + 32 * k), sc);
+                }
+            }
             wgmma_commit();
             wgmma_wait<1>();  // the previous stage's MMAs have finished reading it
             if (prev >= 0) mbar_arrive(&empty[prev]);
@@ -296,8 +306,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
         // ---- bias and GEGLU on the fragment: a thread holds value column c and its gate column c + BN_OUT
         const int n0 = w.nt * BN_OUT;
-#pragma unroll
-        for (int i = 0; i < BN_OUT / 8; ++i) {
+        auto bias_geglu = [&](int i) {
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
                 const int n = n0 + 8 * i + cq + e;
@@ -313,8 +322,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     acc[4 * i + 2 + e] *= gelu_erf_f(acc[4 * (i + BN_OUT / 8) + 2 + e] + bg);
                 }
             }
+        };
+        // GEGLU: all at once, which frees the gate accumulators.  Otherwise per slab as it is staged, so only one
+        // slab's bias loads are in flight next to the accumulators
+        if (GEGLU) {
+#pragma unroll
+            for (int i = 0; i < BN_OUT / 8; ++i) bias_geglu(i);
         }
-
         // ---- the rest of the epilogue, one 64-column slab at a time through this warpgroup's staging buffer
         const int tw = w.mt % p.tiles_w, th = (w.mt / p.tiles_w) % p.tiles_h, tb = w.mt / (p.tiles_w * p.tiles_h);
         const int r = wg * 64 + er;
@@ -332,6 +346,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             for (int j = 0; j < GEMM_EPI_COLS / 8; ++j) {
                 const int i = sl * (GEMM_EPI_COLS / 8) + j;
                 if (i >= BN_OUT / 8) break;
+                if (!GEGLU) bias_geglu(i);
                 const int col = 8 * j + cq;
                 asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(epi_addr(stg, fr, col)), "f"(acc[4 * i]), "f"(acc[4 * i + 1])
                              : "memory");
@@ -340,7 +355,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                              : "memory");
             }
             named_bar_sync(2 + wg, 128);
-            // a thread takes 32 columns of its row, in chunks of CW (16 with 256-column tiles: the accumulators of the
+            // a thread takes 32 columns of its row, in chunks of CW (16 with wider tiles: the accumulators of the
             // later slabs are still live)
             constexpr int CW = BN_OUT > 128 ? 16 : 32;
 #pragma unroll
@@ -435,6 +450,10 @@ constexpr double GEMM_EPI_FIXED = 600.0;      // per tile: drain, row setup
 constexpr double GEMM_EPI_PER_COL = 12.0;     // per output column of a tile (128 rows: stores, residual reads)
 constexpr double GEMM_SPLIT_PER_COL = 12.0;   // per accumulator column and slice moved through the workspace (512 B)
 constexpr int GEMM_MAX_AUTO_SPLIT = 8;
+// 320-column tiles leave room for only 3 ring stages, and the model does not price what that costs a short K loop: on
+// the batch-8 step (H100 80GB HBM3, 400 W, tools/gemm_classes.py) they took 10-45 % longer than the narrower tiles
+// the model picks on every 1x1 GEMM with K <= 1280 (5-20 k-steps), and 10-40 % less time on the 3x3 convs (45+)
+static constexpr int GEMM_WIDE_MIN_KITERS = 40;
 static bool g_attr_set = false;
 
 template <bool GEGLU, int BN>
@@ -484,7 +503,6 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
     // A plan that does not fit the split-K workspace or counters is not considered.  An explicit block_n / split_k
     // overrides the model (split_k then splits every tile).
     const bool explicit_split = a->split_k > 0;
-    const int max_out = p.geglu ? GEMM_MAX_BN / 2 : GEMM_MAX_BN;
     auto plan = [&](int cand, int S, int* s_eff, int* whole) -> double {
         const int bnt = p.geglu ? 2 * cand : cand;
         const long long tiles = (long long)m_tiles * ((p.N + cand - 1) / cand);
@@ -504,8 +522,12 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
     };
     int bn_out = 0, splits = 1, tiles_whole = 0;
     double best_cost = -1;
-    for (int cand = max_out; cand >= 32; cand /= 2) {
+    static const int kWidths[] = {GEMM_MAX_BN, 256, 128, 64, 32};  // tile widths; GEGLU tiles carry half as many outputs
+    for (int wi = 0; wi < 5; ++wi) {
+        const int cand = p.geglu ? kWidths[wi] / 2 : kWidths[wi];
+        if (cand < 32) continue;
         if (a->block_n > 0 && cand != a->block_n) continue;
+        if (a->block_n <= 0 && kWidths[wi] > 256 && k_iters < GEMM_WIDE_MIN_KITERS) continue;
         if (a->seg_width > 0 && a->seg_width % cand != 0) continue;
         for (int S = explicit_split ? a->split_k : 1; S <= (explicit_split ? a->split_k : GEMM_MAX_AUTO_SPLIT); ++S) {
             int s_eff, whole;
@@ -544,6 +566,7 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
     p.head_dim = a->head_dim; p.tok_pad = a->tok_pad;
     p.dup_out = reinterpret_cast<__half*>(a->dup_out); p.dup_ld = a->dup_ld;
 
+    const int b_box = p.geglu || p.BN > 256 ? p.BN / 2 : p.BN;  // rows of a B box (the kernel's BOX)
     CUtensorMap tmA, tmB, tmA2, tmB2;
     {
         uint64_t dims[4] = {(uint64_t)a->a_c, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)p.Bn};
@@ -554,7 +577,7 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
         const uint64_t rows = p.geglu ? 2ull * p.N : (uint64_t)p.N;
         uint64_t wd[3] = {(uint64_t)a->a_c, (uint64_t)p.taps, rows};
         uint64_t ws[2] = {(uint64_t)a->a_c * 2, (uint64_t)a->a_c * 2 * p.taps};
-        uint32_t wb[3] = {GEMM_BK, 1, (uint32_t)bn_out};
+        uint32_t wb[3] = {GEMM_BK, 1, (uint32_t)b_box};
         rc = make_tmap_f16(&tmB, a->w, 3, wd, ws, wb);
         if (rc) return rc;
     }
@@ -567,7 +590,7 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
         if (rc) return rc;
         uint64_t wd[3] = {(uint64_t)a->a2_c, 1, (uint64_t)p.N};
         uint64_t ws[2] = {(uint64_t)a->a2_c * 2, (uint64_t)a->a2_c * 2};
-        uint32_t wb[3] = {GEMM_BK, 1, (uint32_t)bn_out};
+        uint32_t wb[3] = {GEMM_BK, 1, (uint32_t)b_box};
         rc = make_tmap_f16(&tmB2, a->w2, 3, wd, ws, wb);
         if (rc) return rc;
     } else {
@@ -576,8 +599,8 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
     }
     if (!g_attr_set) {
         if (!set_smem_attr<false, 32>() || !set_smem_attr<false, 64>() || !set_smem_attr<false, 128>() ||
-            !set_smem_attr<false, 256>() || !set_smem_attr<true, 64>() || !set_smem_attr<true, 128>() ||
-            !set_smem_attr<true, 256>())
+            !set_smem_attr<false, 256>() || !set_smem_attr<false, 320>() || !set_smem_attr<true, 64>() ||
+            !set_smem_attr<true, 128>() || !set_smem_attr<true, 256>() || !set_smem_attr<true, 320>())
             return CTRLORA_ERR_CUDA;
         g_attr_set = true;
     }
@@ -585,11 +608,13 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
     cudaError_t lrc;
     if (p.geglu) lrc = p.BN == 64  ? launch_gemm<true, 64>(grid, stream, tmA, tmB, tmA2, tmB2, p)
                      : p.BN == 128 ? launch_gemm<true, 128>(grid, stream, tmA, tmB, tmA2, tmB2, p)
-                                   : launch_gemm<true, 256>(grid, stream, tmA, tmB, tmA2, tmB2, p);
+                     : p.BN == 256 ? launch_gemm<true, 256>(grid, stream, tmA, tmB, tmA2, tmB2, p)
+                                   : launch_gemm<true, 320>(grid, stream, tmA, tmB, tmA2, tmB2, p);
     else lrc = p.BN == 32  ? launch_gemm<false, 32>(grid, stream, tmA, tmB, tmA2, tmB2, p)
              : p.BN == 64  ? launch_gemm<false, 64>(grid, stream, tmA, tmB, tmA2, tmB2, p)
              : p.BN == 128 ? launch_gemm<false, 128>(grid, stream, tmA, tmB, tmA2, tmB2, p)
-                           : launch_gemm<false, 256>(grid, stream, tmA, tmB, tmA2, tmB2, p);
+             : p.BN == 256 ? launch_gemm<false, 256>(grid, stream, tmA, tmB, tmA2, tmB2, p)
+                           : launch_gemm<false, 320>(grid, stream, tmA, tmB, tmA2, tmB2, p);
     if (lrc != cudaSuccess) return CTRLORA_ERR_CUDA;
     return cudaGetLastError() == cudaSuccess ? CTRLORA_OK : CTRLORA_ERR_CUDA;
 }

@@ -6,7 +6,9 @@ namespace ctrl {
 
 constexpr int GEMM_BM = 128;            // two consumer warpgroups x wgmma M = 64
 constexpr int GEMM_BK = 64;             // 64 fp16 = 128 B = one SWIZZLE_128B row
-constexpr int GEMM_MAX_BN = 256;        // wgmma N of one tile (GEGLU: value half + gate half); 128 accumulators per thread
+constexpr int GEMM_MAX_BN = 320;        // N of one tile (GEGLU: value half + gate half); 160 accumulators per thread.
+                                        // A 320-column tile is two m64n160 MMAs and two 160-row B boxes (TMA boxes
+                                        // are at most 256 rows); every UNet width is a multiple of 320
 constexpr int GEMM_MAX_STAGES = 8;
 constexpr int GEMM_A_BYTES = GEMM_BM * GEMM_BK * 2;   // 16 KiB
 constexpr int GEMM_THREADS = 384;       // warpgroup 0: TMA producer (one thread), warpgroups 1-2: wgmma + epilogue
@@ -30,7 +32,7 @@ struct GemmKParams {
     int kchunks;                    // ceil(Cin / 64) per tap
     int kchunks2;                   // extra 1x1 segment from the second operand pair (0 = none)
     int geglu;                      // 1: weights are [2N, K]; out = value * gelu(gate)
-    int stages, stage_bytes;        // TMA ring: stage = A tile (16 KiB) + B tile (BN * 128 B, 1 KiB aligned)
+    int stages, stage_bytes;        // TMA ring: stage = A tile (16 KiB) + B tile (BN * 128 B, 1 KiB aligned); 3 at BN 320
     // persistent schedule: work unit u < tiles_whole is output tile u over the whole K range; the units after it are
     // the remaining tiles split `splits` ways along K (partial sums meet in `ws`, fp32; the self-cleaning counter of
     // the tile picks the last-arriving CTA, which sums the slices in slice order and runs the epilogue)

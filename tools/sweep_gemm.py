@@ -42,7 +42,7 @@ if __name__ == "__main__":
         print(f"--- {ks}x{ks} {h}x{w} {c}->{n} (M={b * h * w}), {fl / 1e9:.0f} GF")
         auto = timeit(lambda: ops.gemm(a, wt, ksize=ks, bias=bias, residual=res, out=out))
         print(f"  auto: {auto * 1e3:7.1f} us {fl / auto / 1e9:6.0f} TF/s")
-        for bn in (256, 128, 64, 32):  # the wgmma tile widths of ctrlora_gemm_f16
+        for bn in (320, 256, 128, 64, 32):  # the wgmma tile widths of ctrlora_gemm_f16
             row = []
             for s in (1, 2, 4, 6, 8, 12):
                 try:
