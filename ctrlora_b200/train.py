@@ -24,7 +24,7 @@ import numbers
 import torch
 import torch.nn as nn
 
-from . import ops, prepare
+from . import checkpoint, ops, prepare
 from .runtime import nchw_view, pixel_major, to_f16_rows
 
 f32 = prepare.bias_f32
@@ -986,11 +986,14 @@ class FinetuneTrainer:
         self.step_count += 1
         self.micro_step = 0
         if self._poll_overflow():
-            # GradScaler semantics: the updates were skipped on the device; the scale is halved (re-capturing the graphs,
-            # whose loss kernel has the scale baked in)
-            self.seg_steps = {k: int(v.item()) for k, v in self._step_dev.items()}
-            self.step_count = self.seg_steps[segs[0][2]]
-            self._recapture()
+            self._after_skipped()
+
+    def _after_skipped(self):
+        """GradScaler semantics: the updates were skipped on the device; the scale is halved (re-capturing the graphs,
+        whose loss kernel has the scale baked in) and the host step counts are re-read"""
+        self.seg_steps = {k: int(v.item()) for k, v in self._step_dev.items()}
+        self.step_count = self.seg_steps.get(self.segment_keys()[0], 0)
+        self._recapture()
 
     def _recapture(self):
         if getattr(self, "_graph", None) is not None or self._accum is not None:
@@ -998,6 +1001,101 @@ class FinetuneTrainer:
 
     def _overflowed(self):
         return bool(self.overflow_flag.item())
+
+    # -- checkpoints in the reference's Lightning layout (ctrlora_b200.checkpoint) ---------------------------------------
+    def segment_keys(self):
+        """the step-count segment of every optimizer parameter (GradSink order)"""
+        return ["all"] * len(self.G.names)
+
+    def _alias_key(self, key):
+        """a state-dict key that names a parameter also stored under another key (checkpoint.checkpoint_weights)"""
+        return False
+
+    def _rank(self):
+        return torch.distributed.get_rank(self.pg) if self.world > 1 else 0
+
+    def _exact_counters(self):
+        """Read the device's skipped-step counter now (the periodic poll, forced), so step_count, seg_steps,
+        skipped_steps and loss_scale are exact on the host.  Refused inside an accumulation window."""
+        if self.micro_step != 0:
+            raise RuntimeError(f"cannot checkpoint inside an accumulation window ({self.micro_step} of "
+                               f"{self.accumulate_grad_batches} micro-batches done): the partial gradient is not part of "
+                               "the state; save between windows or after flush()")
+        launched = self._launched
+        try:
+            if self._poll_overflow(force=True):
+                self._after_skipped()
+        finally:
+            self._launched = launched  # the periodic poll keeps its cadence
+
+    def state_dict(self):
+        """The optimizer part of a checkpoint: {"optimizer": torch.optim.AdamW.state_dict() over the reference's
+        parameter list (a Lightning checkpoint's optimizer_states[0]), checkpoint.EXTRA_KEY: loss scale, skipped steps,
+        accumulate_grad_batches}.  Tensors are CPU copies."""
+        self._exact_counters()
+        return {"optimizer": checkpoint.optimizer_state_dict(self), checkpoint.EXTRA_KEY: checkpoint.trainer_extra(self)}
+
+    def load_state_dict(self, sd):
+        """Load state_dict()'s output, or a bare torch.optim.AdamW.state_dict(), in place: the flat moments, the host and
+        device step counters and the file's hyper-parameters (lr, betas, eps, weight_decay).  A parameter without state
+        is fresh (zero moments; its first step is AdamW step 1).  The current accumulation window is dropped.  Graphs
+        whose baked-in loss scale no longer matches are re-captured."""
+        if self._load_optimizer(sd):
+            self._recapture()
+
+    def _load_optimizer(self, sd):
+        """load_state_dict without the re-capture; True if a captured graph's loss scale no longer matches"""
+        opt, extra = (sd, None) if "param_groups" in sd else (sd["optimizer"], sd.get(checkpoint.EXTRA_KEY))
+        scale, skipped = checkpoint.parse_extra(self, extra)
+        checkpoint.load_optimizer_state_dict(self, opt)
+        self.loss_scale, self.skipped_steps = scale, skipped
+        self.micro_step, self._window_tasks = 0, []
+        self.overflow_flag.zero_()
+        self._skipped_dev.zero_()
+        self._skipped_seen = 0
+        return any(s != self._scale_for(self._static[0].numel()) for s in self._captured_scales())
+
+    def _captured_scales(self):
+        """loss scales baked into the captured graphs"""
+        out = [self._scale_used] if getattr(self, "_graph", None) is not None else []
+        if self._accum is not None:
+            out += [c[2] for c in self._accum["compute"].values()]
+        return out
+
+    def save_checkpoint(self, path, epoch=0):
+        """Write a checkpoint in the layout of the reference's `trainer.save_checkpoint` (cldm/logger.py:123):
+        state_dict (model.state_dict(), contiguous CPU copies in the reference shapes), optimizer_states
+        ([state_dict()["optimizer"]]), global_step (step_count: optimizer steps), epoch, and checkpoint.EXTRA_KEY.
+        Under torch.distributed every rank syncs its counters, rank 0 writes, and all ranks leave together."""
+        self._exact_counters()
+        if self._rank() == 0:
+            ckpt = {"epoch": int(epoch), "global_step": int(self.step_count),
+                    "state_dict": checkpoint.model_state_dict(self.model),
+                    "optimizer_states": [checkpoint.optimizer_state_dict(self)],
+                    checkpoint.EXTRA_KEY: checkpoint.trainer_extra(self)}
+            torch.save(ckpt, path)
+        if self.world > 1:
+            torch.distributed.barrier(group=self.pg)
+
+    def load_checkpoint(self, path):
+        """Load a checkpoint written by save_checkpoint or by the reference's Lightning trainer into this trainer, in
+        place: the weights through model.load_state_dict (keys of cond_stage_model, which the drop-in does not ship, are
+        ignored), then load_state_dict of optimizer_states[0] and checkpoint.EXTRA_KEY.  Everything is validated before
+        anything changes.  Trainable-weight copies are rebuilt, and captured graphs are re-captured (the frozen-weight
+        copies they read are built outside the capture).  Every rank of a data-parallel run loads the same file.
+        Returns {"epoch", "global_step"} of the file."""
+        ckpt = torch.load(path, map_location="cpu", weights_only=True)
+        weights = checkpoint.checkpoint_weights(ckpt["state_dict"], self.model.state_dict(), self._alias_key)
+        opts = ckpt.get("optimizer_states") or []
+        if len(opts) != 1:
+            raise ValueError(f"expected one optimizer state in the checkpoint, found {len(opts)}")
+        checkpoint.check_optimizer_state_dict(self, opts[0])
+        checkpoint.parse_extra(self, ckpt.get(checkpoint.EXTRA_KEY))
+        self.model.load_state_dict(weights, strict=False)
+        prepare.bump_train_version()  # the flat parameter buffer was written behind the caches' version counters
+        self._load_optimizer({"optimizer": opts[0], checkpoint.EXTRA_KEY: ckpt.get(checkpoint.EXTRA_KEY)})
+        self._recapture()
+        return {"epoch": ckpt.get("epoch", 0), "global_step": ckpt.get("global_step", self.step_count)}
 
     # -- gradient accumulation (accumulate_grad_batches = k > 1) ------------------------------------------------------
     # A window of k micro-batches: the first zeroes the gradient buffer (and the overflow flag) and fixes the loss scale;
@@ -1409,6 +1507,20 @@ class PretrainTrainer(FinetuneTrainer):
     def _task_param_ids(self, task):
         return {id(p) for n, p in zip(self.G.names, self.G.params) if n.startswith(f"loras_dict.{task}.")}
 
+    def segment_keys(self):
+        """"base" for the ControlNet's own parameters, the task for its LoRA set (active_segments)"""
+        if not self.tasks:
+            return ["base"] * len(self.G.names)
+        return [n.split(".")[1] if n.startswith("loras_dict.") else "base" for n in self.G.names]
+
+    def _alias_key(self, key):
+        """`control_model.<linear>.lora_layer.*`: the attached task's set, whose data is saved under loras_dict.<task>.*
+        (which set a file had attached, if any, does not matter on load)"""
+        return bool(self.tasks) and key.startswith("control_model.") and ".lora_layer." in key
+
+    def _captured_scales(self):
+        return [s for _, s in self._graphs.values()] + super()._captured_scales()
+
     def exchange_plan(self, segs, bucket_ranges):
         """Ranges to all-reduce after each backward bucket: the bucket's part of the ControlNet segment; the LoRA sets live
         behind it in the flat buffer and travel with the LAST bucket, and only the sets some rank trained this step (`segs`,
@@ -1465,4 +1577,5 @@ class PretrainTrainer(FinetuneTrainer):
         elif self._graphs:
             tasks = list(self._graphs)
             self._graphs.clear()
+            self._pool = None  # the freed graphs' pool cannot take new captures
             self.capture(*self._static, tasks=tasks, warmup=1)

@@ -3,11 +3,13 @@
     python tools/make_golden.py            # tiny config (committed fixture, ~300 KB)
     python tools/make_golden.py --full     # SD1.5-size eps for one image (committed fixture, ~70 KB; takes minutes)
     python tools/make_golden.py --accum    # gradient accumulation windows, finetune and pretrain (tiny config)
+    python tools/make_golden.py --resume   # AdamW state of a checkpoint and the steps after it (tiny config)
 
 The reference cannot travel to the GPU box; these fixtures can.  Weights/inputs are regenerated from names by
 oracle/synth.py, so the fixtures hold only key/shape lists and outputs.
 """
 import argparse
+import copy
 import os
 import sys
 import time
@@ -616,6 +618,93 @@ def accum(seed=0, lr=1e-3):
     print("wrote", out, os.path.getsize(out) // 1024, "KiB")
 
 
+RESUME_FT_KEEP = ("zero_convs.2.0.weight", "input_blocks.1.1.transformer_blocks.0.attn1.to_q.lora_layer.up.weight",
+                  "input_blocks.1.1.transformer_blocks.0.attn1.to_q.lora_layer.down.weight", "input_blocks.1.1.norm.weight",
+                  "input_blocks.1.1.norm.bias", "middle_block_out.0.bias")
+RESUME_PT_KEEP = ("input_blocks.0.0.weight", "input_blocks.1.0.in_layers.2.weight", "input_blocks.4.0.in_layers.2.weight",
+                  "input_blocks.4.1.transformer_blocks.0.attn1.to_q.weight", "input_blocks.1.0.in_layers.0.weight",
+                  "zero_convs.3.0.weight", "middle_block_out.0.bias",
+                  "loras_dict.canny.0.down.weight", "loras_dict.depth.5.up.weight",
+                  "loras_dict.seg.0.down.weight", "loras_dict.seg.5.up.weight")
+
+
+def resume(seed=0, lr=1e-3):
+    """The AdamW state a Lightning checkpoint holds (`optimizer_states[0]` = torch.optim.AdamW.state_dict() over the
+    parameter list configure_optimizers builds), and the steps that continue from it, with the reference's modules:
+      finetune (tiny_finetune.yaml): one step on micro-batch 0 (the trainable parameters after it and the whole
+        optimizer state dict), then a second step on micro-batch 1 (the update of the sampled tensors);
+      pretrain (tiny_pretrain.yaml): steps on [canny] then [depth] (index -> name list, which indices have state and
+        their `step`, the moments of the sampled tensors, 3x3 convs included), then a third step on [seg] (the update
+        of the sampled tensors: base at step 3, seg at step 1).
+    Gradients are cleared to None before every step, so a LoRA set no step used gets no state (AdamW skips it)."""
+    B, H = 2, 16
+    ts = [[981, 21], [500, 250], [37, 760]]
+
+    def micro(i):
+        mk = lambda n, s: synth.synth_input(f"{n}_acc{i}", s, seed)
+        return dict(x=mk("x", (B, 4, H, H)), hint=mk("hint", (B, 4, H, H)), ctx=mk("ctx", (B, 77, 64)),
+                    noise=mk("noise", (B, 4, H, H)), t=torch.tensor(ts[i], dtype=torch.long))
+
+    def step(model, opt, i, task=None):
+        model.encode_first_stage = lambda h: h
+        model.get_first_stage_encoding = lambda h: h
+        opt.zero_grad(set_to_none=True)
+        d = micro(i)
+        cond = {"c_crossattn": [d["ctx"]], "c_concat": [d["hint"]]}
+        if task is not None:
+            cond["task"] = task
+        x_noisy = model.q_sample(x_start=d["x"], t=d["t"], noise=d["noise"])
+        eps = model.apply_model(x_noisy, d["t"], cond)
+        loss = model.get_loss(eps, d["noise"], mean=False).mean([1, 2, 3]).mean()
+        loss.backward()
+        opt.step()
+        return loss.detach().clone()
+
+    g = {"seed": seed, "B": B, "H": H, "t": torch.tensor(ts), "lr": lr}
+    # ---------------- finetune
+    model = build_reference(os.path.join(GOLD, "tiny_finetune.yaml"), seed)
+    cn = model.control_model
+    names = [n for n, _ in cn.named_parameters()
+             if "lora_layer" in n or "zero_convs" in n or "middle_block_out" in n or "norm" in n]
+    named = dict(cn.named_parameters())
+    opt = torch.optim.AdamW([named[n] for n in names], lr=lr)
+    ft = {"control_shapes": shapes_of(cn), "unet_shapes": shapes_of(model.model.diffusion_model),
+          "trainable_names": names}
+    ft["loss1"] = step(model, opt, 0)
+    sd = copy.deepcopy(opt.state_dict())  # state_dict() holds the live tensors: the next step would update them
+    ft["param_groups1"] = sd["param_groups"]
+    # whole-set entries live at the top level, where save_golden splits a dict entry by entry into part files
+    g["ft_params1"] = {n: named[n].detach().clone() for n in names}
+    g["ft_state1"] = sd["state"]  # optimizer_states[0]["state"] of a checkpoint taken after step 1
+    ft["loss2"] = step(model, opt, 1)
+    ft["after2"] = {n: named[n].detach().clone() for n in RESUME_FT_KEEP}
+    g["finetune"] = ft
+    # ---------------- pretrain
+    model = build_reference(os.path.join(GOLD, "tiny_pretrain.yaml"), seed)
+    cn = model.control_model
+    shapes = shapes_of(cn)  # before switch_lora attaches a set
+    params = list(cn.parameters())  # configure_optimizers (cldm_ctrlora_pretrain.py:174-182), before any switch_lora
+    name_of = {id(p): n for n, p in cn.named_parameters()}
+    index_names = [name_of[id(p)] for p in params]
+    opt = torch.optim.AdamW(params, lr=lr)
+    by_name = dict(zip(index_names, params))
+    pt = {"control_shapes": shapes, "index_names": index_names}
+    pt["losses"] = torch.stack([step(model, opt, 0, "canny"), step(model, opt, 1, "depth")])
+    sd = copy.deepcopy(opt.state_dict())
+    pt["steps"] = {i: int(s["step"]) for i, s in sd["state"].items()}
+    pt["param_group"] = {k: v for k, v in sd["param_groups"][0].items() if k != "params"}
+    pt["moments"] = {n: {k: sd["state"][index_names.index(n)][k].clone() for k in ("exp_avg", "exp_avg_sq")}
+                     for n in RESUME_PT_KEEP if index_names.index(n) in sd["state"]}
+    pt["before3"] = {n: by_name[n].detach().clone() for n in RESUME_PT_KEEP}
+    pt["loss3"] = step(model, opt, 2, "seg")
+    pt["after3"] = {n: by_name[n].detach().clone() for n in RESUME_PT_KEEP}
+    pt["steps3"] = {i: int(s["step"]) for i, s in opt.state_dict()["state"].items()}
+    g["pretrain"] = pt
+    out = os.path.join(GOLD, "tiny_resume_golden.pt")
+    save_golden(g, out)
+    print("wrote", out, os.path.getsize(out) // 1024, "KiB")
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--accum", action="store_true")
@@ -627,6 +716,7 @@ if __name__ == "__main__":
     ap.add_argument("--vae", action="store_true")
     ap.add_argument("--vae-full", action="store_true")
     ap.add_argument("--style", action="store_true")
+    ap.add_argument("--resume", action="store_true")
     a = ap.parse_args()
     torch.set_num_threads(os.cpu_count())
     if a.full:
@@ -647,5 +737,7 @@ if __name__ == "__main__":
         style()
     elif a.accum:
         accum()
+    elif a.resume:
+        resume()
     else:
         tiny()
