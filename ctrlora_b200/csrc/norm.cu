@@ -689,6 +689,103 @@ gn_bwd_stats_kernel(GnSrc s, const __half* __restrict__ dy, int C, int HW, int g
     }
 }
 
+// Deterministic form of gn_bwd_stats_kernel (used whenever the caller provides a partial workspace), the backward twin of
+// gn_stats_det_kernel: per-lane channel sums reduced through shared memory in lane order, one per-group partial per block
+// (no atomics), and the last block of an image to arrive adds the partials up in block order.  bstats -- and with them every
+// dx the apply kernel writes -- are then bit-reproducible; dgamma/dbeta still accumulate with fp32 atomics (one per
+// channel per block): they feed only the fp32 gradient buffer, never an fp16 activation.
+__global__ void __launch_bounds__(512)
+gn_bwd_stats_det_kernel(GnSrc s, const __half* __restrict__ dy, int C, int HW, int groups, int pix_per_block,
+                        const float* __restrict__ fstats, const float* __restrict__ gamma, const float* __restrict__ beta,
+                        float eps, int silu, float* __restrict__ bstats, float* __restrict__ dgamma, float* __restrict__ dbeta,
+                        float* __restrict__ partial, unsigned int* __restrict__ counters) {
+    pdl_launch_dependents();
+    pdl_wait();
+    extern __shared__ float sm[];  // [lanes][2][C] scratch, then [2][C] channel sums (dz, dz*xhat)
+    __shared__ int is_last;
+    const int b = blockIdx.y;
+    const int vecs = C >> 3, lanes = blockDim.x / vecs;  // blockDim.x == vecs * lanes exactly
+    const int vec = threadIdx.x % vecs, pl = threadIdx.x / vecs;
+    float* c_dz = sm + static_cast<size_t>(lanes) * 2 * C;
+    float* c_dzx = c_dz + C;
+    const int cpg = C / groups;
+    const float inv_n = 1.0f / (static_cast<float>(cpg) * HW);
+    float mu[8], rs[8], ga[8], be[8], a[8], q[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+        const int c = vec * 8 + e, g = c / cpg;
+        const float mean = fstats[(b * groups + g) * 2] * inv_n;
+        const float var = fmaxf(fstats[(b * groups + g) * 2 + 1] * inv_n - mean * mean, 0.f);
+        mu[e] = mean; rs[e] = rsqrtf(var + eps); ga[e] = gamma[c]; be[e] = beta[c]; a[e] = 0.f; q[e] = 0.f;
+    }
+    const int p0 = blockIdx.x * pix_per_block, p1 = min(HW, p0 + pix_per_block);
+    auto accum = [&](const float* x, const float* d) {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+            const float xh = (x[e] - mu[e]) * rs[e];
+            const float dz = silu ? d[e] * dsilu_f(xh * ga[e] + be[e]) : d[e];
+            a[e] += dz; q[e] += dz * xh;
+        }
+    };
+    int p = p0 + pl;
+    for (; p + lanes < p1; p += 2 * lanes) {  // two pixels (four 16-byte loads) in flight per thread
+        const long long pix = static_cast<long long>(b) * HW + p;
+        float x0[8], d0[8], x1[8], d1[8];
+        load8(s, pix, vec * 8, x0);
+        load8h(dy + pix * C + vec * 8, d0);
+        load8(s, pix + lanes, vec * 8, x1);
+        load8h(dy + (pix + lanes) * C + vec * 8, d1);
+        accum(x0, d0);
+        accum(x1, d1);
+    }
+    for (; p < p1; p += lanes) {
+        const long long pix = static_cast<long long>(b) * HW + p;
+        float x[8], d[8];
+        load8(s, pix, vec * 8, x);
+        load8h(dy + pix * C + vec * 8, d);
+        accum(x, d);
+    }
+    float* sp = sm + static_cast<size_t>(pl) * 2 * C + vec * 8;
+    *reinterpret_cast<float4*>(sp) = make_float4(a[0], a[1], a[2], a[3]);
+    *reinterpret_cast<float4*>(sp + 4) = make_float4(a[4], a[5], a[6], a[7]);
+    *reinterpret_cast<float4*>(sp + C) = make_float4(q[0], q[1], q[2], q[3]);
+    *reinterpret_cast<float4*>(sp + C + 4) = make_float4(q[4], q[5], q[6], q[7]);
+    __syncthreads();
+    for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) {
+        float t = 0.f;
+        for (int l = 0; l < lanes; ++l) t += sm[static_cast<size_t>(l) * 2 * C + i];
+        c_dz[i] = t;  // i >= C lands in c_dzx
+    }
+    __syncthreads();
+    const int nblk = gridDim.x;
+    float* mine = partial + (static_cast<size_t>(b) * nblk + blockIdx.x) * groups * 2;
+    for (int g = threadIdx.x; g < groups; g += blockDim.x) {
+        float g1 = 0.f, g2 = 0.f;
+        for (int c = g * cpg; c < (g + 1) * cpg; ++c) { g1 += gamma[c] * c_dz[c]; g2 += gamma[c] * c_dzx[c]; }
+        mine[2 * g] = g1;
+        mine[2 * g + 1] = g2;
+    }
+    if (dgamma) {
+        for (int c = threadIdx.x; c < C; c += blockDim.x) { atomicAdd(&dgamma[c], c_dzx[c]); atomicAdd(&dbeta[c], c_dz[c]); }
+    }
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        const unsigned int old = atomicAdd(&counters[b], 1u);
+        is_last = (old == static_cast<unsigned int>(nblk - 1));
+        if (is_last) counters[b] = 0;  // self-cleaning: ready for the next launch
+    }
+    __syncthreads();
+    if (!is_last) return;
+    __threadfence();
+    for (int i = threadIdx.x; i < 2 * groups; i += blockDim.x) {
+        float t = 0.f;
+        const float* src = partial + static_cast<size_t>(b) * nblk * groups * 2 + i;
+        for (int k = 0; k < nblk; ++k) t += __ldcg(src + static_cast<size_t>(k) * groups * 2);  // block order: fixed
+        bstats[b * groups * 2 + i] = t;
+    }
+}
+
 __global__ void __launch_bounds__(512)
 gn_bwd_apply_kernel(GnSrc s, const __half* __restrict__ dy, int C, int HW, int groups, int pix_per_block,
                     const float* __restrict__ fstats, const float* __restrict__ bstats, const float* __restrict__ gamma,
@@ -883,9 +980,6 @@ extern "C" int ctrlora_groupnorm_bwd_f16(const ctrlora_groupnorm_args* a, const 
     s.x2 = reinterpret_cast<const __half*>(a->x2); s.add2 = reinterpret_cast<const __half*>(a->add2); s.s2 = a->add2_scale;
     s.c2 = a->x2 ? a->c2 : 0; s.ld2 = a->ld2;
     const int HW = a->hw, B = a->batch;
-    if (!a->stats_prezeroed &&
-        cudaMemsetAsync(a->stats_ws, 0, sizeof(float) * 2 * B * a->groups, stream) != cudaSuccess)
-        return CTRLORA_ERR_CUDA;
     int chunks = (592 + B - 1) / B;
     int ppb = (HW + chunks - 1) / chunks;
     if (ppb < 8) ppb = 8;
@@ -894,7 +988,18 @@ extern "C" int ctrlora_groupnorm_bwd_f16(const ctrlora_groupnorm_args* a, const 
     const int vecs = C / 8;
     const int lanes = vecs >= 256 ? 1 : 256 / vecs;
     const int threads = vecs * lanes;
-    if (a->stats_prezeroed)
+    const bool det = a->partial_ws && a->partial_counters && B <= a->partial_counters_len &&
+                     static_cast<long long>(B) * chunks * a->groups * 2 <= a->partial_ws_floats &&
+                     (lanes + 1) * 2 * C * sizeof(float) <= 48 * 1024;
+    if (!det && !a->stats_prezeroed &&
+        cudaMemsetAsync(a->stats_ws, 0, sizeof(float) * 2 * B * a->groups, stream) != cudaSuccess)
+        return CTRLORA_ERR_CUDA;
+    if (det)
+        launch_pdl(gn_bwd_stats_det_kernel, grid, dim3(threads), (size_t)((lanes + 1) * 2 * C * sizeof(float)), stream, s,
+                   reinterpret_cast<const __half*>(dy), C, HW, (int)a->groups, ppb, reinterpret_cast<const float*>(fwd_stats),
+                   a->gamma, a->beta, a->eps, (int)a->silu, reinterpret_cast<float*>(a->stats_ws), dgamma, dbeta,
+                   a->partial_ws, a->partial_counters);
+    else if (a->stats_prezeroed)
         launch_pdl(gn_bwd_stats_kernel, grid, dim3(threads), (size_t)(2 * C * sizeof(float)), stream, s,
                    reinterpret_cast<const __half*>(dy), C, HW, (int)a->groups, ppb, reinterpret_cast<const float*>(fwd_stats),
                    a->gamma, a->beta, a->eps, (int)a->silu, reinterpret_cast<float*>(a->stats_ws), dgamma, dbeta);

@@ -607,6 +607,10 @@ def groupnorm_bwd(dy, fwd_stats, x1, gamma, beta, eps, silu, *, add1=None, add1_
     ws, prezeroed = _stats_take(dy.device, fwd_stats.numel())
     a, (b, h, w, c1, c2) = _gn_args(x1, gamma, beta, eps, silu, add1, add1_scale, x2, add2, add2_scale, groups, ws)
     a.stats_prezeroed = prezeroed
+    if not torch.cuda.is_current_stream_capturing() or dy.device.index in _GN_PARTIAL or torch.cuda.current_device() in _GN_PARTIAL:
+        pws, pcnt = _gn_partial_buffers(dy.device)  # the forward's scratch: bit-reproducible dx (never first allocated in a capture)
+        a.partial_ws, a.partial_ws_floats = _dp(pws), GN_PARTIAL_FLOATS
+        a.partial_counters, a.partial_counters_len = _dp(pcnt), GN_PARTIAL_COUNTERS
     dx1 = torch.empty((b, h, w, c1), device=dy.device, dtype=torch.float16)
     dx2 = torch.empty((b, h, w, c2), device=dy.device, dtype=torch.float16) if (want_dx2 and c2) else None
     _count(2)

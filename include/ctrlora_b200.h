@@ -104,9 +104,10 @@ typedef struct ctrlora_groupnorm_args {
     void* stats_ws;   /* fp32 workspace [batch * groups * 2] */
     int stats_prezeroed; /* 1: the caller guarantees stats_ws is zero on entry (e.g. one memset per step over an arena of
                             workspaces): no memset node in front of the statistics kernel, which is then PDL-chained */
-    float* partial_ws;   /* forward only, optional: scratch for per-block partial statistics (any contents).  With it the
-                            forward is bit-reproducible: no fp32 atomics, the last block of an image sums the partials in a
-                            fixed order.  NULL: round-1 behaviour (atomic accumulation into stats_ws). */
+    float* partial_ws;   /* optional: scratch for per-block partial statistics (any contents).  With it the forward and the
+                            backward's dx are bit-reproducible: no fp32 atomics in the statistics, the last block of an image
+                            sums the partials in a fixed order (the backward's dgamma/dbeta still accumulate atomically).
+                            NULL: round-1 behaviour (atomic accumulation into stats_ws). */
     long long partial_ws_floats;
     unsigned int* partial_counters;   /* [>= batch] arrival counters: all zero on entry, left all zero on exit */
     int partial_counters_len;

@@ -182,12 +182,21 @@ def test_wgrad_direct_and_reduce_paths(m, p, q, ldo_extra, alpha, beta):
     assert err < 3e-5, err  # fp32 tensor-core accumulation over up to 32768 tokens (measured <= 7.8e-6)
 
 
+COLSUM_CASES = [(32768, 320, 320, torch.float16), (2048, 1280, 1280, torch.float16), (8192, 640, 1920, torch.float16),
+                (77, 328, 328, torch.float16), (512, 8, 8, torch.float16),
+                # fp32 input: the time-embedding MLP's bias gradients (rows = batch; emb_layers read a column slice of the
+                # [B, 9600] d(rowbias) buffer), and a tall / ragged form of the same instance
+                (2, 1280, 1280, torch.float32), (2, 320, 9600, torch.float32), (4096, 1280, 1280, torch.float32),
+                (77, 1000, 1003, torch.float32)]
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize("rows,cols,ld", [(32768, 320, 320), (2048, 1280, 1280), (8192, 640, 1920), (77, 328, 328), (512, 8, 8)])
-def test_colsum_vector_path(rows, cols, ld):
+@pytest.mark.parametrize("rows,cols,ld,dtype", COLSUM_CASES,
+                         ids=[f"{r}-{c}-{ld}" + ("-fp32" if dt == torch.float32 else "") for r, c, ld, dt in COLSUM_CASES])
+def test_colsum_vector_path(rows, cols, ld, dtype):
     from ctrlora_b200 import ops
     g = torch.Generator(device="cuda").manual_seed(rows)
-    x = torch.randn(rows, ld, device="cuda", generator=g).half()[:, :cols]
+    x = torch.randn(rows, ld, device="cuda", generator=g).to(dtype)[:, :cols]
     out = torch.ones(cols, device="cuda")
     ops.colsum(x, out, scale=0.25)
     ref = 1.0 + 0.25 * x.double().sum(0)

@@ -31,6 +31,15 @@ TOL = {
     "sd15_loss": 1e-4,           # training loss
     "sd15_grad_norm": 1.2e-3,    # worst of the 246 gradient norms
     "sd15_grad_tensor": 2.3e-3,  # worst of the full gradient tensors kept in the golden
+    # training backward per SD1.5 block (test_train_blocks_gpu.py, B = 2, 64x64, vs fp32 autograd of the oracle): a block is
+    # a handful of fp16 roundings of activations and gradients, so bounds of a few 1e-3
+    "sd15_blk_dx": 1.1e-3,       # input gradients of ControlNet / decoder blocks and of the out head (worst: middle_block)
+    "sd15_blk_demb": 1.15e-3,    # d(emb) of a block, its d(rowbias) mapped through the emb_layers in fp32
+    "sd15_blk_grad": 2e-3,       # every sink gradient of a block, finetune and pretrain (worst: LoRA of the middle block's
+                                 # self-attention)
+    "sd15_emb_mlp_grad": 5.2e-4,  # time_embed / emb_layers gradients of emb_mlp_backward
+    "sd15_pt_grad_tensor": 4.3e-3,  # full pretrain step: worst of the 488 base and active-LoRA gradient tensors (the whole
+                                    # network's fp16 roundings, like sd15_grad_tensor)
     "vae_encode": 2e-3,          # first-stage VAE moments, tiny and SD VAE at 512x512
     "vae_decode": 3.5e-3,        # tiny decode, encode->decode round trip, SD VAE decode
 }
