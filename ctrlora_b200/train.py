@@ -20,6 +20,7 @@ micro-batch; k calls form a window whose gradients add into the flat buffer and 
 micro-batch, before one AdamW step with grad_scale 1 / (world * loss scale * k).  flush() applies a partial window.
 """
 import numbers
+import os
 
 import torch
 import torch.nn as nn
@@ -426,7 +427,7 @@ def down_bwd(ds, s, d_out, G=None):
     if G is not None:
         dense_conv_grads(ds.op, None, pixel_major(d_out), G, col=s["col"])
     # builders read their inputs through the caches (never a tensor fetched earlier): a recorded builder re-run inside a
-    # preparation graph (FinetuneTrainer._capture_window) must derive from the current parameters
+    # preparation graph (FinetuneTrainer._capture_prep) must derive from the current parameters
     wk = lambda: _cache(ds).get("w", [ds.op.weight], lambda: prepare.conv_weight(ds.op.weight).view(ds.out_channels, 1, 9 * c))
     wt = _cache(ds).get("wT", [ds.op.weight], lambda: prepare.weight_T(wk()))
     d_col = ops.gemm(pixel_major(d_out), wt)  # [B, h/2, w/2, 9*C]
@@ -682,25 +683,29 @@ def unet_bwd(unet, saved, d_eps16):
 class FinetuneTrainer:
     """One data-parallel CtrLoRA finetune step per call (configs ctrlora_finetune_sd15_rank*.yaml)."""
 
+    tasks = ()  # finetuning trains one LoRA set: no task to switch (PretrainTrainer: the ControlNet's tasks)
+
     def __init__(self, model, lr=1e-5, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.01, process_group=None,
-                 loss_scale=None, dynamic_loss_scale=True, accumulate_grad_batches=1):
+                 loss_scale=None, dynamic_loss_scale=True, accumulate_grad_batches=1, *, named=None):
+        """named: the optimizer's parameter set, [(name, parameter)] as GradSink takes it; default: the finetune filter"""
         self._init_window(accumulate_grad_batches)
         self.model = model
         self.cn = model.control_model
         self.unet = model.model.diffusion_model
-        self.G = GradSink(self.cn)
+        self.G = GradSink(self.cn, named=named)
         self.lr, self.betas, self.eps, self.wd = lr, betas, eps, weight_decay
         self.pg = process_group
-        self.world = 1
+        self.world, self.rank = 1, 0
         if torch.distributed.is_available() and torch.distributed.is_initialized():
             self.world = torch.distributed.get_world_size(process_group)
+            self.rank = torch.distributed.get_rank(process_group)
         if self.world > 1:
             # DDP's construction-time rank-0 broadcast (the reference relies on it: LoRA `down` is initialised
             # N(0, 1/r) without a seed, cldm/lora.py:67): every replica starts from rank 0's trainable parameters
             torch.distributed.broadcast(self.G.flat_p, src=0, group=process_group)
             prepare.bump_train_version()
         self.step_count = 0
-        self.seg_steps = {}        # per-segment AdamW step counts
+        self.seg_steps = {}        # per-segment AdamW step counts (torch keeps `step` per parameter)
         # Loss scaling (the backward's activation gradients are fp16; the reference trains in fp32 and needs none):
         # d(loss)/d(eps) = 2 (eps - noise) / numel is ~1e-5 at batch 16 x 4 x 64 x 64 -- below fp16's normal range.  The
         # default scale makes it (eps - noise) / LOSS_SCALE_DIV independent of the batch shape; the AdamW kernel divides
@@ -711,6 +716,10 @@ class FinetuneTrainer:
         self.overflow_flag = torch.zeros(1, device=dev, dtype=torch.int32)
         self.skipped_steps = 0
         self._init_step_state(dev)
+        self._graphs = None        # capture(): {"prep": {owner: graph}, "compute": {task: (graph(s), loss, scale)}}
+        self._static = None        # the captured graphs' inputs
+        self._on_stage = None      # backward-stage callback (the overlapped exchange)
+        self._comm = None          # stream of the overlapped all-reduces
 
     LOSS_SCALE_DIV = 8.0
     CHECK_OVERFLOW_EVERY = 16   # host polls the device-side skipped-steps counter this often (no per-step sync)
@@ -723,7 +732,6 @@ class FinetuneTrainer:
         self.accumulate_grad_batches = int(k)
         self.micro_step = 0
         self._window_tasks = []
-        self._accum = None         # graphs of the accumulating path (capture with k > 1)
 
     def _init_step_state(self, dev):
         """AdamW's step counter lives on the device (ops.adamw_begin): a step skipped for a non-finite gradient does not
@@ -757,11 +765,15 @@ class FinetuneTrainer:
     def _scale_for(self, numel):
         return float(self.loss_scale) if self.loss_scale is not None else numel / (2.0 * self.LOSS_SCALE_DIV)
 
-    def loss_and_grads(self, x0, hint_latent, context, t, noise, accumulate=False):
+    def loss_and_grads(self, x0, hint_latent, context, t, noise, task=None, accumulate=False):
         """q_sample -> apply_model -> MSE -> backward into the flat gradient buffer.  Returns the loss (fp32 tensor).
+        task: the LoRA set to attach first, when the trainer has tasks (None keeps the attached one).
         accumulate: add to the gradients already in the buffer (a continuing micro-batch of a window) and keep the window's
         loss scale and overflow flag; otherwise the buffer and the flag are zeroed first."""
         m = self.model
+        if task is not None and self.tasks:
+            self.cn.switch_lora(task)
+            self.task = task
         if not accumulate:
             self.G.zero()
             self.overflow_flag.zero_()
@@ -775,7 +787,7 @@ class FinetuneTrainer:
             d_ctrl = unet_bwd(self.unet, un_saved, d_eps)
             if m.only_mid_control:
                 d_ctrl = [d if d is not None else torch.zeros_like(c) for d, c in zip(d_ctrl, control)]
-            controlnet_bwd(self.cn, cn_saved, d_ctrl, self.G, on_stage=getattr(self, "_on_stage", None))
+            controlnet_bwd(self.cn, cn_saved, d_ctrl, self.G, on_stage=self._on_stage)
         finally:
             ops.stats_arena_end(x0.device)
         self.last_eps = eps
@@ -789,6 +801,12 @@ class FinetuneTrainer:
     # -- the exchange step: all-reduce (SUM) of the flat trainable-gradient buffer (36.9 M fp32 elements for rank 128 =
     # 148 MB; the reference's DDP reduces ~10x more, SURVEY.md §0.7), split into buckets that follow the backward's order so
     # all but the last one overlap the remaining ControlNet backward.  1/world is folded into the AdamW kernel.
+    STAGES = ("middle",) + tuple(STAGE_AFTER_BLOCK.values())  # backward stages that can close a bucket, in order
+    # The active cuts come from the environment variable CUTS_ENV, default CUTS_DEFAULT (_overlap_cuts).  Finetuning:
+    # none by default: every cut splits the CUDA graph and the collective's CTAs compete with the backward it overlaps,
+    # which pays only for collectives longer than the finetune step's (more ranks, multi-node).
+    CUTS_ENV, CUTS_DEFAULT = "CTRLORA_ALLREDUCE_CUTS", ""
+
     def gradient_buckets(self):
         """{stage: [(offset, numel)]}: contiguous flat-buffer ranges whose gradients are final when the backward reaches
         the stage (a block's zero-conv travels with its block); "final" is the rest: input_blocks.0-2 with their zero-convs and
@@ -803,12 +821,12 @@ class FinetuneTrainer:
                 return "middle"
             if n.startswith(("input_blocks.", "zero_convs.")):
                 i = int(n.split(".")[1])
-                for b0, st in ((9, "ib9"), (6, "ib6"), (3, "ib3")):
+                for b0, st in STAGE_AFTER_BLOCK.items():
                     if b0 <= i < b0 + 3:
                         return st
             return "final"
 
-        buckets = {k: [] for k in ("middle", "ib9", "ib6", "ib3", "final")}
+        buckets = {k: [] for k in self.STAGES + ("final",)}
         for name in self.G.names:
             off, n = self.G.offsets[name]
             r = buckets[stage_of(name)]
@@ -818,21 +836,20 @@ class FinetuneTrainer:
                 r.append((off, n))
         return buckets
 
-    def _overlap(self):
-        return bool(self._cuts())
-
-    def _cuts(self):
-        """Backward stages after which a gradient bucket is closed and its all-reduce started (CTRLORA_ALLREDUCE_CUTS, comma
-        separated subset of middle,ib9,ib6,ib3; empty = one all-reduce after the backward).  Default: EMPTY: every cut splits
-        the CUDA graph and the collective's CTAs compete with the backward it overlaps, which pays only for collectives
-        longer than the finetune step's (more ranks, multi-node)."""
-        import os
+    def _overlap_cuts(self):
+        """Backward stages after which a gradient bucket is closed and its all-reduce started, in backward order:
+        `allreduce_cuts` when set, else the environment variable CUTS_ENV (default CUTS_DEFAULT); a comma-separated subset
+        of middle,ib9,ib6,ib3, empty = one all-reduce after the backward."""
         cuts = getattr(self, "allreduce_cuts", None)
         if cuts is None:
-            cuts = os.environ.get("CTRLORA_ALLREDUCE_CUTS", "")
+            cuts = os.environ.get(self.CUTS_ENV, self.CUTS_DEFAULT)
         if isinstance(cuts, str):
             cuts = [c for c in cuts.split(",") if c]
-        return [c for c in ("middle", "ib9", "ib6", "ib3") if c in cuts]
+        return [c for c in self.STAGES if c in cuts]
+
+    def _segmented(self):
+        """the exchange overlaps the backward: one graph per gradient bucket, each bucket reduced after its stage"""
+        return self.world > 1 and bool(self._overlap_cuts())
 
     def merged_buckets(self):
         """[(stage, ranges)] in backward order for the active cuts + ("final", ranges): buckets of skipped stages are merged
@@ -847,8 +864,8 @@ class FinetuneTrainer:
             return out
 
         b = self.gradient_buckets()
-        cuts, out, pending = self._cuts(), [], []
-        for st in ("middle", "ib9", "ib6", "ib3"):
+        cuts, out, pending = self._overlap_cuts(), [], []
+        for st in self.STAGES:
             pending += b[st]
             if st in cuts:
                 out.append((st, coalesce(pending)))
@@ -856,11 +873,24 @@ class FinetuneTrainer:
         out.append(("final", coalesce(pending + b["final"])))
         return out
 
+    def exchange_plan(self, segs, bucket_ranges):
+        """Ranges to all-reduce after each backward bucket, for a window's segments `segs` (window_segments): the bucket's
+        part of the dense first segment ("all" / "base", at offset 0); the other segments (pretraining's LoRA sets, which
+        live behind it in the flat buffer) travel with the LAST bucket.  Every element of `segs` appears exactly once in
+        the plan."""
+        dense_end = segs[0][1]
+        rest = [(off, n) for off, n, _ in segs[1:]]
+        plan = []
+        for i, ranges in enumerate(bucket_ranges):
+            r = [(off, min(n, dense_end - off)) for off, n in ranges if off < dense_end]
+            plan.append(r + rest if i == len(bucket_ranges) - 1 else r)
+        return plan
+
     def _reduce_ranges(self, ranges):
         """all-reduce `ranges` on the communication stream once everything enqueued so far on the compute stream is done"""
         if self.world <= 1 or not ranges:
             return
-        if getattr(self, "_comm", None) is None:
+        if self._comm is None:
             self._comm = torch.cuda.Stream()
         ev = torch.cuda.Event()
         ev.record()
@@ -870,103 +900,146 @@ class FinetuneTrainer:
                 torch.distributed.all_reduce(self.G.flat_g[off:off + n], group=self.pg)
 
     def reduce_gradients(self, ranges=None):
-        """Un-overlapped form (also what the CPU/gloo test drives): one all-reduce per range, whole buffer by default."""
+        """Un-overlapped form (also what the CPU/gloo tests drive): one all-reduce per (offset, numel) range, whole buffer
+        by default."""
         if self.world > 1:
             for off, n in (ranges or [(0, self.G.numel)]):
                 torch.distributed.all_reduce(self.G.flat_g[off:off + n], group=self.pg)
 
     # -- CUDA-graph replay of forward + backward (≈3 000 launches per step; Python cannot enqueue them fast enough)
-    def capture(self, x0, hint_latent, context, t, noise, warmup=2):
-        """Capture loss_and_grads for these shapes.  The LoRA folds / transposes of the trainable parameters are part
-        of the graph (they must re-run every step), the frozen-weight copies are built during warm-up and are not.
-        With accumulate_grad_batches > 1 the graphs of the accumulating path are captured instead (_capture_window)."""
+    def capture(self, x0, hint_latent, context, t, noise, tasks=None, warmup=2):
+        """Capture the step for these shapes: one compute graph per task (`tasks`: default every task of the trainer;
+        finetuning's only task is None; the attached LoRA set is baked into the captured kernels' pointers), all in one
+        memory pool -- only one of them is ever in flight.  A call replaces everything captured before: the inputs are
+        cloned again and the earlier graphs dropped, so a re-capture passes every captured task.
+          * k = 1: the trainable-weight copies (LoRA folds, fp16 / transposed / dgrad copies) are rebuilt inside the
+            compute graph (they must re-run every step); the frozen-weight copies are built during warm-up and are not.
+          * k > 1 (accumulate_grad_batches): the compute graph adds one micro-batch into the buffer, and the trainable
+            copies are rebuilt once per window by preparation graphs (_capture_prep).
+        A compute graph is one graph, or one per gradient bucket when the exchange overlaps the backward (_segmented)."""
+        self._graphs = None
         self._static = [v.clone() for v in (x0, hint_latent, context, t, noise)]
-        if self.accumulate_grad_batches > 1:
-            return self._capture_window([None], warmup)
+        tasks = list(tasks or self.tasks or [None])
+        accumulate = self.accumulate_grad_batches > 1
         cur = torch.cuda.current_stream()
-        side = torch.cuda.Stream()
-        side.wait_stream(cur)
-        with torch.cuda.stream(side):
-            for _ in range(warmup):
-                self.loss_and_grads(*self._static)
-        cur.wait_stream(side)
-        torch.cuda.synchronize()
-        prepare.bump_train_version()  # force the trainable-weight preparation into the captured region
-        self._segments = None
-        if self.world > 1 and self._overlap():
-            # one graph per gradient bucket, sharing a memory pool: replay k, start bucket k's all-reduce on the
-            # communication stream, replay k+1 ...  (NCCL stays outside the captures)
-            merged = self.merged_buckets()
-            buckets = dict(merged)
-            segs, state = [], {}
-            stream = torch.cuda.Stream()
-            stream.wait_stream(cur)
-            with torch.cuda.stream(stream):
-                state["g"] = torch.cuda.CUDAGraph()
-                state["g"].capture_begin()
+        logs, compute, pool = {}, {}, None
 
-                def on_stage(name):
-                    if name not in buckets:
-                        return  # not an active cut
-                    state["g"].capture_end()
-                    segs.append((state["g"], buckets[name]))
-                    state["g"] = torch.cuda.CUDAGraph()
-                    state["g"].capture_begin(pool=segs[0][0].pool())
+        def capture_compute(task):
+            nonlocal pool
+            g, loss, pool = self._capture_compute(
+                lambda: self.loss_and_grads(*self._static, task=task, accumulate=accumulate), pool)
+            compute[task] = (g, loss, self._scale_used)
 
-                self._on_stage = on_stage
-                try:
-                    self._static_loss = self.loss_and_grads(*self._static)
-                finally:
-                    self._on_stage = None
-                state["g"].capture_end()
-                segs.append((state["g"], buckets["final"]))
-            cur.wait_stream(stream)
-            self._segments = segs
-            self._graph = segs[0][0]
-            return self
-        self._graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self._graph):
-            self._static_loss = self.loss_and_grads(*self._static)
+        for task in tasks:
+            side = torch.cuda.Stream()
+            side.wait_stream(cur)
+            with torch.cuda.stream(side):
+                for _ in range(warmup - 1 if accumulate else warmup):
+                    self.loss_and_grads(*self._static, task=task)
+                if accumulate:  # which copies a micro-batch reads, for the preparation graphs
+                    prepare.bump_train_version()
+                    with prepare.record_builds() as logs[task]:
+                        self.loss_and_grads(*self._static, task=task)
+            cur.wait_stream(side)
+            if not accumulate:
+                torch.cuda.synchronize()
+                prepare.bump_train_version()  # force the trainable-weight preparation into the captured region
+                capture_compute(task)
+        prep = {}
+        if accumulate:
+            torch.cuda.synchronize()
+            prep = self._capture_prep(tasks, logs)
+            for task in tasks:
+                capture_compute(task)
+        self._graphs = {"prep": prep, "compute": compute}
         return self
 
-    def loss_and_grads_graphed(self, x0, hint_latent, context, t, noise):
-        for dst, src in zip(self._static, (x0, hint_latent, context, t, noise)):
-            if dst.data_ptr() != src.data_ptr():
-                dst.copy_(src, non_blocking=True)
-        if self._segments:
-            for g, ranges in self._segments:
-                g.replay()
-                self._reduce_ranges(ranges)
-        else:
-            self._graph.replay()
-        return self._static_loss
+    def _capture_prep(self, tasks, logs):
+        """Preparation graphs of the accumulating path, from the copies each task's warm-up read (`logs`):
+          * prep[None]: zero the gradient buffer and the overflow flag, rebuild every trainable-weight copy that does not
+            depend on a task's LoRA set -- replayed at a window's start;
+          * prep[task] (pretraining): rebuild the copies that depend on the task's LoRA set -- replayed on the task's first
+            micro-batch in a window (a window mixes tasks, so not every fold can be built at its start).
+        Each has a memory pool of its own, so no other graph's scratch can overwrite the copies it keeps."""
+        builds, seen = {None: []}, set()
+        for task in tasks:
+            own = {id(p) for n, p in zip(self.G.names, self.G.params) if n.startswith(f"loras_dict.{task}.")}
+            builds.setdefault(task, [])
+            for entry in logs[task]:
+                cache, key, params, _ = entry
+                ps = [p for p in params if p is not None]
+                if not any(getattr(p, "_ctrlora_trainable", False) for p in ps):
+                    continue  # frozen copies are built once and never change
+                owner = task if any(id(p) in own for p in ps) else None
+                if (owner, id(cache), key) not in seen:
+                    seen.add((owner, id(cache), key))
+                    builds[owner].append(entry)
+
+        prepare.bump_train_version()  # every recorded copy is rebuilt inside its prep graph
+        prep = {}
+        for owner, entries in builds.items():
+            if owner is not None and not entries:
+                continue
+            if owner is not None:
+                self.cn.switch_lora(owner)
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                if owner is None:
+                    self.G.zero()
+                    self.overflow_flag.zero_()
+                for cache, key, params, builder in entries:
+                    cache.get(key, params, builder)
+            prep[owner] = g
+        return prep
+
+    def _capture_compute(self, run, pool):
+        """graph of run() in `pool`; one graph per gradient bucket when _segmented()"""
+        kw = {} if pool is None else {"pool": pool}
+        if not self._segmented():
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, **kw):
+                loss = run()
+            return g, loss, g.pool() if pool is None else pool
+        # replay k, start bucket k's all-reduce on the communication stream, replay k+1 ... (NCCL stays outside the
+        # captures)
+        buckets = dict(self.merged_buckets())
+        cur = torch.cuda.current_stream()
+        segs, state = [], {"pool": pool}
+        stream = torch.cuda.Stream()
+        stream.wait_stream(cur)
+        with torch.cuda.stream(stream):
+            state["g"] = torch.cuda.CUDAGraph()
+            state["g"].capture_begin(**kw)
+
+            def on_stage(name):
+                if name not in buckets:
+                    return  # not an active cut
+                state["g"].capture_end()
+                state["pool"] = state["pool"] or state["g"].pool()
+                segs.append((state["g"], buckets[name]))
+                self._after_cut()
+                state["g"] = torch.cuda.CUDAGraph()
+                state["g"].capture_begin(pool=state["pool"])
+
+            self._on_stage = on_stage
+            try:
+                loss = run()
+            finally:
+                self._on_stage = None
+                ops.set_sm_limit(0)
+            state["g"].capture_end()
+            state["pool"] = state["pool"] or state["g"].pool()
+            segs.append((state["g"], buckets["final"]))
+        cur.wait_stream(stream)
+        return segs, loss, state["pool"]
+
+    def _after_cut(self):
+        """hook while capturing the segments that follow a bucket cut (they run next to the bucket's all-reduce)"""
 
     def step(self, x0, hint_latent, context, t, noise):
         """One micro-batch; every accumulate_grad_batches-th call also exchanges the gradients and runs AdamW.  Returns
         this micro-batch's loss (its own mean, not divided by k)."""
-        if self.accumulate_grad_batches > 1:
-            return self._micro_batch((x0, hint_latent, context, t, noise), None)
-        overlapped = False
-        if getattr(self, "_graph", None) is not None:
-            loss = self.loss_and_grads_graphed(x0, hint_latent, context, t, noise)
-            overlapped = bool(self._segments)
-        elif self.world > 1 and self._overlap():
-            buckets = dict(self.merged_buckets())
-            self._on_stage = lambda name: self._reduce_ranges(buckets.get(name))
-            try:
-                loss = self.loss_and_grads(x0, hint_latent, context, t, noise)
-            finally:
-                self._on_stage = None
-            self._reduce_ranges(buckets["final"])
-            overlapped = True
-        else:
-            loss = self.loss_and_grads(x0, hint_latent, context, t, noise)
-        if overlapped:
-            torch.cuda.current_stream().wait_stream(self._comm)  # every bucket reduced before the overflow check / AdamW
-        else:
-            self.reduce_gradients()
-        self._update(self.window_segments([None]))
-        return loss
+        return self._micro_batch((x0, hint_latent, context, t, noise), None)
 
     def _update(self, segs):
         """Overflow check and AdamW over the exchanged gradients of the segments `segs` ([(offset, numel, key)]): the end
@@ -996,8 +1069,8 @@ class FinetuneTrainer:
         self._recapture()
 
     def _recapture(self):
-        if getattr(self, "_graph", None) is not None or self._accum is not None:
-            self.capture(*self._static, warmup=1)
+        if self._graphs is not None:
+            self.capture(*self._static, tasks=list(self._graphs["compute"]), warmup=1)
 
     def _overflowed(self):
         return bool(self.overflow_flag.item())
@@ -1010,9 +1083,6 @@ class FinetuneTrainer:
     def _alias_key(self, key):
         """a state-dict key that names a parameter also stored under another key (checkpoint.checkpoint_weights)"""
         return False
-
-    def _rank(self):
-        return torch.distributed.get_rank(self.pg) if self.world > 1 else 0
 
     def _exact_counters(self):
         """Read the device's skipped-step counter now (the periodic poll, forced), so step_count, seg_steps,
@@ -1057,10 +1127,7 @@ class FinetuneTrainer:
 
     def _captured_scales(self):
         """loss scales baked into the captured graphs"""
-        out = [self._scale_used] if getattr(self, "_graph", None) is not None else []
-        if self._accum is not None:
-            out += [c[2] for c in self._accum["compute"].values()]
-        return out
+        return [scale for _, _, scale in self._graphs["compute"].values()] if self._graphs is not None else []
 
     def save_checkpoint(self, path, epoch=0):
         """Write a checkpoint in the layout of the reference's `trainer.save_checkpoint` (cldm/logger.py:123):
@@ -1068,7 +1135,7 @@ class FinetuneTrainer:
         ([state_dict()["optimizer"]]), global_step (step_count: optimizer steps), epoch, and checkpoint.EXTRA_KEY.
         Under torch.distributed every rank syncs its counters, rank 0 writes, and all ranks leave together."""
         self._exact_counters()
-        if self._rank() == 0:
+        if self.rank == 0:
             ckpt = {"epoch": int(epoch), "global_step": int(self.step_count),
                     "state_dict": checkpoint.model_state_dict(self.model),
                     "optimizer_states": [checkpoint.optimizer_state_dict(self)],
@@ -1097,11 +1164,11 @@ class FinetuneTrainer:
         self._recapture()
         return {"epoch": ckpt.get("epoch", 0), "global_step": ckpt.get("global_step", self.step_count)}
 
-    # -- gradient accumulation (accumulate_grad_batches = k > 1) ------------------------------------------------------
+    # -- gradient accumulation (accumulate_grad_batches = k; a plain step is k = 1) ---------------------------------------
     # A window of k micro-batches: the first zeroes the gradient buffer (and the overflow flag) and fixes the loss scale;
-    # every micro-batch's backward adds into the buffer (every gradient write of the backward accumulates); the trainable
-    # weight copies (LoRA folds, fp16 / transposed / dgrad copies) are built once per window: the caches are keyed on the
-    # train version, which moves only when AdamW runs.  Only the last micro-batch exchanges the gradients.
+    # every micro-batch's backward adds into the buffer (every gradient write of the backward accumulates); with k > 1 the
+    # trainable weight copies (LoRA folds, fp16 / transposed / dgrad copies) are built once per window: the caches are
+    # keyed on the train version, which moves only when AdamW runs.  Only the last micro-batch exchanges the gradients.
     def window_segments(self, tasks):
         """[(offset, numel, key)] a window's update touches, given this rank's micro-batch tasks: the whole buffer."""
         return [(0, self.G.numel, "all")]
@@ -1119,69 +1186,55 @@ class FinetuneTrainer:
         final = self.micro_step == self.accumulate_grad_batches
         return start, first_use, (self.window_segments(self._window_tasks) if final else None)
 
-    def _run(self, args, task, accumulate):
-        return self.loss_and_grads(*args, accumulate=accumulate)
-
-    def _window_plan(self, segs, bucket_ranges):
-        """ranges to all-reduce after each backward bucket of the window's last micro-batch"""
-        return bucket_ranges
-
-    def _reduce_window(self, segs):
-        self.reduce_gradients([(off, n) for off, n, _ in segs])
-
-    def _segmented(self):
-        """capture the accumulating path's compute graph as one graph per gradient bucket (overlapped exchange)"""
-        return self.world > 1 and self._overlap()
-
-    def _after_cut(self):
-        """hook while capturing the segment that follows a bucket cut"""
-
     def _micro_batch(self, args, task):
+        """step(): replay the task's captured graphs, or run it eagerly; the window's last micro-batch exchanges the
+        gradients -- bucket by bucket under its backward when the exchange is segmented -- and runs AdamW."""
         start, first_use, segs = self.begin_micro_batch(task)
         final = segs is not None
+        compute = self._graphs["compute"] if self._graphs else {}
         overlapped = False
-        if self._accum is not None:
+        if task in compute:
             for dst, src in zip(self._static, args):
                 if dst.data_ptr() != src.data_ptr():
                     dst.copy_(src, non_blocking=True)
             if task is not None:
-                self.cn.switch_lora(task)  # host-side pointers follow the graphs
+                self.cn.switch_lora(task)  # host-side pointers follow the graphs (weight caches are keyed on them)
                 self.task = task
-            prep, compute = self._accum["prep"], self._accum["compute"]
-            if task not in compute:
-                raise KeyError(f"no graph captured for task {task!r}: pass it to capture()")
-            if start:
+            prep = self._graphs["prep"]   # empty at k = 1: the compute graph rebuilds the copies
+            if start and None in prep:
                 prep[None].replay()       # zero the buffer and the overflow flag, rebuild the task-independent copies
             if first_use and task is not None and task in prep:
                 prep[task].replay()       # the task's LoRA folds, once per window
             g, static_loss, self._scale_used = compute[task]
             if isinstance(g, list):
-                plan = self._window_plan(segs, [r for _, r in g]) if final else [None] * len(g)
+                plan = self.exchange_plan(segs, [r for _, r in g]) if final else [None] * len(g)
                 for (graph, _), ranges in zip(g, plan):
                     graph.replay()
-                    if final:
-                        self._reduce_ranges(ranges)
+                    self._reduce_ranges(ranges)
                 overlapped = final and self.world > 1
             else:
                 g.replay()
-            loss = static_loss.clone()    # the next micro-batch's graphs may reuse the captured loss's memory
-        elif final and self.world > 1 and self._overlap():
+            loss = static_loss.clone()    # the next replay overwrites the captured loss
+        elif compute and self.accumulate_grad_batches > 1:
+            # at k = 1 an uncaptured task runs eagerly; a window's micro-batches read its preparation graphs' copies
+            raise KeyError(f"no graph captured for task {task!r}: pass it to capture()")
+        elif final and self._segmented():
             merged = self.merged_buckets()
-            plan = dict(zip([st for st, _ in merged], self._window_plan(segs, [r for _, r in merged])))
+            plan = dict(zip([st for st, _ in merged], self.exchange_plan(segs, [r for _, r in merged])))
             self._on_stage = lambda name: self._reduce_ranges(plan.get(name))
             try:
-                loss = self._run(args, task, not start)
+                loss = self.loss_and_grads(*args, task=task, accumulate=not start)
             finally:
                 self._on_stage = None
             self._reduce_ranges(plan["final"])
-            overlapped = True
+            overlapped = self.world > 1
         else:
-            loss = self._run(args, task, not start)
+            loss = self.loss_and_grads(*args, task=task, accumulate=not start)
         if final:
             if overlapped:
-                torch.cuda.current_stream().wait_stream(self._comm)
+                torch.cuda.current_stream().wait_stream(self._comm)  # every bucket reduced before the overflow check / AdamW
             else:
-                self._reduce_window(segs)
+                self.reduce_gradients([(off, n) for off, n, _ in segs])
             self._update(segs)
         return loss
 
@@ -1191,114 +1244,8 @@ class FinetuneTrainer:
         if self.micro_step == 0:
             return
         segs = self.window_segments(self._window_tasks)
-        self._reduce_window(segs)
+        self.reduce_gradients([(off, n) for off, n, _ in segs])
         self._update(segs)
-
-    def _capture_window(self, tasks, warmup):
-        """CUDA graphs of the accumulating path, for the shapes of self._static:
-          * prep[None]: zero the gradient buffer and the overflow flag, rebuild every trainable-weight copy that does not
-            depend on a task's LoRA set -- replayed at a window's start;
-          * prep[task] (pretraining): rebuild the copies that depend on the task's LoRA set -- replayed on the task's first
-            micro-batch in a window (a window mixes tasks, so not every fold can be built at its start);
-          * compute[task]: forward + backward adding into the buffer, reading the copies above (one graph, or one per
-            gradient bucket when the exchange overlaps the backward).
-        Which copies a micro-batch reads is recorded from an eager run.  Each prep graph has a memory pool of its own, so
-        no other graph's scratch can overwrite the copies it keeps; the compute graphs share one pool (one is in flight)."""
-        static = self._static
-        cur = torch.cuda.current_stream()
-        side = torch.cuda.Stream()
-        side.wait_stream(cur)
-        logs = {}
-        with torch.cuda.stream(side):
-            for task in tasks:
-                for _ in range(warmup - 1):
-                    self._run(static, task, False)
-                prepare.bump_train_version()
-                with prepare.record_builds() as log:
-                    self._run(static, task, False)
-                logs[task] = log
-        cur.wait_stream(side)
-        torch.cuda.synchronize()
-        builds, seen = {None: []}, set()
-        for task in tasks:
-            own = self._task_param_ids(task)
-            builds.setdefault(task, [])
-            for entry in logs[task]:
-                cache, key, params, _ = entry
-                ps = [p for p in params if p is not None]
-                if not any(getattr(p, "_ctrlora_trainable", False) for p in ps):
-                    continue  # frozen copies are built once and never change
-                owner = task if any(id(p) in own for p in ps) else None
-                if (owner, id(cache), key) not in seen:
-                    seen.add((owner, id(cache), key))
-                    builds[owner].append(entry)
-
-        def rebuild(entries):
-            for cache, key, params, builder in entries:
-                cache.get(key, params, builder)
-
-        prepare.bump_train_version()  # every recorded copy is rebuilt inside its prep graph
-        prep, compute, pool = {}, {}, None
-        for owner, entries in builds.items():
-            if owner is not None and not entries:
-                continue
-            if owner is not None:
-                self.cn.switch_lora(owner)
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                if owner is None:
-                    self.G.zero()
-                    self.overflow_flag.zero_()
-                rebuild(entries)
-            prep[owner] = g
-        for task in tasks:
-            g, loss, pool = self._capture_compute(lambda: self._run(static, task, True), pool)
-            compute[task] = (g, loss, self._scale_used)
-        self._accum = {"prep": prep, "compute": compute}
-        return self
-
-    def _task_param_ids(self, task):
-        return set()
-
-    def _capture_compute(self, run, pool):
-        """graph of run() (one continuing micro-batch) in `pool`; one graph per gradient bucket when _segmented()"""
-        kw = {} if pool is None else {"pool": pool}
-        if not self._segmented():
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, **kw):
-                loss = run()
-            return g, loss, g.pool() if pool is None else pool
-        buckets = dict(self.merged_buckets())
-        cur = torch.cuda.current_stream()
-        segs, state = [], {"pool": pool}
-        stream = torch.cuda.Stream()
-        stream.wait_stream(cur)
-        with torch.cuda.stream(stream):
-            state["g"] = torch.cuda.CUDAGraph()
-            state["g"].capture_begin(**kw)
-
-            def on_stage(name):
-                if name not in buckets:
-                    return
-                state["g"].capture_end()
-                state["pool"] = state["pool"] or state["g"].pool()
-                segs.append((state["g"], buckets[name]))
-                self._after_cut()
-                state["g"] = torch.cuda.CUDAGraph()
-                state["g"].capture_begin(pool=state["pool"])
-
-            self._on_stage = on_stage
-            try:
-                loss = run()
-            finally:
-                self._on_stage = None
-                ops.set_sm_limit(0)
-            state["g"].capture_end()
-            state["pool"] = state["pool"] or state["g"].pool()
-            segs.append((state["g"], buckets["final"]))
-        cur.wait_stream(stream)
-        return segs, loss, state["pool"]
-
 
 
 # ------------------------------------------------------------------------------------------------ pretraining
@@ -1333,14 +1280,15 @@ class PretrainTrainer(FinetuneTrainer):
     mini-batch (datasets/multi_task_scheduler.py, mirrored by ctrlora_b200.scheduler.TaskSchedule).  Also covers
     ControlNetFinetune(ft_with_lora=False) (full-parameter finetuning, cldm_ctrlora_finetune.py:101-104)."""
 
+    # The dense gradient buffer is 1.5 GB, so part of its exchange can hide under the backward; the rest is lost to the
+    # collective's CTAs and HBM traffic competing with the backward it overlaps.  Default: all four cuts.
+    CUTS_ENV, CUTS_DEFAULT = "CTRLORA_PRETRAIN_ALLREDUCE_CUTS", "middle,ib9,ib6,ib3"
+
     def __init__(self, model, lr=1e-5, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.01, process_group=None,
                  loss_scale=None, dynamic_loss_scale=True, accumulate_grad_batches=1):
-        self._init_window(accumulate_grad_batches)
-        self.model = model
-        self.cn = model.control_model
-        self.unet = model.model.diffusion_model
+        super().__init__(model, lr, betas, eps, weight_decay, process_group, loss_scale, dynamic_loss_scale,
+                         accumulate_grad_batches, named=pretrain_parameters(model.control_model))
         self.tasks = list(getattr(self.cn, "tasks", []))
-        self.G = GradSink(self.cn, named=pretrain_parameters(self.cn))
         names = self.G.names
         first_lora = next((i for i, n in enumerate(names) if n.startswith("loras_dict.")), len(names))
         base_end = self.G.offsets[names[first_lora]][0] if first_lora < len(names) else self.G.numel
@@ -1350,137 +1298,22 @@ class PretrainTrainer(FinetuneTrainer):
             start = mine[0][0]
             assert all(o == start + sum(m[1] for m in mine[:i]) for i, (o, _) in enumerate(mine)), "task set not contiguous"
             self.layout["lora"][task] = (start, sum(m[1] for m in mine))
-        self.lr, self.betas, self.eps, self.wd = lr, betas, eps, weight_decay
-        self.pg = process_group
-        self.world, self.rank = 1, 0
-        if torch.distributed.is_available() and torch.distributed.is_initialized():
-            self.world = torch.distributed.get_world_size(process_group)
-            self.rank = torch.distributed.get_rank(process_group)
-        if self.world > 1:
-            torch.distributed.broadcast(self.G.flat_p, src=0, group=process_group)
-            prepare.bump_train_version()
-        self.step_count = 0
-        self.seg_steps = {}        # per-segment AdamW step counts (torch keeps `step` per parameter)
-        self.loss_scale, self.dynamic_loss_scale = loss_scale, dynamic_loss_scale
-        self.overflow_flag = torch.zeros(1, device=self.G.flat_p.device, dtype=torch.int32)
-        self.skipped_steps = 0
-        self._init_step_state(self.G.flat_p.device)
-        self._graphs, self._pool, self._static, self._static_loss = {}, None, None, {}
         self.task = self.tasks[0] if self.tasks else None
 
-    def loss_and_grads(self, x0, hint_latent, context, t, noise, task=None, accumulate=False):
-        if task is not None and self.tasks:
-            self.cn.switch_lora(task)
-            self.task = task
-        return super().loss_and_grads(x0, hint_latent, context, t, noise, accumulate=accumulate)
+    def _after_cut(self):
+        """Segments after a cut run next to a collective: their persistent GEMM grids leave CTRLORA_OVERLAP_SM_RESERVE
+        (default 16) SMs to its CTAs."""
+        reserve = int(os.environ.get("CTRLORA_OVERLAP_SM_RESERVE", "16"))
+        ops.set_sm_limit(max(2, torch.cuda.get_device_properties(self.G.flat_p.device).multi_processor_count - reserve))
 
-    def _run(self, args, task, accumulate):
-        return self.loss_and_grads(*args, task=task, accumulate=accumulate)
-
-    # -- one CUDA graph per task (the attached LoRA set is baked into the captured kernels' pointers); the graphs share one
-    # memory pool: only one of them is ever in flight
-    def _overlap_cuts(self):
-        """Backward stages that close a bucket whose all-reduce then runs under the rest of the backward
-        (CTRLORA_PRETRAIN_ALLREDUCE_CUTS, default all four: middle,ib9,ib6,ib3; empty = one exchange after the backward).
-        The dense gradient buffer is 1.5 GB, so part of its exchange can hide under the backward; the rest is lost to the
-        collective's CTAs and HBM traffic competing with the backward it overlaps."""
-        import os
-        cuts = getattr(self, "allreduce_cuts", None)
-        if cuts is None:
-            cuts = os.environ.get("CTRLORA_PRETRAIN_ALLREDUCE_CUTS", "middle,ib9,ib6,ib3")
-        if isinstance(cuts, str):
-            cuts = [c for c in cuts.split(",") if c]
-        return [c for c in ("middle", "ib9", "ib6", "ib3") if c in cuts]
-
-    def _cuts(self):
-        return self._overlap_cuts()
-
-    @staticmethod
-    def _sm_reserve():
-        """SMs left to the collective's CTAs while it overlaps the backward (persistent GEMM grids shrink by this much)"""
-        import os
-        return int(os.environ.get("CTRLORA_OVERLAP_SM_RESERVE", "16"))
-
-    def capture(self, x0, hint_latent, context, t, noise, tasks=None, warmup=2):
-        if self._static is None:
-            self._static = [v.clone() for v in (x0, hint_latent, context, t, noise)]
-        if self.accumulate_grad_batches > 1:
-            return self._capture_window(list(tasks or self.tasks or [None]), warmup)
-        overlap = self.world > 1 and bool(self._overlap_cuts())
-        for task in (tasks or self.tasks or [None]):
-            cur = torch.cuda.current_stream()
-            side = torch.cuda.Stream()
-            side.wait_stream(cur)
-            with torch.cuda.stream(side):
-                for _ in range(warmup):
-                    self.loss_and_grads(*self._static, task=task)
-            cur.wait_stream(side)
-            torch.cuda.synchronize()
-            prepare.bump_train_version()
-            if overlap:
-                # one graph per gradient bucket (shared pool): replay k, start bucket k's all-reduce on the communication
-                # stream, replay k+1 ... (NCCL stays outside the captures).  Segments after the first cut run next to a
-                # collective: their persistent GEMM grids leave `_sm_reserve()` SMs to it.
-                buckets = dict(self.merged_buckets())
-                segs, state = [], {}
-                stream = torch.cuda.Stream()
-                stream.wait_stream(cur)
-                with torch.cuda.stream(stream):
-                    state["g"] = torch.cuda.CUDAGraph()
-                    if self._pool is None:
-                        state["g"].capture_begin()
-                    else:
-                        state["g"].capture_begin(pool=self._pool)
-
-                    def on_stage(name):
-                        if name not in buckets:
-                            return  # not an active cut
-                        state["g"].capture_end()
-                        if self._pool is None:
-                            self._pool = state["g"].pool()
-                        segs.append((state["g"], buckets[name]))
-                        ops.set_sm_limit(max(2, torch.cuda.get_device_properties(self.G.flat_p.device).multi_processor_count
-                                             - self._sm_reserve()))
-                        state["g"] = torch.cuda.CUDAGraph()
-                        state["g"].capture_begin(pool=self._pool)
-
-                    self._on_stage = on_stage
-                    try:
-                        self._static_loss[task] = self.loss_and_grads(*self._static, task=task)
-                    finally:
-                        self._on_stage = None
-                        ops.set_sm_limit(0)
-                    state["g"].capture_end()
-                    if self._pool is None:
-                        self._pool = state["g"].pool()
-                    segs.append((state["g"], buckets["final"]))
-                cur.wait_stream(stream)
-                self._graphs[task] = (segs, self._scale_used)
-                continue
-            g = torch.cuda.CUDAGraph()
-            kw = {} if self._pool is None else {"pool": self._pool}
-            with torch.cuda.graph(g, **kw):
-                self._static_loss[task] = self.loss_and_grads(*self._static, task=task)
-            if self._pool is None:
-                self._pool = g.pool()
-            self._graphs[task] = (g, self._scale_used)
-        return self
-
-    def _tasks_on_ranks(self, task):
-        if self.world == 1 or not self.tasks:
-            return [task]
-        mine = torch.tensor([self.tasks.index(task)], device=self.G.flat_p.device, dtype=torch.int64)
-        allv = [torch.empty_like(mine) for _ in range(self.world)]
-        torch.distributed.all_gather(allv, mine, group=self.pg)
-        return [self.tasks[int(v.item())] for v in allv]
-
-    def segments_for(self, task):
-        return active_segments(self.layout, self._tasks_on_ranks(task)) if self.tasks else [(0, self.G.numel, "base")]
+    def step(self, x0, hint_latent, context, t, noise, task=None):
+        """One micro-batch of `task` (default: the attached one); see FinetuneTrainer.step."""
+        return self._micro_batch((x0, hint_latent, context, t, noise), task if task is not None else self.task)
 
     def window_segments(self, tasks):
         """Segments of a window whose micro-batches on this rank trained `tasks`: the ControlNet plus every LoRA set that
         any rank used in any micro-batch of the window.  The ranks exchange their used-task masks once per window (one
-        all-reduce)."""
+        all-reduce), before its last backward."""
         if not self.tasks:
             return [(0, self.G.numel, "base")]
         used = sorted({self.tasks.index(t) for t in tasks})
@@ -1490,22 +1323,6 @@ class PretrainTrainer(FinetuneTrainer):
             torch.distributed.all_reduce(mask, group=self.pg)
             used = [i for i, v in enumerate(mask.tolist()) if v]
         return active_segments(self.layout, [self.tasks[i] for i in used])
-
-    def _window_plan(self, segs, bucket_ranges):
-        return self.exchange_plan(segs, bucket_ranges)
-
-    def _reduce_window(self, segs):
-        self.reduce_gradients(segs)
-
-    def _segmented(self):
-        return self.world > 1 and bool(self._overlap_cuts())
-
-    def _after_cut(self):
-        ops.set_sm_limit(max(2, torch.cuda.get_device_properties(self.G.flat_p.device).multi_processor_count
-                             - self._sm_reserve()))
-
-    def _task_param_ids(self, task):
-        return {id(p) for n, p in zip(self.G.names, self.G.params) if n.startswith(f"loras_dict.{task}.")}
 
     def segment_keys(self):
         """"base" for the ControlNet's own parameters, the task for its LoRA set (active_segments)"""
@@ -1517,65 +1334,3 @@ class PretrainTrainer(FinetuneTrainer):
         """`control_model.<linear>.lora_layer.*`: the attached task's set, whose data is saved under loras_dict.<task>.*
         (which set a file had attached, if any, does not matter on load)"""
         return bool(self.tasks) and key.startswith("control_model.") and ".lora_layer." in key
-
-    def _captured_scales(self):
-        return [s for _, s in self._graphs.values()] + super()._captured_scales()
-
-    def exchange_plan(self, segs, bucket_ranges):
-        """Ranges to all-reduce after each backward bucket: the bucket's part of the ControlNet segment; the LoRA sets live
-        behind it in the flat buffer and travel with the LAST bucket, and only the sets some rank trained this step (`segs`,
-        from segments_for) are exchanged.  Every element of `segs` appears exactly once in the plan."""
-        base_end = self.layout["base"][1]
-        lora = [(off, n) for off, n, key in segs if key != "base"]
-        plan = []
-        for i, ranges in enumerate(bucket_ranges):
-            r = [(off, min(n, base_end - off)) for off, n in ranges if off < base_end]
-            plan.append(r + lora if i == len(bucket_ranges) - 1 else r)
-        return plan
-
-    def reduce_gradients(self, segs=None):
-        """The exchange step: all-reduce (SUM) of the ControlNet segment and of every LoRA set some rank trained this step
-        (the reference's DDP reduces all 589 M elements every step; unused sets are all-zero there)."""
-        if self.world > 1:
-            for off, n, _ in (segs or [(0, self.G.numel, "all")]):
-                torch.distributed.all_reduce(self.G.flat_g[off:off + n], group=self.pg)
-
-    def step(self, x0, hint_latent, context, t, noise, task=None):
-        task = task if task is not None else self.task
-        if self.accumulate_grad_batches > 1:
-            return self._micro_batch((x0, hint_latent, context, t, noise), task)
-        segs = self.segments_for(task)  # (ranks exchange their task index first: known before the backward starts)
-        overlapped = False
-        if task in self._graphs:
-            for dst, src in zip(self._static, (x0, hint_latent, context, t, noise)):
-                if dst.data_ptr() != src.data_ptr():
-                    dst.copy_(src, non_blocking=True)
-            if self.tasks:
-                self.cn.switch_lora(task)  # host-side pointers follow the graph (weight caches are keyed on them)
-                self.task = task
-            g, self._scale_used = self._graphs[task]
-            if isinstance(g, list):
-                for (graph, _), ranges in zip(g, self.exchange_plan(segs, [r for _, r in g])):
-                    graph.replay()
-                    self._reduce_ranges(ranges)
-                overlapped = True
-            else:
-                g.replay()
-            loss = self._static_loss[task]
-        else:
-            loss = self.loss_and_grads(x0, hint_latent, context, t, noise, task=task)
-        if overlapped:
-            torch.cuda.current_stream().wait_stream(self._comm)  # every bucket reduced before the overflow check / AdamW
-        else:
-            self.reduce_gradients(segs)
-        self._update(segs)
-        return loss
-
-    def _recapture(self):
-        if self._accum is not None:
-            self.capture(*self._static, tasks=list(self._accum["compute"]), warmup=1)
-        elif self._graphs:
-            tasks = list(self._graphs)
-            self._graphs.clear()
-            self._pool = None  # the freed graphs' pool cannot take new captures
-            self.capture(*self._static, tasks=tasks, warmup=1)

@@ -74,12 +74,12 @@ def _pretrain_worker(rank, world, port, q):
         synced = all(torch.equal(sums[0], s) for s in sums)
         # ranks train different tasks in the same step (per-rank un-seeded permutation, multi_task_scheduler.py:59)
         task = trainer.tasks[2 * rank]  # rank 0: canny, rank 1: seg; nobody trains depth
-        segs = trainer.segments_for(task)
+        segs = trainer.window_segments([task])
         keys = [k for _, _, k in segs]
         gen = torch.Generator().manual_seed(100 + rank)
         G.flat_g.copy_(torch.randn(G.numel, generator=gen))
         mine = G.flat_g.clone()
-        trainer.reduce_gradients(segs)
+        trainer.reduce_gradients([(off, n) for off, n, _ in segs])
         gathered = [torch.empty_like(mine) for _ in range(world)]
         dist.all_gather(gathered, mine)
         total = sum(gathered)
@@ -110,7 +110,7 @@ def _pretrain_worker(rank, world, port, q):
         dist.destroy_process_group()
 
 
-def test_pretrain_segments_world2():
+def test_pretrain_window_segments_world2():
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
     port = 31500 + (os.getpid() % 2000)

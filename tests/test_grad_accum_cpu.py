@@ -44,7 +44,7 @@ def _worker(rank, world, port, q):
             G.flat_g.copy_(torch.randn(G.numel, generator=gen))
             mine = G.flat_g.clone()
             calls.clear()
-            trainer._reduce_window(segs)
+            trainer.reduce_gradients([(off, n) for off, n, _ in segs])
             res["grad_exchange"] = sorted(calls) == sorted(n for _, n, _ in segs)
         finally:
             torch.distributed.all_reduce = orig
@@ -56,7 +56,7 @@ def _worker(rank, world, port, q):
         res["depth_untouched"] = torch.equal(G.flat_g[d_off:d_off + d_n], mine[d_off:d_off + d_n])
         # the overlapped form: every element of the window's segments in exactly one bucket's exchange
         trainer.allreduce_cuts = "middle,ib9,ib6,ib3"
-        plan = trainer._window_plan(segs, [r for _, r in trainer.merged_buckets()])
+        plan = trainer.exchange_plan(segs, [r for _, r in trainer.merged_buckets()])
         flat = sorted(r for ranges in plan for r in ranges)
         covered = [0] * len(segs)
         for off, n in flat:
@@ -70,7 +70,7 @@ def _worker(rank, world, port, q):
         dist.destroy_process_group()
 
 
-def test_window_segments_and_collectives_world2():
+def test_window_segments_plan_and_collectives_world2():
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
     port = 33500 + (os.getpid() % 2000)

@@ -140,20 +140,22 @@ def rerun_close(a, b, p0):
 @pytest.mark.parametrize("graphed", [False, True])
 def test_k1_is_the_plain_trainer(gold, graphed, monkeypatch):
     """accumulate_grad_batches=1 runs the same kernels in the same order as a trainer built without it (recorded ops
-    sequence of the eager steps, or of the captures), and reaches the same state up to the run-to-run atomics noise."""
+    sequence of the eager steps, or of the captures), and reaches the same state up to the run-to-run atomics noise.
+    Every step returns a loss tensor of its own (a replayed graph's loss is overwritten by its next replay)."""
     a, b = make(gold, "finetune"), make(gold, "finetune", accumulate_grad_batches=1)
     p0 = a.G.flat_p.clone()
-    seqs = []
+    seqs, losses = [], []
     for tr in (a, b):
         seq = record_ops(monkeypatch)
         if graphed:
             tr.capture(*micro(gold, 0))
-        for i in range(2):
-            tr.step(*micro(gold, i))
+        losses.append([tr.step(*micro(gold, i)) for i in range(2)])
         seqs.append(list(seq))
         monkeypatch.undo()
     torch.cuda.synchronize()
     assert len(seqs[0]) > 100 and seqs[0] == seqs[1]
+    for first, second in losses:
+        assert first is not second and first.item() != second.item()
     rerun_close(a, b, p0)
     assert a.step_count == b.step_count == 2 and b.micro_step == 0
 
@@ -216,7 +218,7 @@ def test_k_micro_batches_equal_one_batch_of_k_b(gold):
     assert e_g < ACCUM_TOL["kb_grad"] and e_u < ACCUM_TOL["kb_update"]
 
 
-def test_graph_window_equals_eager_window(gold):
+def test_captured_window_equals_eager_window(gold):
     """Captured windows (pretrain, mixed tasks; finetune, segmented at the overlap cuts) against eager ones: the same
     kernels in the same order, equal up to the run-to-run noise of the float-atomic reductions (rerun_close)."""
     tasks = [["canny", "depth", "canny"], ["seg", "seg", "depth"]]
@@ -238,7 +240,7 @@ def test_graph_window_equals_eager_window(gold):
         tr.allreduce_cuts = "middle,ib9,ib6,ib3"
     graph._segmented = lambda: True  # one graph per bucket even on one GPU (the all-reduces are no-ops there)
     graph.capture(*micro(gold, 0))
-    assert isinstance(graph._accum["compute"][None][0], list) and len(graph._accum["compute"][None][0]) == 5
+    assert isinstance(graph._graphs["compute"][None][0], list) and len(graph._graphs["compute"][None][0]) == 5
     for _ in range(2):
         for i in range(3):
             le, lg = eager.step(*micro(gold, i)), graph.step(*micro(gold, i))
