@@ -76,6 +76,7 @@ _ARGTYPES = {
     "ctrlora_nchw_f32_to_nhwc_f16": [_P, _P, _I, _I, _I, _I, _P],
     "ctrlora_nhwc_to_nchw_f32": [_P, _I, _L, _P, _I, _I, _I, _P],
     "ctrlora_timestep_embedding": [_P, _P, _P, _I, _I, _P],
+    "ctrlora_timestep_embedding_f32": [_P, _P, _P, _I, _I, _P],
     "ctrlora_small_linear": [_P, _I, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P],
     "ctrlora_upsample2x_f16": [_P, _P, _I, _I, _I, _I, _P],
     "ctrlora_im2col_s2_f16": [_P, _P, _I, _I, _I, _I, _P],
@@ -108,6 +109,7 @@ _ARGTYPES = {
     "ctrlora_memset_zero": [_P, _L, _P],
     "ctrlora_q_sample": [_P, _P, _P, _P, _P, _P, _I, _I, _P],
     "ctrlora_ddim_encode_update": [_P, _P, _P, _P, _I, _F, _F, _F, _P],
+    "ctrlora_dpm_multistep_update": [_P, _P, _P, _P, _P, _P, _I, _F, _F, _F, _F, _F, _F, _F, _P],
     "ctrlora_weighted_sum_f16": [_P, _P, _I, _P, _L, _P],
 }
 
@@ -140,6 +142,7 @@ EXPORTS = [
     "ctrlora_nchw_f32_to_nhwc_f16",
     "ctrlora_nhwc_to_nchw_f32",
     "ctrlora_timestep_embedding",
+    "ctrlora_timestep_embedding_f32",
     "ctrlora_small_linear",
     "ctrlora_upsample2x_f16",
     "ctrlora_im2col_s2_f16",
@@ -174,4 +177,5 @@ EXPORTS = [
     "ctrlora_silu_bwd_f32",
     "ctrlora_cast_rows_f32_to_f16",
     "ctrlora_ddim_encode_update",
+    "ctrlora_dpm_multistep_update",
 ]

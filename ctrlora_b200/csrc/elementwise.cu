@@ -1,6 +1,6 @@
 // Small HBM/latency-bound kernels of the hot path: layout/dtype conversion at the module boundary, timestep embedding,
 // the M = batch linears of the time-embedding MLP, nearest-2x upsample, the stride-2 gather, weight preparation and
-// the DDIM update.
+// the DDIM and DPM-Solver++ updates.
 #include "common.cuh"
 #include "ctrlora_b200.h"
 
@@ -36,6 +36,18 @@ __global__ void timestep_embedding_kernel(const long long* __restrict__ t, const
     if (i >= B * half) return;
     const int b = i / half, k = i % half;
     const float arg = __fmul_rn(static_cast<float>(t[b]), freqs[k]);
+    out[b * 2 * half + k] = cosf(arg);
+    out[b * 2 * half + half + k] = sinf(arg);
+}
+
+// ---- same embedding at fp32 t (DPM-Solver's fractional model times, e.g. 949.05): the product is rounded once and fed
+// to the accurate cosf / sinf (the __cosf / __sinf intrinsics are far off at |arg| ~ 1000)
+__global__ void timestep_embedding_f32_kernel(const float* __restrict__ t, const float* __restrict__ freqs,
+                                              float* __restrict__ out, int B, int half) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= B * half) return;
+    const int b = i / half, k = i % half;
+    const float arg = __fmul_rn(t[b], freqs[k]);
     out[b * 2 * half + k] = cosf(arg);
     out[b * 2 * half + half + k] = sinf(arg);
 }
@@ -319,6 +331,28 @@ ddim_encode_kernel(const float* __restrict__ x, const float* __restrict__ e_cond
     x_next[i] = __fadd_rn(__fmul_rn(c1, x[i]), __fmul_rn(c2, e));
 }
 
+// DPM-Solver++ multistep step (ldm/models/diffusion/dpm_solver/dpm_solver.py, data prediction, solver_type 'dpm_solver'):
+// CFG combine (:311-312), data prediction m = (x - sigma_s e) / alpha_s (:356-359) written to m_out, then the order-1
+// (:490-497) or order-2 (:748-758) update.  Explicit round-to-nearest ops in the reference's order: no FMA contraction.
+__global__ void __launch_bounds__(256)
+dpm_multistep_kernel(const float* __restrict__ x, const float* __restrict__ e_cond, const float* __restrict__ e_uncond,
+                     const float* __restrict__ m_prev, float* __restrict__ m_out, float* __restrict__ x_next, int total,
+                     float cfg_scale, float sigma_s, float alpha_s, float c_x, float c_m, float c_d, float inv_r0) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    float e = e_cond[i];
+    if (e_uncond) {
+        const float u = e_uncond[i];
+        e = __fadd_rn(u, __fmul_rn(cfg_scale, __fsub_rn(e, u)));
+    }
+    const float xi = x[i];
+    const float m = __fdiv_rn(__fsub_rn(xi, __fmul_rn(sigma_s, e)), alpha_s);
+    float xn = __fsub_rn(__fmul_rn(c_x, xi), __fmul_rn(c_m, m));
+    if (m_prev) xn = __fsub_rn(xn, __fmul_rn(c_d, __fmul_rn(inv_r0, __fsub_rn(m, m_prev[i]))));
+    m_out[i] = m;
+    x_next[i] = xn;
+}
+
 static inline unsigned blocks_for(long long total, int threads) { return static_cast<unsigned>((total + threads - 1) / threads); }
 
 }  // namespace ctrl
@@ -353,6 +387,14 @@ extern "C" int ctrlora_timestep_embedding(const long long* t, const float* freqs
                                           void* stream) {
     if (!t || !freqs || !out) return CTRLORA_ERR_ARG;
     timestep_embedding_kernel<<<blocks_for(static_cast<long long>(batch) * half, 128), 128, 0, STREAM(stream)>>>(
+        t, freqs, out, batch, half);
+    return LAUNCH_OK();
+}
+
+extern "C" int ctrlora_timestep_embedding_f32(const float* t, const float* freqs, float* out, int batch, int half,
+                                              void* stream) {
+    if (!t || !freqs || !out) return CTRLORA_ERR_ARG;
+    timestep_embedding_f32_kernel<<<blocks_for(static_cast<long long>(batch) * half, 128), 128, 0, STREAM(stream)>>>(
         t, freqs, out, batch, half);
     return LAUNCH_OK();
 }
@@ -612,5 +654,14 @@ extern "C" int ctrlora_ddim_encode_update(const float* x, const float* e_cond, c
                                           int total, float cfg_scale, float c1, float c2, void* stream) {
     if (!x || !e_cond || !x_next) return CTRLORA_ERR_ARG;
     ddim_encode_kernel<<<blocks_for(total, 256), 256, 0, STREAM(stream)>>>(x, e_cond, e_uncond, x_next, total, cfg_scale, c1, c2);
+    return LAUNCH_OK();
+}
+
+extern "C" int ctrlora_dpm_multistep_update(const float* x, const float* e_cond, const float* e_uncond, const float* m_prev,
+                                            float* m_out, float* x_next, int total, float cfg_scale, float sigma_s,
+                                            float alpha_s, float c_x, float c_m, float c_d, float inv_r0, void* stream) {
+    if (!x || !e_cond || !m_out || !x_next || total < 0) return CTRLORA_ERR_ARG;
+    dpm_multistep_kernel<<<blocks_for(total, 256), 256, 0, STREAM(stream)>>>(
+        x, e_cond, e_uncond, m_prev, m_out, x_next, total, cfg_scale, sigma_s, alpha_s, c_x, c_m, c_d, inv_r0);
     return LAUNCH_OK();
 }

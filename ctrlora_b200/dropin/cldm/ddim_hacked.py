@@ -203,7 +203,7 @@ class DDIMSampler(object):
         """[cond | uncond] batch of one CFG step in persistent buffers: plain device-to-device copies (no ATen cat
         kernels per step); the conditioning halves are re-copied only when their tensors change."""
         b = x.shape[0]
-        sig = (tuple(x.shape), x.dtype, tuple((tuple(a.shape), a.dtype) for a in cond_tensors))
+        sig = (tuple(x.shape), x.dtype, t.dtype, tuple((tuple(a.shape), a.dtype) for a in cond_tensors))
         if self._cfg_buf is None or self._cfg_buf["sig"] != sig:
             mk = lambda a: torch.empty((2 * a.shape[0],) + tuple(a.shape[1:]), device=a.device, dtype=a.dtype)
             self._cfg_buf = {"sig": sig, "x": mk(x), "t": mk(t), "c": [mk(a) for a in cond_tensors], "src": None}
@@ -249,7 +249,9 @@ class DDIMSampler(object):
         if not self.use_cuda_graph or flat is None or not x.is_cuda:
             return self.model.apply_model(x, t, c)
         keys, tensors = flat
-        key = (keys, tuple(x.shape), tuple(tuple(tt.shape) for tt in tensors), tuple(self.model.control_scales),
+        # t's dtype is part of the key: a graph captured with int64 t would copy_ a float t (DPM-Solver's fractional
+        # model times) into its int64 static input, truncating it
+        key = (keys, tuple(x.shape), t.dtype, tuple(tuple(tt.shape) for tt in tensors), tuple(self.model.control_scales),
                self.model.only_mid_control, ctx_mode, self._weights_fingerprint())
         if self._graph is None or self._graph_key != key:
             cached = self._graphs.pop(key, None)  # a sampler alternates between at most a few keys (run mode on / off)

@@ -84,12 +84,15 @@ def embedding_freqs(dim, max_period, device):
 
 
 def timestep_embedding(timesteps, dim, max_period=10000, repeat_only=False):
-    """reference util.py:154-174 -> ctrlora_timestep_embedding.  timesteps: int64 [B] on a CUDA device."""
+    """reference util.py:154-174 -> ctrlora_timestep_embedding.  timesteps: [B] on a CUDA device.  Integer timesteps
+    (the trainers, q_sample, DDIM) take the int64 kernel; floating ones (DPM-Solver's fractional model times) are
+    embedded at their fp32 value, as the reference's `timesteps[:, None].float()` does (:168)."""
     if repeat_only or dim % 2:
         raise NotImplementedError("repeat_only / odd dims are not on the CtrLoRA path")
     if not timesteps.is_cuda:
         raise RuntimeError("ctrlora_b200: timestep_embedding needs CUDA tensors (no CPU path)")
-    return ops.timestep_embedding(timesteps.to(torch.int64).contiguous(), embedding_freqs(dim, max_period, timesteps.device))
+    t = timesteps.to(torch.float32 if timesteps.is_floating_point() else torch.int64).contiguous()
+    return ops.timestep_embedding(t, embedding_freqs(dim, max_period, timesteps.device))
 
 
 # ------------------------------------------------------------------------------------------------ parameter holders

@@ -4,6 +4,8 @@ One apply_model is ~1000 kernel launches issued through ctypes; at batch 4 the G
 can enqueue them, so the launch-bound inner loop is captured once and replayed (the graph also pins the TMA tensor
 maps and tile schedules that the C ABI computed at capture time).
 """
+import gc
+
 import torch
 
 
@@ -26,9 +28,19 @@ class GraphedCallable:
                 fn(*self.static_in)
         cur.wait_stream(side)
         torch.cuda.synchronize()
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self.static_out = fn(*self.static_in)
+        # A dropped sampler's graph is cyclic garbage (its callable closes over the sampler). Collected in the middle of
+        # this capture, its destruction is an illegal call while capturing and invalidates the capture; so collect
+        # now, and not during the capture.
+        gc.collect()
+        gc_was_enabled = gc.isenabled()
+        gc.disable()
+        try:
+            self.graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(self.graph):
+                self.static_out = fn(*self.static_in)
+        finally:
+            if gc_was_enabled:
+                gc.enable()
 
     def __call__(self, *inputs):
         for s, i in zip(self.static_in, inputs):

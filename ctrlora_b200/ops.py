@@ -391,13 +391,14 @@ def nhwc_to_nchw_f32(x, channels=None):
 
 
 def timestep_embedding(t, freqs):
-    """t int64 [B] (device), freqs fp32 [half] (device) -> fp32 [B, 2*half]"""
+    """t int64 or fp32 [B] (device), freqs fp32 [half] (device) -> fp32 [B, 2*half].  int64 t takes the integer kernel;
+    fp32 t (DPM-Solver's fractional model times) takes ctrlora_timestep_embedding_f32, never a truncation."""
     _require_cuda(t, freqs)
-    assert t.dtype == torch.int64 and freqs.dtype == torch.float32
+    assert t.dtype in (torch.int64, torch.float32) and freqs.dtype == torch.float32
     out = torch.empty((t.shape[0], 2 * freqs.shape[0]), device=t.device, dtype=torch.float32)
+    fn = _lib.load().ctrlora_timestep_embedding if t.dtype == torch.int64 else _lib.load().ctrlora_timestep_embedding_f32
     _count(1)
-    check(_lib.load().ctrlora_timestep_embedding(_dp(t), _dp(freqs), _dp(out), t.shape[0], freqs.shape[0], _sp()),
-          "timestep_embedding")
+    check(fn(_dp(t), _dp(freqs), _dp(out), t.shape[0], freqs.shape[0], _sp()), "timestep_embedding")
     return out
 
 
@@ -564,6 +565,21 @@ def ddim_encode_update(x, e_cond, e_uncond, cfg_scale, c1, c2):
     check(_lib.load().ctrlora_ddim_encode_update(_dp(x), _dp(e_cond), _dp(e_uncond), _dp(out), x.numel(), float(cfg_scale),
                                                  float(c1), float(c2), _sp()), "ddim_encode_update")
     return out
+
+
+def dpm_multistep_update(x, e_cond, e_uncond, m_prev, m_out, cfg_scale, sigma_s, alpha_s, c_x, c_m, c_d=0.0, inv_r0=0.0):
+    """One DPM-Solver++ multistep step (ldm/models/diffusion/dpm_solver/dpm_solver.py): writes the data prediction
+    (x - sigma_s * e) / alpha_s into m_out and returns x_next; order 2 when m_prev is given, order 1 otherwise.
+    fp32 contiguous [B,C,H,W] tensors; the scalars come from ctrlora_b200.dpm_schedule."""
+    _require_cuda(x, e_cond, e_uncond, m_prev, m_out)
+    for t in (x, e_cond, e_uncond, m_prev, m_out):
+        assert t is None or (t.dtype == torch.float32 and t.is_contiguous() and t.shape == x.shape)
+    x_next = torch.empty_like(x)
+    _count()
+    check(_lib.load().ctrlora_dpm_multistep_update(_dp(x), _dp(e_cond), _dp(e_uncond), _dp(m_prev), _dp(m_out), _dp(x_next),
+                                                   x.numel(), float(cfg_scale), float(sigma_s), float(alpha_s), float(c_x),
+                                                   float(c_m), float(c_d), float(inv_r0), _sp()), "dpm_multistep_update")
+    return x_next
 
 
 def wgrad_tn(a, b, out=None, alpha=1.0, beta=0.0):

@@ -133,6 +133,11 @@ int ctrlora_nhwc_to_nchw_f32(const void* src, int src_is_f32, long long ld, floa
 /* timestep_embedding   ldm/modules/diffusionmodules/util.py:154-174: out[b] = [cos(t_b * f) | sin(t_b * f)];
  * freqs (fp32 [half]) are computed on the host exactly as the reference does; t is int64. */
 int ctrlora_timestep_embedding(const long long* t, const float* freqs, float* out, int batch, int half, void* stream);
+/* timestep_embedding   ldm/modules/diffusionmodules/util.py:154-174 at fp32 t (the reference embeds `t[:, None].float()`,
+ * :168): DPM-Solver's model times (t_continuous - 1/N) * 1000 (ldm/models/diffusion/dpm_solver/dpm_solver.py:246-253)
+ * are fractional.  arg = t[b] * freqs[k] rounded once, then accurate cosf / sinf; integer-valued t gives the bits of
+ * ctrlora_timestep_embedding. */
+int ctrlora_timestep_embedding_f32(const float* t, const float* freqs, float* out, int batch, int half, void* stream);
 
 /* y = act_out(act_in(x) W^T + b) for M = batch rows, fp32 activations, fp16 weights [n, k].
  * replaces time_embed (Linear-SiLU-Linear, openaimodel.py:526-531) and every ResBlock emb_layers (SiLU-Linear, :208-215). */
@@ -185,6 +190,17 @@ int ctrlora_q_sample(const float* x0, const float* noise, const long long* t, co
  * by the caller in fp32 like the reference's 0-dim tensor arithmetic. */
 int ctrlora_ddim_encode_update(const float* x, const float* e_cond, const float* e_uncond, float* x_next, int total,
                                float cfg_scale, float c1, float c2, void* stream);
+/* One step of DPMSolverSampler (ldm/models/diffusion/dpm_solver/sampler.py:72-85: DPM-Solver++, multistep, data
+ * prediction), all fp32 with round-to-nearest ops in the reference's order (dpm_solver.py):
+ *   e = e_uncond + cfg * (e_cond - e_uncond)                 :311-312 (e_uncond may be NULL: no guidance)
+ *   m_out = (x - sigma_s * e) / alpha_s                      :356-359 (data prediction at the step's start time)
+ *   x_next = c_x * x - c_m * m_out                           order 1, :490-497 (m_prev NULL)
+ *            - c_d * (inv_r0 * (m_out - m_prev))             order 2, :748-758
+ * The per-step scalars (c_x = sigma_t / sigma_s, c_m = alpha_t * expm1(-h) or alpha_t * (exp(-h) - 1),
+ * c_d = 0.5 * c_m, inv_r0 = 1 / r0) are computed by the caller from NoiseScheduleVP('discrete') (:60-160). */
+int ctrlora_dpm_multistep_update(const float* x, const float* e_cond, const float* e_uncond, const float* m_prev, float* m_out,
+                                 float* x_next, int total, float cfg_scale, float sigma_s, float alpha_s, float c_x, float c_m,
+                                 float c_d, float inv_r0, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Training (backward of the trainable set; reference: autograd over cldm/lora.py:70-80,285-291 and cldm/cldm.py:281-282,

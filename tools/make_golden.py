@@ -4,6 +4,8 @@
     python tools/make_golden.py --full     # SD1.5-size eps for one image (committed fixture, ~70 KB; takes minutes)
     python tools/make_golden.py --accum    # gradient accumulation windows, finetune and pretrain (tiny config)
     python tools/make_golden.py --resume   # AdamW state of a checkpoint and the steps after it (tiny config)
+    python tools/make_golden.py --dpm      # DPMSolverSampler samples (tiny configs) and host schedule (SD1.5 alphas)
+    python tools/make_golden.py --dpm-full # DPMSolverSampler samples at SD1.5 size, batch 1 (about a minute)
 
 The reference cannot travel to the GPU box; these fixtures can.  Weights/inputs are regenerated from names by
 oracle/synth.py, so the fixtures hold only key/shape lists and outputs.
@@ -705,8 +707,145 @@ def resume(seed=0, lr=1e-3):
     print("wrote", out, os.path.getsize(out) // 1024, "KiB")
 
 
+DPM_TINY_STEPS = (4, 5, 16)            # both sides of lower_order_final's `steps < 15` switch
+DPM_SCHEDULE_STEPS = (4, 5, 10, 16, 20, 25)
+
+
+def _sd15_reference_ldm(seed):
+    """The reference's ControlFinetuneLDM at SD1.5 size (rank-128 finetune config) with synthetic weights.  torch.nn.init
+    is stubbed while it is built: the default init of 1.33 B parameters takes minutes and is overwritten anyway."""
+    from unittest import mock
+    ref_shims.install()
+    from cldm.model import create_model
+    yaml_path = os.path.join(ref_shims.REFERENCE_ROOT, "configs", "ctrlora_finetune_sd15_rank128.yaml")
+    keep = lambda t, *a, **k: t
+    with mock.patch.multiple(torch.nn.init, kaiming_uniform_=keep, uniform_=keep, normal_=keep, xavier_uniform_=keep):
+        model = create_model(yaml_path)
+    model.eval()
+    for sub, prefix in ((model.control_model, "control_model."), (model.model.diffusion_model, "model.diffusion_model.")):
+        shapes = {k: tuple(v.shape) for k, v in sub.state_dict().items()}
+        sub.load_state_dict(synth.synth_state_dict(shapes, seed, prefix), strict=True)
+    return model
+
+
+def _dpm_reference_sample(model, x_T, steps, cond, ucond, scale):
+    """DPMSolverSampler.sample (ldm/models/diffusion/dpm_solver/sampler.py:60-87) with the reference's own
+    NoiseScheduleVP, model_wrapper and DPM_Solver and the arguments of :72-85, on the reference model's apply_model.
+    Two substitutions where the reference cannot run on ControlLDM conditioning (DESIGN.md §7):
+      * the `.shape` check of the conditioning (:51-58) is skipped (c_concat is a list; the inference model's
+        conditioning is a list of dicts);
+      * with guidance, model_wrapper's classifier-free branch `torch.cat`s the cond dicts (dpm_solver.py:308-310), so
+        model_wrapper(guidance_type="uncond") gets a model that evaluates apply_model on cond and on uncond and combines
+        them with :312's formula, e_u + scale * (e_c - e_u).  Without guidance the classifier-free branch runs as is."""
+    from ldm.models.diffusion.dpm_solver.dpm_solver import DPM_Solver, NoiseScheduleVP, model_wrapper
+    ns = NoiseScheduleVP('discrete', alphas_cumprod=model.alphas_cumprod.clone().detach().to(torch.float32))
+    if ucond is None or scale == 1.:
+        model_fn = model_wrapper(lambda x, t, c: model.apply_model(x, t, c), ns, model_type="noise",
+                                 guidance_type="classifier-free", condition=cond, unconditional_condition=ucond,
+                                 guidance_scale=scale)
+    else:
+        def guided(x, t):
+            e_c, e_u = model.apply_model(x, t, cond), model.apply_model(x, t, ucond)
+            return e_u + scale * (e_c - e_u)
+        model_fn = model_wrapper(guided, ns, model_type="noise", guidance_type="uncond")
+    dpm_solver = DPM_Solver(model_fn, ns, predict_x0=True, thresholding=False)
+    with torch.no_grad():
+        return dpm_solver.sample(x_T.clone(), steps=steps, skip_type="time_uniform", method="multistep", order=2,
+                                 lower_order_final=True)
+
+
+def _dpm_schedule_record(alphas_cumprod, steps):
+    """Per step of the reference's multistep loop (dpm_solver.py:1044-1074), from its own objects at batch 1: the step
+    time, the model input time the wrapper hands apply_model, alpha / sigma / lambda there, and the update coefficients
+    read back from multistep_dpm_solver_update through probe inputs: x = 1 -> c_x; m = m_prev = 1 -> -c_m;
+    m = 0, m_prev = -1 -> -(c_d * inv_r0)."""
+    from ldm.models.diffusion.dpm_solver.dpm_solver import DPM_Solver, NoiseScheduleVP, model_wrapper
+    ns = NoiseScheduleVP('discrete', alphas_cumprod=alphas_cumprod)
+    seen = []
+
+    def record(x, t_input):
+        seen.append(t_input.clone())
+        return torch.zeros_like(x)
+    dpm = DPM_Solver(model_wrapper(record, ns, model_type="noise", guidance_type="uncond"), ns, predict_x0=True)
+    dpm.sample(torch.zeros(1, 1), steps=steps, skip_type="time_uniform", method="multistep", order=2, lower_order_final=True)
+    ts = dpm.get_time_steps(skip_type="time_uniform", t_T=ns.T, t_0=1. / ns.total_N, N=steps, device="cpu")
+    one, zero = torch.ones(1, 1), torch.zeros(1, 1)
+    rec = {"t": [], "model_time": [float(v[0]) for v in seen], "alpha": [], "sigma": [], "lambda": [], "order": [],
+           "c_x": [], "neg_c_m": [], "neg_c_d_inv_r0": []}
+    for i in range(steps):
+        s = ts[i].expand(1)
+        order = 1 if i == 0 else (min(2, steps - i) if steps < 15 else 2)
+        rec["t"].append(float(s[0]))
+        rec["alpha"].append(float(ns.marginal_alpha(s)[0]))
+        rec["sigma"].append(float(ns.marginal_std(s)[0]))
+        rec["lambda"].append(float(ns.marginal_lambda(s)[0]))
+        rec["order"].append(order)
+        t_prev = [ts[max(i - 1, 0)].expand(1), s]
+        upd = lambda x, m1, m0: float(dpm.multistep_dpm_solver_update(x, [m1, m0], t_prev, ts[i + 1].expand(1), order)[0, 0])
+        rec["c_x"].append(upd(one, zero, zero))
+        rec["neg_c_m"].append(upd(zero, one, one))
+        rec["neg_c_d_inv_r0"].append(upd(zero, -one, zero) if order == 2 else 0.0)
+    return rec
+
+
+def dpm(seed=0, full=False):
+    """The reference's DPMSolverSampler (see _dpm_reference_sample): final samples from a seeded x_T.
+      default: tiny finetune config, steps 4 / 5 / 16, with and without CFG 7.5; tiny 2-LoRA inference config, steps 5
+        with CFG 7.5 and lora_weights [0.7, 0.3]; and the host schedule for the SD1.5 alphas_cumprod
+        (_dpm_schedule_record, steps 4 / 5 / 10 / 16 / 20 / 25);
+      --dpm-full: SD1.5 rank 128, batch 1, 64x64 latent, steps 3 with CFG 7.5 (order-1 start, order 2, order-1 end)."""
+    if full:
+        model = _sd15_reference_ldm(seed)
+        model.encode_first_stage = lambda h: h
+        model.get_first_stage_encoding = lambda h: h
+        B, R = 1, 64
+        x_T = synth.synth_input("dpm_xT", (B, 4, R, R), seed)
+        hint = synth.synth_input("hint", (B, 4, R, R), seed)
+        ctx, uc = synth.synth_input("ctx", (B, 77, 768), seed), synth.synth_input("uc_ctx", (B, 77, 768), seed)
+        cond, ucond = {"c_crossattn": [ctx], "c_concat": [hint]}, {"c_crossattn": [uc], "c_concat": [hint]}
+        t0 = time.time()
+        g = {"seed": seed, "B": B, "R": R, "steps": 3, "scale": 7.5,
+             "samples": _dpm_reference_sample(model, x_T, 3, cond, ucond, 7.5)}
+        print("sampled in", time.time() - t0, "s")
+        out = os.path.join(GOLD, "sd15_dpm_golden.pt")
+        save_golden(g, out)
+        print("wrote", out, os.path.getsize(out) // 1024, "KiB")
+        return
+    B, H = 2, 16
+    x_T = synth.synth_input("dpm_xT", (B, 4, H, H), seed)
+    hint, hint2 = synth.synth_input("hint", (B, 4, H, H), seed), synth.synth_input("hint2", (B, 4, H, H), seed)
+    ctx, uc = synth.synth_input("ctx", (B, 77, 64), seed), synth.synth_input("uc_ctx", (B, 77, 64), seed)
+    g = {"seed": seed, "B": B, "H": H, "scale": 7.5, "finetune": {}, "inference": {}}
+    model = build_reference(os.path.join(GOLD, "tiny_finetune.yaml"), seed)
+    model.encode_first_stage = lambda h: h
+    model.get_first_stage_encoding = lambda h: h
+    cond, ucond = {"c_crossattn": [ctx], "c_concat": [hint]}, {"c_crossattn": [uc], "c_concat": [hint]}
+    for S in DPM_TINY_STEPS:
+        g["finetune"][(S, 1.0)] = _dpm_reference_sample(model, x_T, S, cond, None, 1.0)
+        g["finetune"][(S, 7.5)] = _dpm_reference_sample(model, x_T, S, cond, ucond, 7.5)
+    model = build_reference(_variant_yaml("inference"), seed)
+    model.encode_first_stage = lambda h: h
+    model.get_first_stage_encoding = lambda h: h
+    model.lora_weights = [0.7, 0.3]
+    g["inference_lora_weights"] = [0.7, 0.3]
+    conds = [{"c_crossattn": [ctx], "c_concat": [hint]}, {"c_crossattn": [ctx], "c_concat": [hint2]}]
+    uconds = [{"c_crossattn": [uc], "c_concat": [hint]}, {"c_crossattn": [uc], "c_concat": [hint2]}]
+    g["inference"][(5, 7.5)] = _dpm_reference_sample(model, x_T, 5, conds, uconds, 7.5)
+    # host schedule for the SD1.5 alphas_cumprod (the configs' linear schedule, 0.00085 .. 0.012)
+    from ldm.modules.diffusionmodules.util import make_beta_schedule
+    betas = make_beta_schedule("linear", 1000, linear_start=0.00085, linear_end=0.012)
+    ac = torch.tensor(np.cumprod(1. - betas, axis=0), dtype=torch.float32)
+    g["sd15_alphas_cumprod"] = ac
+    g["schedule"] = {S: _dpm_schedule_record(ac, S) for S in DPM_SCHEDULE_STEPS}
+    out = os.path.join(GOLD, "tiny_dpm_golden.pt")
+    save_golden(g, out)
+    print("wrote", out, os.path.getsize(out) // 1024, "KiB")
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
+    ap.add_argument("--dpm", action="store_true")
+    ap.add_argument("--dpm-full", action="store_true")
     ap.add_argument("--accum", action="store_true")
     ap.add_argument("--full", action="store_true")
     ap.add_argument("--variants", action="store_true")
@@ -739,5 +878,9 @@ if __name__ == "__main__":
         accum()
     elif a.resume:
         resume()
+    elif a.dpm:
+        dpm()
+    elif a.dpm_full:
+        dpm(full=True)
     else:
         tiny()
