@@ -22,7 +22,9 @@ import numbers
 import torch
 
 EXTRA_KEY = "ctrlora_b200"
-IGNORED_PREFIXES = ("cond_stage_model.",)  # CLIP is not part of the drop-in (DESIGN.md §9)
+IGNORED_PREFIXES = ("cond_stage_model.",)  # CLIP, unless the model opted into ctrlora_b200.text_encoder (DESIGN.md §9)
+# a buffer transformers 4 persisted in SD1.5 files and transformers 5 does not; the text encoder has no such key
+CLIP_POSITION_IDS = "cond_stage_model.transformer.text_model.embeddings.position_ids"
 
 
 def _host(flat, shape):
@@ -178,10 +180,17 @@ def model_state_dict(model):
 
 def checkpoint_weights(sd, expected, alias=lambda k: False):
     """The file's weights restricted to what the model holds: keys of modules the drop-in does not ship
-    (IGNORED_PREFIXES) and aliases (`alias(key)`) are dropped; any other difference from `expected` (the model's
+    (IGNORED_PREFIXES, unless the model holds such keys itself: a model built with the text encoder loads its CLIP
+    weights like any other) and aliases (`alias(key)`) are dropped; any other difference from `expected` (the model's
     state_dict()) in keys or shapes raises before anything is loaded."""
-    keep = {k: v for k, v in sd.items() if not k.startswith(IGNORED_PREFIXES) and not alias(k)}
-    want = {k for k in expected if not k.startswith(IGNORED_PREFIXES) and not alias(k)}
+    if any(k.startswith(IGNORED_PREFIXES) for k in expected):
+        def dropped(k):
+            return k == CLIP_POSITION_IDS or alias(k)
+    else:
+        def dropped(k):
+            return k.startswith(IGNORED_PREFIXES) or alias(k)
+    keep = {k: v for k, v in sd.items() if not dropped(k)}
+    want = {k for k in expected if not dropped(k)}
     missing = [k for k in expected if k in want and k not in keep]
     unexpected = [k for k in keep if k not in want]
     if missing or unexpected:

@@ -256,7 +256,11 @@ class DDIMSampler(object):
         if self._graph is None or self._graph_key != key:
             cached = self._graphs.pop(key, None)  # a sampler alternates between at most a few keys (run mode on / off)
             if cached is None:
-                fn = lambda xx, tt, *cs: self.model.apply_model(xx, tt, self._rebuild(keys, list(cs)))
+                # the callable must not refer to the sampler: the sampler holds the graph, and a cycle through it would
+                # keep a dropped sampler's graph pools (and its model) on the device until a cyclic collection, which a
+                # process that has called gc.freeze() never runs
+                model, rebuild = self.model, self._rebuild
+                fn = lambda xx, tt, *cs: model.apply_model(xx, tt, rebuild(keys, list(cs)))
                 cached = GraphedCallable(fn, [x, t] + tensors, adopt_inputs=persistent)
             if self._graph is not None:
                 self._graphs[self._graph_key] = self._graph

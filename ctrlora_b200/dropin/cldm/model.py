@@ -50,13 +50,28 @@ class skip_param_init:
             setattr(torch.nn.init, n, f)
 
 
-def create_model(config_path, init_weights=True):
+TEXT_ENCODER_TARGET = "ctrlora_b200.text_encoder.FrozenCLIPEmbedder"
+
+
+def create_model(config_path, init_weights=True, text_encoder=False):
+    """Build the model of `config_path` on the CPU.  text_encoder=True builds this package's CLIP text encoder
+    (ctrlora_b200.text_encoder.FrozenCLIPEmbedder) as `cond_stage_model`, from the config's cond_stage_config params;
+    a dict also overrides those params (e.g. {"version": local_dir, "layer": "hidden", "layer_idx": -2}).  Without it
+    cond_stage_model is whatever the config's target resolves to (None when it is not importable)."""
     config = load_config(config_path)
     model_cfg = config["model"] if isinstance(config, dict) else config.model
+    if text_encoder:
+        cond = model_cfg["params"].get("cond_stage_config")
+        params = dict(cond.get("params") or {}) if cond is not None and not isinstance(cond, str) else {}
+        if isinstance(text_encoder, dict):
+            params.update(text_encoder)
+        model_cfg["params"]["cond_stage_config"] = {"target": TEXT_ENCODER_TARGET, "params": params}
     if init_weights:
         model = instantiate_from_config(model_cfg).cpu()
     else:
         with skip_param_init():
             model = instantiate_from_config(model_cfg).cpu()
+    if text_encoder and getattr(model, "cond_stage_model", None) is None:
+        raise RuntimeError(f"{config_path}: the text encoder ({TEXT_ENCODER_TARGET}) could not be built")
     print(f'Loaded model config from [{config_path}]')
     return model

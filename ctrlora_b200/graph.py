@@ -28,9 +28,9 @@ class GraphedCallable:
                 fn(*self.static_in)
         cur.wait_stream(side)
         torch.cuda.synchronize()
-        # A dropped sampler's graph is cyclic garbage (its callable closes over the sampler). Collected in the middle of
-        # this capture, its destruction is an illegal call while capturing and invalidates the capture; so collect
-        # now, and not during the capture.
+        # A dropped graph that is cyclic garbage (a callable closing over the graph's owner), collected in the middle of
+        # this capture, is destroyed by an illegal call while capturing and invalidates the capture; so collect now,
+        # and not during the capture.
         gc.collect()
         gc_was_enabled = gc.isenabled()
         gc.disable()

@@ -807,6 +807,59 @@ def conv_dgrad_weight(w16):
     return out
 
 
+# ------------------------------------------------------------------------------------------------ CLIP text encoder
+def causal_attention(q, k, vt, batch, heads, n, out=None):
+    """Causal self-attention, d_head 64, n <= 128: q, k [batch*n, heads*64] (row strides free), vt [batch, heads, 64,
+    nk_pad] (fp16) -> [batch*n, heads*64]."""
+    _require_cuda(q, k, vt)
+    if out is None:
+        out = torch.empty((batch * n, heads * 64), device=q.device, dtype=torch.float16)
+    _count()
+    check(_lib.load().ctrlora_causal_attention_f16(_dp(q), q.stride(0), _dp(k), k.stride(0), _dp(vt), vt.shape[-1], _dp(out),
+                                                   out.stride(0), batch, heads, n, 64, _sp()), "ctrlora_causal_attention_f16")
+    return out
+
+
+def clip_embed(ids, token_embedding, position_embedding, out_f32=True, out=None):
+    """ids int64 [B, n] (device) -> token_embedding[ids] + position_embedding[:n], [B*n, C] fp32 (or fp16)"""
+    _require_cuda(ids, token_embedding, position_embedding)
+    assert ids.dtype == torch.int64 and ids.is_contiguous() and ids.dim() == 2
+    assert token_embedding.dtype == position_embedding.dtype == torch.float32
+    assert token_embedding.is_contiguous() and position_embedding.is_contiguous()
+    b, n = ids.shape
+    vocab, cols = token_embedding.shape
+    assert position_embedding.shape[0] >= n and position_embedding.shape[1] == cols
+    if out is None:
+        out = torch.empty((b * n, cols), device=ids.device, dtype=torch.float32 if out_f32 else torch.float16)
+    _count()
+    check(_lib.load().ctrlora_clip_embed(_dp(ids), _dp(token_embedding), _dp(position_embedding), _dp(out),
+                                         int(out.dtype == torch.float32), b, n, cols, vocab, _sp()), "clip_embed")
+    return out
+
+
+def quick_gelu_(x):
+    """x * sigmoid(1.702 x) in place on a contiguous fp16 tensor"""
+    _require_cuda(x)
+    assert x.dtype == torch.float16 and x.is_contiguous()
+    _count()
+    check(_lib.load().ctrlora_quick_gelu_f16(_dp(x), x.numel(), _sp()), "quick_gelu")
+    return x
+
+
+def layernorm_rows(x, gamma, beta, eps=1e-5, out_f32=False, out=None):
+    """LayerNorm over the last dim of x fp32 or fp16 [rows, C] (row stride free) -> fp32 or fp16 [rows, C]"""
+    _require_cuda(x)
+    assert x.dim() == 2 and x.stride(1) == 1 and x.dtype in (torch.float32, torch.float16)
+    rows, cols = x.shape
+    if out is None:
+        out = torch.empty((rows, cols), device=x.device, dtype=torch.float32 if out_f32 else torch.float16)
+    _count()
+    check(_lib.load().ctrlora_layernorm_rows(_dp(x), int(x.dtype == torch.float32), x.stride(0), _dp(out),
+                                             int(out.dtype == torch.float32), out.stride(0), rows, cols, _dp(gamma), _dp(beta),
+                                             float(eps), _sp()), "layernorm_rows")
+    return out
+
+
 def set_sm_limit(limit):
     """persistent GEMM grids use at most `limit` SMs (0 = all); baked into CUDA graphs at capture"""
     check(_lib.load().ctrlora_set_sm_limit(int(limit)), "set_sm_limit")

@@ -1146,9 +1146,9 @@ class FinetuneTrainer:
 
     def load_checkpoint(self, path):
         """Load a checkpoint written by save_checkpoint or by the reference's Lightning trainer into this trainer, in
-        place: the weights through model.load_state_dict (keys of cond_stage_model, which the drop-in does not ship, are
-        ignored), then load_state_dict of optimizer_states[0] and checkpoint.EXTRA_KEY.  Everything is validated before
-        anything changes.  Trainable-weight copies are rebuilt, and captured graphs are re-captured (the frozen-weight
+        place: the weights through model.load_state_dict (keys of cond_stage_model are ignored unless the model was built
+        with the text encoder), then load_state_dict of optimizer_states[0] and checkpoint.EXTRA_KEY.  Everything is
+        validated before anything changes.  Trainable-weight copies are rebuilt, and captured graphs are re-captured (the frozen-weight
         copies they read are built outside the capture).  Every rank of a data-parallel run loads the same file.
         Returns {"epoch", "global_step"} of the file."""
         ckpt = torch.load(path, map_location="cpu", weights_only=True)

@@ -279,6 +279,25 @@ int ctrlora_nonfinite_flag_f32(const float* x, long long n, int* flag, void* str
  * the weighted control sum of multi-LoRA inference, cldm/cldm_ctrlora_inference.py:172-176.  srcs / weights: HOST arrays. */
 int ctrlora_weighted_sum_f16(const void* const* srcs, const float* weights, int count, void* out, long long n, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * CLIP text encoder (FrozenCLIPEmbedder, ldm/modules/encoders/modules.py:88-135, running transformers' CLIPTextModel).
+ * Causal self-attention of CLIPAttention with its causal mask and no padding mask (the embedder passes no
+ * attention_mask, :118-121): out[b, i, h*64:(h+1)*64] = sum_{j <= i} softmax_j(q_i . k_j / 8) v_j, fp32 logits and
+ * softmax.  Operands as for ctrlora_attention_f16 (q, k [batch, n, heads*64], V^T [batch, heads, 64, nk_pad]); only
+ * keys < n of V^T are read.  head_dim != 64 or n > 128: CTRLORA_STATUS_UNSUPPORTED. */
+int ctrlora_causal_attention_f16(const void* q, long long ldq, const void* k, long long ldk, const void* vt, int nk_pad,
+                                 void* out, long long ldo, int batch, int heads, int n, int head_dim, void* stream);
+/* CLIPTextEmbeddings: out[b*n + t, :] = token_embedding[ids[b, t], :] + position_embedding[t, :] (fp32 tables [*, cols],
+ * ids int64 [batch, n]); out fp32 or fp16 [batch*n, cols].  An id outside [0, vocab) fills its row with NaN. */
+int ctrlora_clip_embed(const long long* ids, const float* token_embedding, const float* position_embedding, void* out,
+                       int out_f32, int batch, int n, int cols, int vocab, void* stream);
+/* quick-GELU x * sigmoid(1.702 x) (CLIP's hidden_act), fp32 math, in place on fp16 [n] (n % 8 == 0) */
+int ctrlora_quick_gelu_f16(void* x, long long n, void* stream);
+/* LayerNorm over the last dim with fp32 or fp16 input and output (x_f32 / y_f32): the CLIP encoder's layer_norm1/2 and
+ * final_layer_norm on its fp32 residual stream.  cols % 4 == 0, cols <= 2048. */
+int ctrlora_layernorm_rows(const void* x, int x_f32, long long ldx, void* y, int y_f32, long long ldy, int rows, int cols,
+                           const float* gamma, const float* beta, float eps, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
