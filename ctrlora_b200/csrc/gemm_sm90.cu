@@ -5,9 +5,11 @@
 // A tiles are TMA boxes over the (C, W, H, B) activation tensor: a filter tap is a coordinate shift and the conv zero
 // padding is the TMA out-of-bounds fill, so no im2col buffer exists in HBM.  The grid is persistent: each CTA walks a
 // static list of 128 x BN output tiles (BN up to 320), a producer thread fills a ring of TMA stages, and two consumer
-// warpgroups (64 rows each) run wgmma with accumulators in registers, then run a row-per-thread epilogue through a
-// staging buffer of their own while the producer already loads the next tile.  Tiles of a last, partial wave may be
-// split along K.
+// warpgroups (64 rows each) run wgmma with accumulators in registers, then run the epilogue while the producer already
+// loads the next tile.  fp16 row-major outputs leave through shared-memory slots that a second thread of the producer
+// warpgroup stores by TMA and into which it has loaded the tile's residual ahead of time, so that epilogue never waits
+// on global memory; everything else (fp32, transposed or unaligned outputs, split tiles) takes a row-per-thread
+// epilogue through a staging buffer.  Tiles of a last, partial wave may be split along K.
 #include "gemm_sm90.cuh"
 #include "wgmma.cuh"
 #include "ctrlora_b200.h"
@@ -16,6 +18,7 @@
 
 namespace ctrl {
 
+__device__ __forceinline__ bool aligned16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; }
 __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
     __half2 h = __floats2half2_rn(a, b);
     return *reinterpret_cast<uint32_t*>(&h);
@@ -31,7 +34,7 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, float* v, i
     if (!row_ok) return;
     if (p.rowbias) {
         const float* rb = p.rowbias + static_cast<long long>(img) * p.rowbias_ld + nbase;
-        if (full_chunk && (p.rowbias_ld & 3) == 0) {
+        if (full_chunk && aligned16(rb)) {
 #pragma unroll
             for (int q = 0; q < CW / 4; ++q) {
                 const float4 b4 = __ldg(reinterpret_cast<const float4*>(rb) + q);
@@ -49,7 +52,7 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, float* v, i
     }
     if (p.residual && p.residual_f32) {
         const float* rp = reinterpret_cast<const float*>(p.residual) + m * p.ldr + nbase;
-        if (full_chunk && (p.ldr & 3) == 0) {  // LoRA folds: W (fp32 master) + s * up . down
+        if (full_chunk && aligned16(rp)) {  // LoRA folds: W (fp32 master) + s * up . down
 #pragma unroll
             for (int q = 0; q < CW / 4; ++q) {
                 const float4 r4 = __ldg(reinterpret_cast<const float4*>(rp) + q);
@@ -62,7 +65,7 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, float* v, i
         }
     } else if (p.residual) {
         const __half* rp = p.residual + m * p.ldr + nbase;
-        if (full_chunk && (p.ldr & 7) == 0) {
+        if (full_chunk && aligned16(rp)) {
             uint4 u[CW / 8];
 #pragma unroll
             for (int q = 0; q < CW / 8; ++q) u[q] = __ldg(reinterpret_cast<const uint4*>(rp) + q);
@@ -97,7 +100,7 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, float* v, i
         }
     } else if (p.out_f32) {
         float* o = reinterpret_cast<float*>(p.out[seg]) + m * p.ldc + nloc;
-        if (full_chunk && (p.ldc & 3) == 0) {
+        if (full_chunk && aligned16(o)) {
 #pragma unroll
             for (int q = 0; q < CW / 4; ++q)
                 reinterpret_cast<float4*>(o)[q] = make_float4(v[q * 4], v[q * 4 + 1], v[q * 4 + 2], v[q * 4 + 3]);
@@ -108,7 +111,7 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, float* v, i
         }
     } else {
         __half* o = reinterpret_cast<__half*>(p.out[seg]) + m * p.ldc + nloc;
-        if (full_chunk && (p.ldc & 7) == 0) {
+        if (full_chunk && aligned16(o)) {
 #pragma unroll
             for (int q = 0; q < CW / 8; ++q) {
                 uint4 u;
@@ -158,20 +161,51 @@ __device__ __forceinline__ uint32_t epi_addr(uint32_t base, int r, int col) {
 // Persistent: CTA b runs work units b, b + gridDim.x, ...  The producer thread walks the same sequence, so it fills
 // the ring for the next unit while the consumers run the epilogue of the current one; the ring position (stage,
 // phase) carries across units.  CTAs never wait on each other, so correctness does not depend on co-residency.
+//
+// TMA epilogue.  A tile's output is cut into slabs of SW = 64 (32 where 64 does not divide the tile) columns; slab j of
+// the CTA's q-th such tile is number q * NSLAB + j of one sequence that the consumers and the epilogue thread both walk,
+// through p.epi_slots slots.  The epilogue thread opens a slot (loads the residual slab into it, or just marks it free:
+// slot_ready), the consumers add it to their fragment, write the fp16 result over it and arrive on slot_done, the
+// epilogue thread stores the slot through the output map and opens it for the slab epi_slots further on once the
+// store has read it.  A tile reads only its own residual box and stores after that box has arrived, so the output may
+// alias the residual.  The tiles that take this epilogue come first in every CTA's list (p.tma_tiles); the
+// row-per-thread epilogue of the later units reuses the slots' memory after `drained`.
+// In a slot, row r is SW * 2 bytes and its 16-byte chunk c sits at chunk c ^ (r & 7) (SW = 64, SWIZZLE_128B) or
+// c ^ ((r >> 1) & 3) (SW = 32, SWIZZLE_64B).
+__host__ __device__ constexpr int gemm_slab_cols(int bn_out) { return bn_out % 64 == 0 ? 64 : 32; }
+__device__ __forceinline__ uint32_t lds32(uint32_t addr) {
+    uint32_t v;
+    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) {
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ float2 h2_to_f2(uint32_t u) { return __half22float2(*reinterpret_cast<const __half2*>(&u)); }
+
 template <bool GEGLU, int BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
+                  const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmO0,
+                  const __grid_constant__ CUtensorMap tmO1, const __grid_constant__ CUtensorMap tmO2,
                   const __grid_constant__ GemmKParams p) {
     constexpr int BN_OUT = GEGLU ? BN / 2 : BN;
     constexpr int NACC = BN / 2;  // fp32 accumulators per consumer thread (64 rows x BN per warpgroup)
     constexpr int BOX = GEGLU || BN > 256 ? BN / 2 : BN;  // rows of one B TMA box: a tile is one box or two
+    constexpr int SW = gemm_slab_cols(BN_OUT);            // columns of a TMA epilogue slab
+    constexpr int NSLAB_TMA = BN_OUT / SW;
+    constexpr int SLOT = GEMM_BM * SW * 2;                // bytes of a slot
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + GEMM_SMEM_DATA + GEMM_EPI_BYTES);
+    uint8_t* ring = smem + p.epi_slots * SLOT;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + GEMM_SMEM_DATA);
     uint64_t* full = bars;
     uint64_t* empty = bars + GEMM_MAX_STAGES;
-    volatile int* last_flag = reinterpret_cast<volatile int*>(bars + 2 * GEMM_MAX_STAGES);
+    uint64_t* slot_ready = bars + 2 * GEMM_MAX_STAGES;
+    uint64_t* slot_done = slot_ready + GEMM_MAX_SLOTS;
+    uint64_t* drained = slot_done + GEMM_MAX_SLOTS;
+    volatile int* last_flag = reinterpret_cast<volatile int*>(drained + 1);
 
     pdl_launch_dependents();
     const int warp = uniform_warp_idx();
@@ -188,6 +222,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             mbar_init(&full[i], 1);
             mbar_init(&empty[i], GEMM_CONSUMERS);
         }
+        for (int i = 0; i < p.epi_slots; ++i) {
+            mbar_init(&slot_ready[i], 1);
+            mbar_init(&slot_done[i], GEMM_CONSUMERS);
+        }
+        mbar_init(drained, 1);
         fence_barrier_init();
     }
     __syncthreads();
@@ -210,7 +249,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 const int w0 = tw * p.bw - p.pad, h0 = th * p.bh - p.pad, b0 = tb * p.nb, n0 = w.nt * BN_OUT;
                 for (int it = w.it0; it < w.it1; ++it) {
                     mbar_wait_nocall(&empty[s], phase ^ 1);
-                    uint8_t* dst = smem + s * p.stage_bytes;
+                    uint8_t* dst = ring + s * p.stage_bytes;
                     mbar_expect_tx(&full[s], tx_bytes);
                     if (it < main_iters) {
                         const int tap = it / p.kchunks, kc = it - tap * p.kchunks, ky = tap / p.kw, kx = tap - ky * p.kw;
@@ -227,6 +266,48 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     if (++s == nstages) { s = 0; phase ^= 1; }
                 }
             }
+        } else if (warp == 1 && p.tma_tiles > 0 && elect_one()) {
+            // ------------------------------------------------ epilogue thread: residual loads and output stores
+            const int nslots = p.epi_slots;
+            // slab (u, j): open its slot
+            auto open = [&](int u, int j, int slot) {
+                if (!p.residual) { mbar_arrive(&slot_ready[slot]); return; }
+                const int mt = u % m_tiles, nt = u / m_tiles;
+                const int tw = mt % p.tiles_w, th = (mt / p.tiles_w) % p.tiles_h, tb = mt / (p.tiles_w * p.tiles_h);
+                mbar_expect_tx(&slot_ready[slot], GEMM_BM * SW * 2);
+                tma_load_4d(smem + slot * SLOT, &tmR, &slot_ready[slot], nt * BN_OUT + j * SW, tw * p.bw, th * p.bh,
+                            tb * p.nb);
+            };
+            int ou = blockIdx.x, oj = 0;  // the next slab to open
+            for (int k = 0; k < nslots && ou < p.tma_tiles; ++k) {
+                open(ou, oj, k);
+                if (++oj == NSLAB_TMA) { oj = 0; ou += gridDim.x; }
+            }
+            int slot = 0, prev_slot = -1;
+            uint32_t phase = 0;
+            for (int u = blockIdx.x; u < p.tma_tiles; u += gridDim.x) {
+                const int mt = u % m_tiles, nt = u / m_tiles;
+                const int tw = mt % p.tiles_w, th = (mt / p.tiles_w) % p.tiles_h, tb = mt / (p.tiles_w * p.tiles_h);
+                for (int j = 0; j < NSLAB_TMA; ++j) {
+                    int col = nt * BN_OUT + j * SW, seg = 0;
+                    if (p.seg_width > 0) { seg = col / p.seg_width; col -= seg * p.seg_width; }
+                    mbar_wait_nocall(&slot_done[slot], phase);
+                    tma_store_4d(seg == 0 ? &tmO0 : seg == 1 ? &tmO1 : &tmO2, smem_u32(smem + slot * SLOT), col,
+                                 tw * p.bw, th * p.bh, tb * p.nb);
+                    bulk_commit_group();
+                    if (prev_slot >= 0) {
+                        bulk_wait_group_read<1>();  // the store before this one has read its slot
+                        if (ou < p.tma_tiles) {
+                            open(ou, oj, prev_slot);
+                            if (++oj == NSLAB_TMA) { oj = 0; ou += gridDim.x; }
+                        }
+                    }
+                    prev_slot = slot;
+                    if (++slot == nslots) { slot = 0; phase ^= 1; }
+                }
+            }
+            bulk_wait_group<0>();
+            mbar_arrive(drained);
         }
         return;  // the consumers synchronise among themselves only (named barriers 1-3)
     }
@@ -235,13 +316,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     setmaxnreg_inc<GEMM_CONSUMER_REGS>();
     const int ct = threadIdx.x - 128;  // 0..255
     const int wg = ct >> 7, t = ct & 127;
-    const uint32_t smem0 = smem_u32(smem);
-    const uint32_t stg = smem0 + GEMM_SMEM_DATA + wg * (64 * GEMM_EPI_COLS * 4);
+    const uint32_t ring0 = smem_u32(ring);
     const int fr = ((t >> 5) << 4) + (lane >> 2), cq = 2 * (lane & 3);  // accumulator fragment: rows fr, fr + 8
     const int er = t & 63, eh = t >> 6;                                  // epilogue: row er, 32-column half eh of a slab
     const long long slice = static_cast<long long>(GEMM_BM) * BN;       // floats of one split-K workspace slice
     int s = 0;
-    uint32_t phase = 0;
+    uint32_t phase = 0, slot_pos = 0;  // slot_pos: the TMA epilogue's slot, its phase in bit 16
     for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
         const GemmUnit w = gemm_unit(p, u, m_tiles, k_iters);
         float acc[NACC];
@@ -250,8 +330,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         int prev = -1;
         for (int it = w.it0; it < w.it1; ++it) {
             mbar_wait_nocall(&full[s], phase);
-            const uint32_t a_base = smem0 + s * p.stage_bytes + wg * 64 * 128;
-            const uint32_t b_base = smem0 + s * p.stage_bytes + GEMM_A_BYTES;
+            const uint32_t a_base = ring0 + s * p.stage_bytes + wg * 64 * 128;
+            const uint32_t b_base = ring0 + s * p.stage_bytes + GEMM_A_BYTES;
             wgmma_fence();
 #pragma unroll
             for (int k = 0; k < GEMM_BK / 16; ++k) {
@@ -329,8 +409,63 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
             for (int i = 0; i < BN_OUT / 8; ++i) bias_geglu(i);
         }
-        // ---- the rest of the epilogue, one 64-column slab at a time through this warpgroup's staging buffer
         const int tw = w.mt % p.tiles_w, th = (w.mt / p.tiles_w) % p.tiles_h, tb = w.mt / (p.tiles_w * p.tiles_h);
+        if (u < p.tma_tiles) {
+            // ---- TMA epilogue on the fragment: time-embedding row term, scale, residual, one rounding, each in the
+            // order of the row-per-thread epilogue.  A thread owns rows fr and fr + 8 of its warpgroup's 64; a warp's
+            // 4-byte accesses to one 16-byte chunk of 8 rows fall on 8 different chunk positions: no bank conflicts.
+            const uint32_t row_off = (wg * 64 + fr) * (SW * 2) + cq * 2, row_x = SW == 64 ? (fr & 7) : ((fr >> 1) & 3);
+            const float* rb0 = nullptr;
+            const float* rb1 = nullptr;
+            if (p.rowbias) {
+                auto row_img = [&](int r) {  // image of tile row r (a tile can span several); 0 for rows past the end
+                    const int iw = r % p.bw, ih = (r / p.bw) % p.bh, ib = r / (p.bw * p.bh);
+                    const int gw = tw * p.bw + iw, gh = th * p.bh + ih, gb = tb * p.nb + ib;
+                    if (gw >= p.W || gh >= p.H || gb >= p.Bn) return 0LL;
+                    return ((static_cast<long long>(gb) * p.H + gh) * p.W + gw) / p.rows_per_img;
+                };
+                rb0 = p.rowbias + row_img(wg * 64 + fr) * p.rowbias_ld;
+                rb1 = p.rowbias + row_img(wg * 64 + fr + 8) * p.rowbias_ld;
+            }
+#pragma unroll
+            for (int j = 0; j < NSLAB_TMA; ++j) {
+                const int slot = slot_pos & 0xffff;
+                mbar_wait_nocall(&slot_ready[slot], slot_pos >> 16);
+                const uint32_t sb = ring0 - (p.epi_slots - slot) * SLOT + row_off;
+#pragma unroll
+                for (int c = 0; c < SW / 8; ++c) {
+                    const int i = j * (SW / 8) + c;
+                    if (!GEGLU) bias_geglu(i);
+                    float v00 = acc[4 * i], v01 = acc[4 * i + 1], v10 = acc[4 * i + 2], v11 = acc[4 * i + 3];
+                    const int n = n0 + 8 * i + cq;
+                    if (rb0) {
+                        if (n < p.N) { v00 = __fadd_rn(v00, __ldg(rb0 + n)); v10 = __fadd_rn(v10, __ldg(rb1 + n)); }
+                        if (n + 1 < p.N) { v01 = __fadd_rn(v01, __ldg(rb0 + n + 1)); v11 = __fadd_rn(v11, __ldg(rb1 + n + 1)); }
+                    }
+                    if (p.out_scale != 1.0f) {
+                        v00 = __fmul_rn(v00, p.out_scale); v01 = __fmul_rn(v01, p.out_scale);
+                        v10 = __fmul_rn(v10, p.out_scale); v11 = __fmul_rn(v11, p.out_scale);
+                    }
+                    const uint32_t a0 = sb + ((static_cast<uint32_t>(c) ^ row_x) << 4);
+                    const uint32_t a1 = a0 + 8 * SW * 2;
+                    if (p.residual) {
+                        const float2 r0 = h2_to_f2(lds32(a0)), r1 = h2_to_f2(lds32(a1));
+                        v00 = __fadd_rn(v00, r0.x); v01 = __fadd_rn(v01, r0.y);
+                        v10 = __fadd_rn(v10, r1.x); v11 = __fadd_rn(v11, r1.y);
+                    }
+                    sts32(a0, pack_h2(v00, v01));
+                    sts32(a1, pack_h2(v10, v11));
+                }
+                fence_proxy_async_smem();  // the slot is stored by TMA
+                mbar_arrive(&slot_done[slot]);
+                slot_pos = slot + 1 == p.epi_slots ? (slot_pos & 0x10000) ^ 0x10000 : slot_pos + 1;
+            }
+            continue;
+        }
+        // ---- the rest of the epilogue, one 64-column slab at a time through this warpgroup's staging buffer
+        // the staging buffer is slot memory: the TMA epilogue's last stores have left it (the barrier completes once)
+        if (p.tma_tiles > 0) mbar_wait_nocall(drained, 0);
+        const uint32_t stg = ring0 - p.epi_slots * SLOT + wg * (64 * GEMM_EPI_COLS * 4);
         const int r = wg * 64 + er;
         const int iw = r % p.bw, ih = (r / p.bw) % p.bh, ib = r / (p.bw * p.bh);
         const int gw = tw * p.bw + iw, gh = th * p.bh + ih, gb = tb * p.nb + ib;
@@ -457,10 +592,9 @@ static constexpr int GEMM_WIDE_MIN_KITERS = 40;
 static bool g_attr_set = false;
 
 template <bool GEGLU, int BN>
-static cudaError_t launch_gemm(dim3 grid, cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB,
-                               const CUtensorMap& tmA2, const CUtensorMap& tmB2, const GemmKParams& p) {
-    return launch_pdl(gemm_wgmma_kernel<GEGLU, BN>, grid, dim3(GEMM_THREADS), (size_t)GEMM_SMEM_BYTES, stream, tmA, tmB, tmA2,
-                      tmB2, p);
+static cudaError_t launch_gemm(dim3 grid, cudaStream_t stream, const CUtensorMap* tm, const GemmKParams& p) {
+    return launch_pdl(gemm_wgmma_kernel<GEGLU, BN>, grid, dim3(GEMM_THREADS), (size_t)GEMM_SMEM_BYTES, stream, tm[0], tm[1],
+                      tm[2], tm[3], tm[4], tm[5], tm[6], tm[7], p);
 }
 template <bool GEGLU, int BN>
 static bool set_smem_attr() {
@@ -522,12 +656,16 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
     };
     int bn_out = 0, splits = 1, tiles_whole = 0;
     double best_cost = -1;
-    static const int kWidths[] = {GEMM_MAX_BN, 256, 128, 64, 32};  // tile widths; GEGLU tiles carry half as many outputs
-    for (int wi = 0; wi < 5; ++wi) {
+    // tile widths; GEGLU tiles carry half as many outputs (and have no 80 + 80 tile)
+    static const int kWidths[] = {GEMM_MAX_BN, 256, 160, 128, 64, 32};
+    for (int wi = 0; wi < 6; ++wi) {
         const int cand = p.geglu ? kWidths[wi] / 2 : kWidths[wi];
-        if (cand < 32) continue;
+        if (cand < 32 || (p.geglu && kWidths[wi] == 160)) continue;
         if (a->block_n > 0 && cand != a->block_n) continue;
         if (a->block_n <= 0 && kWidths[wi] > 256 && k_iters < GEMM_WIDE_MIN_KITERS) continue;
+        // 160 columns are the exact tile of N = 320 on the short loops that exclude 320; on long ones the model chose
+        // them for split tiles of the 8x8 level, which measured 30-40 % slower than its choice without them
+        if (a->block_n <= 0 && kWidths[wi] == 160 && k_iters >= GEMM_WIDE_MIN_KITERS) continue;
         if (a->seg_width > 0 && a->seg_width % cand != 0) continue;
         for (int S = explicit_split ? a->split_k : 1; S <= (explicit_split ? a->split_k : GEMM_MAX_AUTO_SPLIT); ++S) {
             int s_eff, whole;
@@ -551,10 +689,35 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
         p.ws = a->splitk_ws;
         p.counters = a->splitk_counters;
     }
-    p.stage_bytes = GEMM_A_BYTES + ((p.BN * 128 + 1023) / 1024) * 1024;
-    p.stages = GEMM_SMEM_DATA / p.stage_bytes;
-    if (p.stages > GEMM_MAX_STAGES) p.stages = GEMM_MAX_STAGES;
     for (int i = 0; i < 3; ++i) { p.out[i] = a->out[i]; p.transposed[i] = a->transposed[i]; }
+    // ---- which tiles take the TMA epilogue: fp16 row-major outputs and an fp16 (or no) residual that tensor maps can
+    // address.  The segments it serves must come first (q and k of a q | k | V^T launch), so that every CTA runs its
+    // TMA-epilogue tiles before the others; split tiles keep the row-per-thread epilogue (only the CTA that arrives
+    // last knows that it needs the residual).
+    const int n_segs = a->seg_width > 0 ? (p.N + a->seg_width - 1) / a->seg_width : 1;
+    if (n_segs > 3) return CTRLORA_ERR_ARG;
+    auto tma_ok = [](const void* ptr, long long ld) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && ld % 8 == 0; };
+    int tma_segs = 0;
+    while (tma_segs < n_segs && !a->transposed[tma_segs]) ++tma_segs;
+    bool tma_epi = !a->out_f32 && tma_segs > 0 && (!a->residual || (!a->residual_f32 && tma_ok(a->residual, a->ldr)));
+    for (int i = 0; i < n_segs; ++i) {
+        if (i < tma_segs ? !a->out[i] || !tma_ok(a->out[i], a->ldc) : !a->transposed[i]) tma_epi = false;
+    }
+    if (tma_epi) {
+        const long long t = tma_segs == n_segs ? (long long)m_tiles * p.n_tiles : (long long)m_tiles * tma_segs * (a->seg_width / bn_out);
+        p.tma_tiles = (int)(t < tiles_whole ? t : tiles_whole);
+    }
+    // shared memory: slots for one tile's slabs if the ring keeps 3 stages, and what is left over after whole stages
+    const int slab_cols = gemm_slab_cols(bn_out);
+    const int slot_bytes = GEMM_BM * slab_cols * 2;
+    int epi_want = p.tma_tiles > 0 ? (bn_out / slab_cols) * slot_bytes : GEMM_EPI_BYTES;
+    if (epi_want < GEMM_EPI_BYTES) epi_want = GEMM_EPI_BYTES;
+    p.stage_bytes = GEMM_A_BYTES + ((p.BN * 128 + 1023) / 1024) * 1024;
+    p.stages = (GEMM_SMEM_DATA - epi_want) / p.stage_bytes;
+    if (p.stages < 3) p.stages = 3;
+    if (p.stages > GEMM_MAX_STAGES) p.stages = GEMM_MAX_STAGES;
+    p.epi_slots = (GEMM_SMEM_DATA - p.stages * p.stage_bytes) / slot_bytes;
+    if (p.epi_slots > GEMM_MAX_SLOTS) p.epi_slots = GEMM_MAX_SLOTS;
     p.seg_width = a->seg_width;
     p.ldc = a->ldc; p.out_f32 = a->out_f32;
     p.bias = a->bias; p.rowbias = a->rowbias;
@@ -567,7 +730,8 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
     p.dup_out = reinterpret_cast<__half*>(a->dup_out); p.dup_ld = a->dup_ld;
 
     const int b_box = p.geglu || p.BN > 256 ? p.BN / 2 : p.BN;  // rows of a B box (the kernel's BOX)
-    CUtensorMap tmA, tmB, tmA2, tmB2;
+    CUtensorMap tm[8];  // A, B, A2, B2, residual, out[0..2]
+    CUtensorMap &tmA = tm[0], &tmB = tm[1], &tmA2 = tm[2], &tmB2 = tm[3];
     {
         uint64_t dims[4] = {(uint64_t)a->a_c, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)p.Bn};
         uint64_t str[3] = {(uint64_t)a->a_ld * 2, (uint64_t)a->a_ld * 2 * p.W, (uint64_t)a->a_ld * 2 * p.W * p.H};
@@ -597,24 +761,46 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
         tmA2 = tmA;
         tmB2 = tmB;
     }
+    for (int i = 4; i < 8; ++i) tm[i] = tmA;
+    if (p.tma_tiles > 0) {
+        // the residual and the outputs have the geometry of A with C = N (a segment: seg_width): the map clips partial
+        // tiles, and a column slice of a wider buffer (ld > N) keeps its neighbours
+        const CUtensorMapSwizzle swz = slab_cols == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+        const uint32_t box[4] = {(uint32_t)slab_cols, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.nb};
+        auto pixel_map = [&](CUtensorMap* m, const void* base, int cols, long long ld) {
+            uint64_t dims[4] = {(uint64_t)cols, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)p.Bn};
+            uint64_t str[3] = {(uint64_t)ld * 2, (uint64_t)ld * 2 * p.W, (uint64_t)ld * 2 * p.W * p.H};
+            return make_tmap_f16_sw(m, base, 4, dims, str, box, swz);
+        };
+        if (a->residual) {
+            int rc = pixel_map(&tm[4], a->residual, p.N, a->ldr);
+            if (rc) return rc;
+        }
+        for (int i = 0; i < tma_segs; ++i) {
+            const int cols = a->seg_width > 0 ? (p.N - i * a->seg_width < a->seg_width ? p.N - i * a->seg_width : a->seg_width) : p.N;
+            int rc = pixel_map(&tm[5 + i], a->out[i], cols, a->ldc);
+            if (rc) return rc;
+        }
+    }
     if (!g_attr_set) {
         if (!set_smem_attr<false, 32>() || !set_smem_attr<false, 64>() || !set_smem_attr<false, 128>() ||
-            !set_smem_attr<false, 256>() || !set_smem_attr<false, 320>() || !set_smem_attr<true, 64>() ||
+            !set_smem_attr<false, 160>() || !set_smem_attr<false, 256>() || !set_smem_attr<false, 320>() || !set_smem_attr<true, 64>() ||
             !set_smem_attr<true, 128>() || !set_smem_attr<true, 256>() || !set_smem_attr<true, 320>())
             return CTRLORA_ERR_CUDA;
         g_attr_set = true;
     }
     const dim3 grid((unsigned)(p.units < sms ? p.units : sms));
     cudaError_t lrc;
-    if (p.geglu) lrc = p.BN == 64  ? launch_gemm<true, 64>(grid, stream, tmA, tmB, tmA2, tmB2, p)
-                     : p.BN == 128 ? launch_gemm<true, 128>(grid, stream, tmA, tmB, tmA2, tmB2, p)
-                     : p.BN == 256 ? launch_gemm<true, 256>(grid, stream, tmA, tmB, tmA2, tmB2, p)
-                                   : launch_gemm<true, 320>(grid, stream, tmA, tmB, tmA2, tmB2, p);
-    else lrc = p.BN == 32  ? launch_gemm<false, 32>(grid, stream, tmA, tmB, tmA2, tmB2, p)
-             : p.BN == 64  ? launch_gemm<false, 64>(grid, stream, tmA, tmB, tmA2, tmB2, p)
-             : p.BN == 128 ? launch_gemm<false, 128>(grid, stream, tmA, tmB, tmA2, tmB2, p)
-             : p.BN == 256 ? launch_gemm<false, 256>(grid, stream, tmA, tmB, tmA2, tmB2, p)
-                           : launch_gemm<false, 320>(grid, stream, tmA, tmB, tmA2, tmB2, p);
+    if (p.geglu) lrc = p.BN == 64  ? launch_gemm<true, 64>(grid, stream, tm, p)
+                     : p.BN == 128 ? launch_gemm<true, 128>(grid, stream, tm, p)
+                     : p.BN == 256 ? launch_gemm<true, 256>(grid, stream, tm, p)
+                                   : launch_gemm<true, 320>(grid, stream, tm, p);
+    else lrc = p.BN == 32  ? launch_gemm<false, 32>(grid, stream, tm, p)
+             : p.BN == 64  ? launch_gemm<false, 64>(grid, stream, tm, p)
+             : p.BN == 128 ? launch_gemm<false, 128>(grid, stream, tm, p)
+             : p.BN == 160 ? launch_gemm<false, 160>(grid, stream, tm, p)
+             : p.BN == 256 ? launch_gemm<false, 256>(grid, stream, tm, p)
+                           : launch_gemm<false, 320>(grid, stream, tm, p);
     if (lrc != cudaSuccess) return CTRLORA_ERR_CUDA;
     return cudaGetLastError() == cudaSuccess ? CTRLORA_OK : CTRLORA_ERR_CUDA;
 }

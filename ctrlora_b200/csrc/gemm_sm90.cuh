@@ -15,10 +15,15 @@ constexpr int GEMM_THREADS = 384;       // warpgroup 0: TMA producer (one thread
 constexpr int GEMM_CONSUMERS = 256;
 constexpr int GEMM_PRODUCER_REGS = 40;  // setmaxnreg split: 128 * 40 + 256 * 232 <= 64 K registers
 constexpr int GEMM_CONSUMER_REGS = 232;
-constexpr int GEMM_SMEM_DATA = 192 * 1024;            // operand ring (the producer fills it during the epilogue)
-constexpr int GEMM_EPI_COLS = 64;                     // epilogue slab: 64 rows x 64 fp32 columns per consumer warpgroup
+// Shared memory: [epilogue slots][operand ring][barriers].  The host divides GEMM_SMEM_DATA between the two per tile
+// width (GemmKParams::epi_slots, stages).
+constexpr int GEMM_SMEM_DATA = 225 * 1024;
+constexpr int GEMM_EPI_COLS = 64;                     // row-per-thread epilogue: 64 rows x 64 fp32 columns per warpgroup
 constexpr int GEMM_EPI_BYTES = 2 * 64 * GEMM_EPI_COLS * 4;  // 32 KiB, 16-byte chunks XOR-swizzled by row
-constexpr int GEMM_SMEM_BYTES = GEMM_SMEM_DATA + GEMM_EPI_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+// TMA epilogue: a slot holds one slab of the output tile, 128 rows x 64 (or 32) fp16 columns in the layout of a
+// SWIZZLE_128B (SWIZZLE_64B) box.  The residual slab is loaded into it, the result is written over it and stored from it.
+constexpr int GEMM_MAX_SLOTS = 8;
+constexpr int GEMM_SMEM_BYTES = GEMM_SMEM_DATA + 1024 /*align slack*/ + 512 /*barriers*/;
 
 struct GemmKParams {
     // tile geometry over the (B, H, W) pixel grid; a plain [M, K] matrix is B=1, H=1, W=M
@@ -33,6 +38,8 @@ struct GemmKParams {
     int kchunks2;                   // extra 1x1 segment from the second operand pair (0 = none)
     int geglu;                      // 1: weights are [2N, K]; out = value * gelu(gate)
     int stages, stage_bytes;        // TMA ring: stage = A tile (16 KiB) + B tile (BN * 128 B, 1 KiB aligned); 3 at BN 320
+    int epi_slots;                  // epilogue slots in front of the ring (GEMM_EPI_BYTES or more)
+    int tma_tiles;                  // whole tiles [0, tma_tiles) run the TMA epilogue, every later unit the row-per-thread one
     // persistent schedule: work unit u < tiles_whole is output tile u over the whole K range; the units after it are
     // the remaining tiles split `splits` ways along K (partial sums meet in `ws`, fp32; the self-cleaning counter of
     // the tile picks the last-arriving CTA, which sums the slices in slice order and runs the epilogue)

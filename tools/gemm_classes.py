@@ -37,10 +37,12 @@ def model_cycles(a, sms, widths, m=MODEL):
     m_tiles = -(-a.a_w // bw) * -(-a.a_h // bh) * -(-a.a_b // nb)
     k_iters = a.kh * a.kw * -(-a.a_c // 64) + (-(-a.a2_c // 64) if a.a2 else 0)
     best = None
-    for cand in ([w // 2 for w in widths if w >= 64] if a.geglu else widths):
+    for cand in ([w // 2 for w in widths if w >= 64 and w != 160] if a.geglu else widths):  # no 80 + 80 GEGLU tile
         if a.seg_width and a.seg_width % cand:
             continue
         if (2 * cand if a.geglu else cand) > 256 and k_iters < 40:  # GEMM_WIDE_MIN_KITERS
+            continue
+        if not a.geglu and cand == 160 and k_iters >= 40:  # 160 only where 320 is excluded
             continue
         bnt = 2 * cand if a.geglu else cand
         tiles = m_tiles * -(-a.n // cand)
@@ -98,7 +100,7 @@ def main():
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--json", default=None)
     ap.add_argument("--sm-scaling", action="store_true")
-    ap.add_argument("--widths", default="320,256,128,64,32", help="tile widths the model chooses among")
+    ap.add_argument("--widths", default="320,256,160,128,64,32", help="tile widths the model chooses among")
     ap.add_argument("--clock-mhz", type=float, default=1980.0, help="SM clock the model's cycles are converted at")
     args = ap.parse_args()
     device = torch.device("cuda", 0)
