@@ -115,6 +115,9 @@ _ARGTYPES = {
     "ctrlora_clip_embed": [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P],
     "ctrlora_quick_gelu_f16": [_P, _L, _P],
     "ctrlora_layernorm_rows": [_P, _I, _L, _P, _I, _L, _I, _I, _P, _P, _F, _P],
+    "ctrlora_clip_patch_gather": [_P, _I, _P, _I, _I, _I, _I, _I, _P],
+    "ctrlora_clip_vision_embed": [_P, _L, _P, _P, _P, _I, _I, _I, _P],
+    "ctrlora_gelu_f16": [_P, _L, _P],
 }
 
 
@@ -186,4 +189,7 @@ EXPORTS = [
     "ctrlora_clip_embed",
     "ctrlora_quick_gelu_f16",
     "ctrlora_layernorm_rows",
+    "ctrlora_clip_patch_gather",
+    "ctrlora_clip_vision_embed",
+    "ctrlora_gelu_f16",
 ]

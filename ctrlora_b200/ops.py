@@ -860,6 +860,52 @@ def layernorm_rows(x, gamma, beta, eps=1e-5, out_f32=False, out=None):
     return out
 
 
+# ------------------------------------------------------------------------------------------------ CLIP image encoder
+def clip_patch_gather(pixels, patch, k_pad, out=None):
+    """pixels fp32 or fp16 [B, C, S, S] (contiguous) -> fp16 patch rows [B * (S/patch)^2, k_pad] in the Conv2d weight's
+    (c, kh, kw) column order, zero beyond C * patch^2"""
+    _require_cuda(pixels)
+    assert pixels.dim() == 4 and pixels.is_contiguous() and pixels.dtype in (torch.float32, torch.float16)
+    b, c, s, s2 = pixels.shape
+    assert s == s2 and s % patch == 0
+    rows = b * (s // patch) ** 2
+    if out is None:
+        out = torch.empty((rows, k_pad), device=pixels.device, dtype=torch.float16)
+    assert out.shape == (rows, k_pad) and out.is_contiguous() and out.dtype == torch.float16
+    _count()
+    check(_lib.load().ctrlora_clip_patch_gather(_dp(pixels), int(pixels.dtype == torch.float32), _dp(out), b, c, s, patch,
+                                                k_pad, _sp()), "clip_patch_gather")
+    return out
+
+
+def clip_vision_embed(patch_out, class_embedding, position_embedding, batch, out=None):
+    """patch_out fp32 [batch * P, C] (row stride free) -> fp32 [batch * (P + 1), C]: per image the class embedding, then
+    its P patch rows, each plus its position embedding"""
+    _require_cuda(patch_out, class_embedding, position_embedding)
+    assert patch_out.dtype == class_embedding.dtype == position_embedding.dtype == torch.float32 and patch_out.stride(1) == 1
+    assert class_embedding.is_contiguous() and position_embedding.is_contiguous()
+    rows, cols = patch_out.shape
+    patches = rows // batch
+    assert rows == batch * patches and position_embedding.shape == (patches + 1, cols) and class_embedding.numel() == cols
+    if out is None:
+        out = torch.empty((batch * (patches + 1), cols), device=patch_out.device, dtype=torch.float32)
+    assert out.shape == (batch * (patches + 1), cols) and out.is_contiguous() and out.dtype == torch.float32
+    _count()
+    check(_lib.load().ctrlora_clip_vision_embed(_dp(patch_out), patch_out.stride(0), _dp(class_embedding),
+                                                _dp(position_embedding), _dp(out), batch, patches, cols, _sp()),
+          "clip_vision_embed")
+    return out
+
+
+def gelu_(x):
+    """exact GELU 0.5 x (1 + erf(x / sqrt 2)) in place on a contiguous fp16 tensor"""
+    _require_cuda(x)
+    assert x.dtype == torch.float16 and x.is_contiguous()
+    _count()
+    check(_lib.load().ctrlora_gelu_f16(_dp(x), x.numel(), _sp()), "gelu")
+    return x
+
+
 def set_sm_limit(limit):
     """persistent GEMM grids use at most `limit` SMs (0 = all); baked into CUDA graphs at capture"""
     check(_lib.load().ctrlora_set_sm_limit(int(limit)), "set_sm_limit")

@@ -8,7 +8,8 @@ weights come from the checkpoint, and the tokenizer is built on the first call t
 
 Per layer the forward is four ctrlora_gemm_f16 launches (one stacked q|k|v GEMM that stores V transposed, out_proj +
 residual, fc1, fc2 + residual), ctrlora_causal_attention_f16, ctrlora_quick_gelu_f16 and two ctrlora_layernorm_rows.
-The residual stream stays fp32 like the reference's (CLIP-L's activations carry large outliers at the EOS position,
+That layer loop (`run_layers`) is shared with the image-prompt towers of `image_encoder.py`, which add exact GELU and
+full (non-causal) attention.  The residual stream stays fp32 like the reference's (CLIP-L's activations carry large outliers at the EOS position,
 which an fp16 stream rounds coarsely; DESIGN.md §3 has the measured errors of both).
 It is inference only: no autograd, parameters frozen.
 """
@@ -37,15 +38,21 @@ def text_config(version):
             raw = json.load(f)
         raw = raw.get("text_config", raw)
         cfg.update({k: raw[k] for k in cfg if k in raw})
-    if cfg["hidden_act"] != "quick_gelu":
-        raise ValueError(f"CLIP text config of {version!r}: hidden_act {cfg['hidden_act']!r}, only quick_gelu is implemented")
+    check_text_config(cfg, version, ("quick_gelu",))
+    return cfg
+
+
+def check_text_config(cfg, version, acts):
+    """raise ValueError unless the causal d_head-64 layer loop runs `cfg` (hidden_act one of `acts`)"""
+    if cfg["hidden_act"] not in acts:
+        raise ValueError(f"CLIP text config of {version!r}: hidden_act {cfg['hidden_act']!r}, only "
+                         f"{' / '.join(acts)} is implemented")
     if cfg["hidden_size"] != 64 * cfg["num_attention_heads"]:
         raise ValueError(f"CLIP text config of {version!r}: head size {cfg['hidden_size']} / {cfg['num_attention_heads']}, "
                          "the causal attention kernel takes 64")
     if cfg["max_position_embeddings"] > 128:
         raise ValueError(f"CLIP text config of {version!r}: {cfg['max_position_embeddings']} positions, at most 128 are "
                          "supported")
-    return cfg
 
 
 class _Embeddings(nn.Module):
@@ -103,6 +110,70 @@ class _Transformer(nn.Module):
     def __init__(self, cfg):
         super().__init__()
         self.text_model = _TextModel(cfg)
+
+
+def pooled_rows(ids, eos):
+    """the EOS row of each sequence, as transformers' CLIPTextTransformer picks it: the largest token id when the
+    config's eos_token_id is 2 (the original CLIP configs), else the first occurrence of eos_token_id"""
+    if eos == 2:
+        return ids.to(torch.int).argmax(dim=-1)
+    return (ids.to(torch.int) == eos).int().argmax(dim=-1)
+
+
+def layer_weights(prep, layer, i):
+    """kernel copies of CLIP encoder layer i from `prep` (a PrepCache): fp16 stacked q|k|v [3C, 1, C] + fp32 bias,
+    out_proj, fc1 and fc2 as (fp16 [N, 1, K], fp32 bias), and layer_norm1 / layer_norm2 as fp32 (gamma, beta, eps).
+    fp32 parameters are used as they are; fp16 ones (a module moved with .to(dtype=torch.float16)) get fp32 copies."""
+    at, mlp = layer.self_attn, layer.mlp
+    lins = (at.q_proj, at.k_proj, at.v_proj)
+
+    def qkv():
+        c = at.q_proj.in_features
+        w = torch.empty((3 * c, 1, c), device=at.q_proj.weight.device, dtype=torch.float16)
+        for j, lin in enumerate(lins):
+            prepare.linear_weight(lin.weight, out=w[j * c:(j + 1) * c])
+        return w, torch.cat([prepare.bias_f32(lin.bias) for lin in lins])
+
+    def lin(m):
+        return lambda: (prepare.linear_weight(m.weight), prepare.bias_f32(m.bias))
+
+    def ln(m):
+        return lambda: (prepare.bias_f32(m.weight), prepare.bias_f32(m.bias), m.eps)
+
+    get = prep.get
+    return (get(("qkv", i), [p for m in lins for p in (m.weight, m.bias)], qkv),
+            get(("out", i), [at.out_proj.weight, at.out_proj.bias], lin(at.out_proj)),
+            get(("fc1", i), [mlp.fc1.weight, mlp.fc1.bias], lin(mlp.fc1)),
+            get(("fc2", i), [mlp.fc2.weight, mlp.fc2.bias], lin(mlp.fc2)),
+            get(("ln1", i), [layer.layer_norm1.weight, layer.layer_norm1.bias], ln(layer.layer_norm1)),
+            get(("ln2", i), [layer.layer_norm2.weight, layer.layer_norm2.bias], ln(layer.layer_norm2)))
+
+
+def run_layers(layers, prep, h, b, n, heads, hidden_act, causal, f32=True):
+    """CLIPEncoder over `layers` on the residual stream h ([b * n, C], fp32 when f32, else fp16): per layer
+    layer_norm1, one stacked q|k|v GEMM that stores V transposed, self-attention (causal d_head 64, or the full
+    ctrlora_attention_f16), out_proj + residual, layer_norm2, fc1, GELU (hidden_act "quick_gelu" or "gelu", in place),
+    fc2 + residual.  Returns the new residual stream."""
+    dev = h.device
+    c = h.shape[1]
+    d = c // heads
+    n_pad = (n + 7) // 8 * 8
+    act = {"quick_gelu": ops.quick_gelu_, "gelu": ops.gelu_}[hidden_act]
+    for i, layer in enumerate(layers):
+        (w_qkv, b_qkv), (w_out, b_out), (w_fc1, b_fc1), (w_fc2, b_fc2), ln1, ln2 = layer_weights(prep, layer, i)
+        x = ops.layernorm_rows(h, *ln1)
+        q = torch.empty((b * n, c), device=dev, dtype=torch.float16)
+        k = torch.empty_like(q)
+        vt = torch.empty((b, heads, d, n_pad), device=dev, dtype=torch.float16)
+        ops.gemm(x, w_qkv, bias=b_qkv, seg_outs=[q, k, vt], seg_width=c, transposed=(0, 0, 1), rows_per_img=n, head_dim=d,
+                 tok_pad=n_pad)
+        a = ops.causal_attention(q, k, vt, b, heads, n) if causal else ops.attention(q, k, vt, b, heads, n, n, d)
+        h = ops.gemm(a, w_out, bias=b_out, residual=h, out_f32=f32)
+        x = ops.layernorm_rows(h, *ln2)
+        f = ops.gemm(x, w_fc1, bias=b_fc1)
+        act(f)
+        h = ops.gemm(f, w_fc2, bias=b_fc2, residual=h, out_f32=f32)
+    return h
 
 
 class FrozenCLIPEmbedder(nn.Module):
@@ -170,28 +241,6 @@ class FrozenCLIPEmbedder(nn.Module):
         return self(text)
 
     # ---- the encoder on the kernels ------------------------------------------------------------------------------------
-    def _weights(self, i):
-        """fp16 kernel copies of layer i: stacked q|k|v [3C, 1, C] + fp32 bias, out_proj, fc1, fc2"""
-        layer = self.transformer.text_model.encoder.layers[i]
-        at, mlp = layer.self_attn, layer.mlp
-        lins = (at.q_proj, at.k_proj, at.v_proj)
-
-        def qkv():
-            c = at.q_proj.in_features
-            w = torch.empty((3 * c, 1, c), device=at.q_proj.weight.device, dtype=torch.float16)
-            for j, lin in enumerate(lins):
-                prepare.linear_weight(lin.weight, out=w[j * c:(j + 1) * c])
-            return w, torch.cat([prepare.bias_f32(lin.bias) for lin in lins])
-
-        def lin(m):
-            return lambda: (prepare.linear_weight(m.weight), prepare.bias_f32(m.bias))
-
-        get = self._prep.get
-        return (get(("qkv", i), [p for m in lins for p in (m.weight, m.bias)], qkv),
-                get(("out", i), [at.out_proj.weight, at.out_proj.bias], lin(at.out_proj)),
-                get(("fc1", i), [mlp.fc1.weight, mlp.fc1.bias], lin(mlp.fc1)),
-                get(("fc2", i), [mlp.fc2.weight, mlp.fc2.bias], lin(mlp.fc2)))
-
     def _depth(self):
         """(number of encoder layers to run, apply final_layer_norm)"""
         n_layers = self.config["num_hidden_layers"]
@@ -203,12 +252,7 @@ class FrozenCLIPEmbedder(nn.Module):
         return n_layers, True
 
     def _pooled_rows(self, ids):
-        """the EOS row of each sequence, as transformers' CLIPTextTransformer picks it: the largest token id when the
-        config's eos_token_id is 2 (the original CLIP configs), else the first occurrence of eos_token_id"""
-        eos = self.config["eos_token_id"]
-        if eos == 2:
-            return ids.to(torch.int).argmax(dim=-1)
-        return (ids.to(torch.int) == eos).int().argmax(dim=-1)
+        return pooled_rows(ids, self.config["eos_token_id"])
 
     @torch.no_grad()
     def encode_tokens(self, ids):
@@ -226,22 +270,7 @@ class FrozenCLIPEmbedder(nn.Module):
         depth, final_ln = self._depth()
         f32 = self.residual_f32
         h = ops.clip_embed(ids_dev, tm.embeddings.token_embedding.weight, tm.embeddings.position_embedding.weight, out_f32=f32)
-        n_pad = (n + 7) // 8 * 8
-        for i in range(depth):
-            layer = tm.encoder.layers[i]
-            (w_qkv, b_qkv), (w_out, b_out), (w_fc1, b_fc1), (w_fc2, b_fc2) = self._weights(i)
-            x = ops.layernorm_rows(h, layer.layer_norm1.weight, layer.layer_norm1.bias, layer.layer_norm1.eps)
-            q = torch.empty((b * n, c), device=dev, dtype=torch.float16)
-            k = torch.empty_like(q)
-            vt = torch.empty((b, heads, 64, n_pad), device=dev, dtype=torch.float16)
-            ops.gemm(x, w_qkv, bias=b_qkv, seg_outs=[q, k, vt], seg_width=c, transposed=(0, 0, 1), rows_per_img=n, head_dim=64,
-                     tok_pad=n_pad)
-            a = ops.causal_attention(q, k, vt, b, heads, n)
-            h = ops.gemm(a, w_out, bias=b_out, residual=h, out_f32=f32)
-            x = ops.layernorm_rows(h, layer.layer_norm2.weight, layer.layer_norm2.bias, layer.layer_norm2.eps)
-            f = ops.gemm(x, w_fc1, bias=b_fc1)
-            ops.quick_gelu_(f)
-            h = ops.gemm(f, w_fc2, bias=b_fc2, residual=h, out_f32=f32)
+        h = run_layers(tm.encoder.layers[:depth], self._prep, h, b, n, heads, "quick_gelu", causal=True, f32=f32)
         if final_ln:
             ln = tm.final_layer_norm
             h = ops.layernorm_rows(h, ln.weight, ln.bias, ln.eps, out_f32=True)

@@ -298,6 +298,24 @@ int ctrlora_quick_gelu_f16(void* x, long long n, void* stream);
 int ctrlora_layernorm_rows(const void* x, int x_f32, long long ldx, void* y, int y_f32, long long ldy, int rows, int cols,
                            const float* gamma, const float* beta, float eps, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * IP-Adapter image encoder (app/gradio_ctrlora_style_transfer.py:385-409, running transformers'
+ * CLIPVisionModelWithProjection and, for the negative content prompt, CLIPTextModelWithProjection).
+ * Patch gather for CLIPVisionEmbeddings.patch_embedding (transformers models/clip/modeling_clip.py, Conv2d with
+ * kernel = stride = patch and no bias), which then runs as one ctrlora_gemm_f16 with a [C, 1, k_pad] weight:
+ * pixels fp32 (pixels_f32 = 1) or fp16 NCHW [batch, channels, image, image] -> fp16 [batch * P, k_pad], P = (image/patch)^2,
+ * row b * P + py * (image/patch) + px, column c * patch^2 + kh * patch + kw; columns >= channels * patch^2 are zero.
+ * image % patch == 0, k_pad % 8 == 0. */
+int ctrlora_clip_patch_gather(const void* pixels, int pixels_f32, void* out, int batch, int channels, int image, int patch,
+                              int k_pad, void* stream);
+/* CLIPVisionEmbeddings.forward after the conv: out[b * (P+1) + t, :] = (t == 0 ? class_embedding : patch_out[b * P + t-1, :])
+ * + position_embedding[t, :], fp32 throughout (patch_out row stride ldp); pre_layrnorm follows as ctrlora_layernorm_rows. */
+int ctrlora_clip_vision_embed(const float* patch_out, long long ldp, const float* class_embedding,
+                              const float* position_embedding, float* out, int batch, int patches, int cols, void* stream);
+/* exact GELU 0.5 x (1 + erf(x / sqrt 2)) (transformers' GELUActivation, hidden_act "gelu" of the ViT-H/14 image and text
+ * towers), fp32 math, in place on fp16 [n] (n % 8 == 0) */
+int ctrlora_gelu_f16(void* x, long long n, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
