@@ -147,8 +147,9 @@ class CrossAttention(nn.Module):
                     hit[1].shape[0] == batch * nk:
                 return self._finish(ops.attention(q, hit[1], hit[2], batch, h, nq, nk, d), q, batch, nq, residual)
             k = torch.empty((batch * nk, inner), device=dev, dtype=torch.float16)
-            # key padding columns (77 -> 80) are never written by the projection: they must hold finite values (their
-            # probabilities are exactly 0, but 0 x NaN from recycled memory would poison the row) -> zero-initialised
+            # the key padding columns (77 -> 80) are never written by the projection, and ops.attention never reads
+            # them: its V^T tensor map ends at key nk, so keys >= nk load as zeros.  The zero fill is not needed for
+            # correctness.
             vt = ops.zeros((batch, h, d, nk_pad), dev) if nk_pad != nk else torch.empty((batch, h, d, nk_pad), device=dev, dtype=torch.float16)
             w = self._cat_weight("kv", [self.to_k, self.to_v])
             ops.gemm(ctx2d, w, seg_outs=[k, vt], seg_width=inner, transposed=(0, 1, 0), rows_per_img=nk, head_dim=d,

@@ -66,7 +66,9 @@ class IPCrossAttention(CrossAttention):
         h, d = self.heads, inner // self.heads
         nk_pad = (nk + 7) // 8 * 8
         k_ip = torch.empty((batch * nk, inner), device=q.device, dtype=torch.float16)
-        vt_ip = ops.zeros((batch, h, d, nk_pad), q.device)  # key padding columns must be finite (probability exactly 0)
+        # the key padding (4 -> 8) is neither written by the projection nor read by ops.attention (its V^T map ends at
+        # key nk); the zero fill is not needed for correctness
+        vt_ip = ops.zeros((batch, h, d, nk_pad), q.device)
         w = self._cat_weight("kv_ip", [self.to_k_ip, self.to_v_ip])
         ops.gemm(ip2d, w, seg_outs=[k_ip, vt_ip], seg_width=inner, transposed=(0, 1, 0), rows_per_img=nk, head_dim=d,
                  tok_pad=nk_pad)
