@@ -110,6 +110,7 @@ _ARGTYPES = {
     "ctrlora_q_sample": [_P, _P, _P, _P, _P, _P, _I, _I, _P],
     "ctrlora_ddim_encode_update": [_P, _P, _P, _P, _I, _F, _F, _F, _P],
     "ctrlora_dpm_multistep_update": [_P, _P, _P, _P, _P, _P, _I, _F, _F, _F, _F, _F, _F, _F, _P],
+    "ctrlora_plms_update": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _F, _F, _F, _F, _F, _P],
     "ctrlora_weighted_sum_f16": [_P, _P, _I, _P, _L, _P],
     "ctrlora_causal_attention_f16": [_P, _L, _P, _L, _P, _I, _P, _L, _I, _I, _I, _I, _P],
     "ctrlora_clip_embed": [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P],
@@ -185,6 +186,7 @@ EXPORTS = [
     "ctrlora_cast_rows_f32_to_f16",
     "ctrlora_ddim_encode_update",
     "ctrlora_dpm_multistep_update",
+    "ctrlora_plms_update",
     "ctrlora_causal_attention_f16",
     "ctrlora_clip_embed",
     "ctrlora_quick_gelu_f16",

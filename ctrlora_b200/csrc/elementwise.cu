@@ -353,6 +353,54 @@ dpm_multistep_kernel(const float* __restrict__ x, const float* __restrict__ e_co
     x_next[i] = xn;
 }
 
+// PLMS step (ldm/models/diffusion/plms.py:178-244): guided e_t (:184-192) written to e_out, e' of the given order
+// (:226-240), then DDIM's pred_x0 / x_prev with e' (:205-223, sigma_t = 0).  Explicit round-to-nearest ops in torch's
+// order; the divisions by 2 / 12 / 24 are products with the fp32 reciprocal, which is what torch does on a CUDA tensor
+// divided by a Python number.
+__device__ __forceinline__ float guided_eps(const float* __restrict__ e_cond, const float* __restrict__ e_uncond, int i,
+                                            float cfg_scale) {
+    const float e = e_cond[i];
+    if (!e_uncond) return e;
+    const float u = e_uncond[i];
+    return __fadd_rn(u, __fmul_rn(cfg_scale, __fsub_rn(e, u)));
+}
+
+__global__ void __launch_bounds__(256)
+plms_update_kernel(const float* __restrict__ x, const float* __restrict__ e_cond, const float* __restrict__ e_uncond,
+                   const float* __restrict__ e_next_cond, const float* __restrict__ e_next_uncond,
+                   const float* __restrict__ old1, const float* __restrict__ old2, const float* __restrict__ old3,
+                   float* __restrict__ e_out, float* __restrict__ x_prev, float* __restrict__ pred_x0, int order, int total,
+                   float cfg_scale, float sqrt_a_t, float sqrt_one_minus_at, float sqrt_a_prev, float dir_coef) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    const float e = guided_eps(e_cond, e_uncond, i, cfg_scale);
+    float ep;
+    switch (order) {
+    case 0:   // (e_t + e_t_next) / 2
+        ep = __fmul_rn(__fadd_rn(e, guided_eps(e_next_cond, e_next_uncond, i, cfg_scale)), 0.5f);
+        break;
+    case 1:
+        ep = e;
+        break;
+    case 2:   // (3 e - o1) / 2
+        ep = __fmul_rn(__fsub_rn(__fmul_rn(3.f, e), old1[i]), 0.5f);
+        break;
+    case 3:   // (23 e - 16 o1 + 5 o2) / 12
+        ep = __fmul_rn(__fadd_rn(__fsub_rn(__fmul_rn(23.f, e), __fmul_rn(16.f, old1[i])), __fmul_rn(5.f, old2[i])),
+                       1.f / 12.f);
+        break;
+    default:  // (55 e - 59 o1 + 37 o2 - 9 o3) / 24
+        ep = __fmul_rn(__fsub_rn(__fadd_rn(__fsub_rn(__fmul_rn(55.f, e), __fmul_rn(59.f, old1[i])),
+                                           __fmul_rn(37.f, old2[i])),
+                                 __fmul_rn(9.f, old3[i])),
+                       1.f / 24.f);
+    }
+    const float p0 = __fdiv_rn(__fsub_rn(x[i], __fmul_rn(sqrt_one_minus_at, ep)), sqrt_a_t);
+    e_out[i] = e;
+    pred_x0[i] = p0;
+    x_prev[i] = __fadd_rn(__fmul_rn(sqrt_a_prev, p0), __fmul_rn(dir_coef, ep));
+}
+
 static inline unsigned blocks_for(long long total, int threads) { return static_cast<unsigned>((total + threads - 1) / threads); }
 
 }  // namespace ctrl
@@ -663,5 +711,22 @@ extern "C" int ctrlora_dpm_multistep_update(const float* x, const float* e_cond,
     if (!x || !e_cond || !m_out || !x_next || total < 0) return CTRLORA_ERR_ARG;
     dpm_multistep_kernel<<<blocks_for(total, 256), 256, 0, STREAM(stream)>>>(
         x, e_cond, e_uncond, m_prev, m_out, x_next, total, cfg_scale, sigma_s, alpha_s, c_x, c_m, c_d, inv_r0);
+    return LAUNCH_OK();
+}
+
+extern "C" int ctrlora_plms_update(const float* x, const float* e_cond, const float* e_uncond, const float* e_next_cond,
+                                   const float* e_next_uncond, const float* old1, const float* old2, const float* old3,
+                                   float* e_out, float* x_prev, float* pred_x0, int order, int total, float cfg_scale,
+                                   float sqrt_a_t, float sqrt_one_minus_at, float sqrt_a_prev, float dir_coef,
+                                   void* stream) {
+    if (!x || !e_cond || !e_out || !x_prev || !pred_x0 || total < 0 || order < 0 || order > 4) return CTRLORA_ERR_ARG;
+    // exactly the inputs the order reads: a stray pointer means the caller's history bookkeeping is wrong
+    const bool ok = order == 0 ? (e_next_cond && !old1 && !old2 && !old3 && !e_next_uncond == !e_uncond)
+                               : (!e_next_cond && !e_next_uncond && !old1 == (order < 2) && !old2 == (order < 3) &&
+                                  !old3 == (order < 4));
+    if (!ok) return CTRLORA_ERR_ARG;
+    plms_update_kernel<<<blocks_for(total, 256), 256, 0, STREAM(stream)>>>(
+        x, e_cond, e_uncond, e_next_cond, e_next_uncond, old1, old2, old3, e_out, x_prev, pred_x0, order, total,
+        cfg_scale, sqrt_a_t, sqrt_one_minus_at, sqrt_a_prev, dir_coef);
     return LAUNCH_OK();
 }

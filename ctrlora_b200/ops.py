@@ -582,6 +582,28 @@ def dpm_multistep_update(x, e_cond, e_uncond, m_prev, m_out, cfg_scale, sigma_s,
     return x_next
 
 
+def plms_update(x, e_cond, e_uncond, e_out, cfg_scale, sqrt_a_t, sqrt_one_minus_at, sqrt_a_prev, dir_coef, old=(),
+                e_next=None):
+    """One PLMS step (ldm/models/diffusion/plms.py:178-244): writes the guided eps e_t into e_out and returns
+    (x_prev, pred_x0).  e_next = (e_next_cond, e_next_uncond | None) gives step 0's average with the eval at t_next
+    (order 0); otherwise `old` = (old_eps[-1], old_eps[-2], ...) of up to 3 earlier e_t selects the Adams-Bashforth
+    order len(old) + 1.  fp32 contiguous [B,C,H,W] tensors; the scalars come from ctrlora_b200.plms_schedule."""
+    assert len(old) <= 3 and (e_next is None or not old)
+    en_c, en_u = (None, None) if e_next is None else e_next
+    o = list(old) + [None] * (3 - len(old))
+    _require_cuda(x, e_cond, e_uncond, e_out, en_c, en_u, *o)
+    for t in (x, e_cond, e_uncond, e_out, en_c, en_u, *o):
+        assert t is None or (t.dtype == torch.float32 and t.is_contiguous() and t.shape == x.shape)
+    x_prev, pred_x0 = torch.empty_like(x), torch.empty_like(x)
+    order = 0 if e_next is not None else len(old) + 1
+    _count()
+    check(_lib.load().ctrlora_plms_update(_dp(x), _dp(e_cond), _dp(e_uncond), _dp(en_c), _dp(en_u), _dp(o[0]), _dp(o[1]),
+                                          _dp(o[2]), _dp(e_out), _dp(x_prev), _dp(pred_x0), order, x.numel(),
+                                          float(cfg_scale), float(sqrt_a_t), float(sqrt_one_minus_at), float(sqrt_a_prev),
+                                          float(dir_coef), _sp()), "plms_update")
+    return x_prev, pred_x0
+
+
 def wgrad_tn(a, b, out=None, alpha=1.0, beta=0.0):
     """out[p, q] = alpha * sum_m a[m, p] * b[m, q] + beta * out  (fp16 a [M,P], b [M,Q] -> fp32 [P,Q])."""
     _require_cuda(a, b)

@@ -201,6 +201,26 @@ int ctrlora_ddim_encode_update(const float* x, const float* e_cond, const float*
 int ctrlora_dpm_multistep_update(const float* x, const float* e_cond, const float* e_uncond, const float* m_prev, float* m_out,
                                  float* x_next, int total, float cfg_scale, float sigma_s, float alpha_s, float c_x, float c_m,
                                  float c_d, float inv_r0, void* stream);
+/* One step of PLMSSampler (ldm/models/diffusion/plms.py:178-244, eta 0), fp32 with round-to-nearest ops in torch's order:
+ *   e = e_uncond + cfg * (e_cond - e_uncond) -> e_out               :184-192 (e_uncond may be NULL: no guidance); the
+ *                                                                   guided e_t the caller keeps as old_eps (:164-167)
+ *   e' = (e + e_next) / 2                       order 0             :227-231 (e_next guided from e_next_cond /
+ *                                                                   e_next_uncond, the eval at t_next on the provisional
+ *                                                                   x_prev that ctrlora_ddim_update gives)
+ *        e                                      order 1             (a DDIM step; PLMSSampler does not use it)
+ *        (3 e - o1) / 2                         order 2             :232-234
+ *        (23 e - 16 o1 + 5 o2) / 12             order 3             :235-237
+ *        (55 e - 59 o1 + 37 o2 - 9 o3) / 24     order 4             :238-240   (o1 = old_eps[-1], o2 = [-2], o3 = [-3])
+ *   pred_x0 = (x - sqrt_one_minus_at * e') / sqrt_a_t               :207-213
+ *   x_prev = sqrt_a_prev * pred_x0 + dir_coef * e'                  :219-223 (dir_coef = sqrt(1 - a_prev - sigma_t^2))
+ * The divisions are products with the fp32 reciprocal, as torch computes a CUDA tensor divided by a Python number.
+ * Inputs an order does not read must be NULL.  The scalars are computed by the caller in torch CPU fp32 ops, the
+ * reference's values as run on a CPU (whose sqrt is not always correctly rounded, unlike the sqrtf of
+ * ctrlora_ddim_update). */
+int ctrlora_plms_update(const float* x, const float* e_cond, const float* e_uncond, const float* e_next_cond,
+                        const float* e_next_uncond, const float* old1, const float* old2, const float* old3, float* e_out,
+                        float* x_prev, float* pred_x0, int order, int total, float cfg_scale, float sqrt_a_t,
+                        float sqrt_one_minus_at, float sqrt_a_prev, float dir_coef, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Training (backward of the trainable set; reference: autograd over cldm/lora.py:70-80,285-291 and cldm/cldm.py:281-282,
