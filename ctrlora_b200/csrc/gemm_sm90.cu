@@ -10,6 +10,8 @@
 // warpgroup stores by TMA and into which it has loaded the tile's residual ahead of time, so that epilogue never waits
 // on global memory; everything else (fp32, transposed or unaligned outputs, split tiles) takes a row-per-thread
 // epilogue through a staging buffer.  Tiles of a last, partial wave may be split along K.
+// Launches of whole tiles that all take the TMA epilogue and have a short K loop may run ping-pong instead: each
+// consumer warpgroup owns whole 128-row tiles and runs its epilogue while the other's MMAs run.
 #include "gemm_sm90.cuh"
 #include "wgmma.cuh"
 #include "ctrlora_b200.h"
@@ -183,7 +185,159 @@ __device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) {
 }
 __device__ __forceinline__ float2 h2_to_f2(uint32_t u) { return __half22float2(*reinterpret_cast<const __half2*>(&u)); }
 
+// Entry `idx` of a ring of n barriers walked in order from 0: barrier idx % n, in the phase of parity (idx / n) & 1.
+// The producer and the epilogue thread step through consecutive entries (slot + 1, wrapping with a phase flip); the
+// ping-pong consumers jump to the first entry of each of their tiles.  A tile is k_iters ring entries and NSLAB_TMA
+// slot entries, so tile q of a CTA starts at entry q * k_iters (q * NSLAB_TMA).
+struct RingPos {
+    int slot;
+    uint32_t phase;
+};
+__host__ __device__ __forceinline__ RingPos ring_pos(uint32_t idx, int n) {
+    return RingPos{static_cast<int>(idx % static_cast<uint32_t>(n)), (idx / static_cast<uint32_t>(n)) & 1u};
+}
+
+// Ping-pong consumers: every unit of the launch is a whole tile with the TMA epilogue.  Warpgroup wg owns the CTA's
+// tiles q = wg, wg + 2, ... (unit blockIdx.x + q * gridDim.x) and all 128 rows of each: two m64nBNk16 per k16, BN
+// accumulators per thread.  The K loops take turns (named barrier 4 + wg: the other warpgroup has issued the MMAs of
+// tile q - 1), so one warpgroup's epilogue runs while the other's MMAs occupy the tensor cores.  Each element of the
+// epilogue is computed as in the cooperative schedule, so the two give the same bits.
 template <bool GEGLU, int BN>
+__device__ __forceinline__ void gemm_pingpong_consumers(const GemmKParams& p, uint8_t* ring, uint64_t* full,
+                                                        uint64_t* empty, uint64_t* slot_ready, uint64_t* slot_done,
+                                                        int m_tiles, int k_iters) {
+    constexpr int BN_OUT = GEGLU ? BN / 2 : BN;
+    constexpr int HALF = BN / 2;  // accumulators of one 64-row half of the tile
+    constexpr int SW = gemm_slab_cols(BN_OUT);
+    constexpr int NSLAB_TMA = BN_OUT / SW;
+    constexpr int SLOT = GEMM_BM * SW * 2;
+    static_assert(BN <= 160, "ping-pong tiles hold BN accumulators per thread");
+    const int ct = threadIdx.x - 128;
+    const int wg = ct >> 7, t = ct & 127, lane = threadIdx.x & 31;
+    const uint32_t ring0 = smem_u32(ring);
+    const int fr = ((t >> 5) << 4) + (lane >> 2), cq = 2 * (lane & 3);
+    const int n_local = (p.units - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) / static_cast<int>(gridDim.x);
+    for (int q = wg; q < n_local; q += 2) {
+        const int u = blockIdx.x + q * gridDim.x;
+        const int mt = u % m_tiles, nt = u / m_tiles;
+        float acc[BN];
+#pragma unroll
+        for (int i = 0; i < BN; ++i) acc[i] = 0.f;
+        if (q > 0) named_bar_sync(4 + wg, 256);
+        RingPos rp = ring_pos(static_cast<uint32_t>(q) * k_iters, p.stages);
+        int s = rp.slot, prev = -1;
+        uint32_t phase = rp.phase;
+        for (int it = 0; it < k_iters; ++it) {
+            mbar_wait_nocall(&full[s], phase);
+            const uint32_t a_base = ring0 + s * p.stage_bytes;
+            const uint32_t b_base = a_base + GEMM_A_BYTES;
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < GEMM_BK / 16; ++k) {
+                const uint32_t sc = (it > 0 || k > 0) ? 1u : 0u;
+                const uint64_t db = wgmma_desc_kmajor(b_base + 32 * k);
+                WgmmaSS<BN, 0, 0>::mma(acc, wgmma_desc_kmajor(a_base + 32 * k), db, sc);
+                WgmmaSS<BN, 0, 0>::mma(acc + HALF, wgmma_desc_kmajor(a_base + 64 * 128 + 32 * k), db, sc);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();  // the previous stage's MMAs have finished reading it
+            if (prev >= 0) mbar_arrive(&empty[prev]);
+            prev = s;
+            if (++s == p.stages) { s = 0; phase ^= 1; }
+        }
+        if (q + 1 < n_local) named_bar_arrive(4 + (wg ^ 1), 256);  // the other warpgroup may issue tile q + 1's MMAs
+        wgmma_wait<0>();
+        wgmma_fence_regs<BN>(acc);
+        mbar_arrive(&empty[prev]);
+
+        // ---- the TMA epilogue of the cooperative schedule, over both row halves: h = 0 holds rows fr, fr + 8 of the
+        // tile in acc[0, HALF), h = 1 rows 64 + fr, 72 + fr in acc[HALF, BN)
+        const int n0 = nt * BN_OUT;
+        auto bias_geglu = [&](float* a, int i) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int n = n0 + 8 * i + cq + e;
+                float bv = 0.f, bg = 0.f;
+                if (p.bias && n < p.N) {
+                    bv = __ldg(p.bias + n);
+                    if (GEGLU) bg = __ldg(p.bias + p.N + n);
+                }
+                a[4 * i + e] += bv;
+                a[4 * i + 2 + e] += bv;
+                if (GEGLU) {
+                    a[4 * i + e] *= gelu_erf_f(a[4 * (i + BN_OUT / 8) + e] + bg);
+                    a[4 * i + 2 + e] *= gelu_erf_f(a[4 * (i + BN_OUT / 8) + 2 + e] + bg);
+                }
+            }
+        };
+        if (GEGLU) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int i = 0; i < BN_OUT / 8; ++i) bias_geglu(acc + h * HALF, i);
+        }
+        const int tw = mt % p.tiles_w, th = (mt / p.tiles_w) % p.tiles_h, tb = mt / (p.tiles_w * p.tiles_h);
+        const uint32_t row_x = SW == 64 ? (fr & 7) : ((fr >> 1) & 3);  // the same for rows fr, 64 + fr
+        const float* rb[4] = {nullptr, nullptr, nullptr, nullptr};     // rows fr, fr + 8, 64 + fr, 72 + fr
+        if (p.rowbias) {
+            auto row_img = [&](int r) {
+                const int iw = r % p.bw, ih = (r / p.bw) % p.bh, ib = r / (p.bw * p.bh);
+                const int gw = tw * p.bw + iw, gh = th * p.bh + ih, gb = tb * p.nb + ib;
+                if (gw >= p.W || gh >= p.H || gb >= p.Bn) return 0LL;
+                return ((static_cast<long long>(gb) * p.H + gh) * p.W + gw) / p.rows_per_img;
+            };
+#pragma unroll
+            for (int r = 0; r < 4; ++r) rb[r] = p.rowbias + row_img((r >> 1) * 64 + fr + (r & 1) * 8) * p.rowbias_ld;
+        }
+#pragma unroll
+        for (int j = 0; j < NSLAB_TMA; ++j) {
+            const uint32_t idx = static_cast<uint32_t>(q) * NSLAB_TMA + j;
+            const RingPos sp = ring_pos(idx, p.epi_slots);
+            // The slot's previous slab may be the other warpgroup's, still unopened: slot_ready would then be a whole
+            // phase behind and its parity would pass.  Wait until that slab is written (slot_done); with epi_slots >=
+            // NSLAB_TMA the one before it is a finished tile's, so this parity cannot alias either.
+            if (idx >= static_cast<uint32_t>(p.epi_slots)) mbar_wait_nocall(&slot_done[sp.slot], sp.phase ^ 1);
+            mbar_wait_nocall(&slot_ready[sp.slot], sp.phase);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                float* a = acc + h * HALF;
+                const uint32_t sb = ring0 - (p.epi_slots - sp.slot) * SLOT + (h * 64 + fr) * (SW * 2) + cq * 2;
+#pragma unroll
+                for (int c = 0; c < SW / 8; ++c) {
+                    const int i = j * (SW / 8) + c;
+                    if (!GEGLU) bias_geglu(a, i);
+                    float v00 = a[4 * i], v01 = a[4 * i + 1], v10 = a[4 * i + 2], v11 = a[4 * i + 3];
+                    const int n = n0 + 8 * i + cq;
+                    if (rb[0]) {
+                        const float* r0 = rb[2 * h];
+                        const float* r1 = rb[2 * h + 1];
+                        if (n < p.N) { v00 = __fadd_rn(v00, __ldg(r0 + n)); v10 = __fadd_rn(v10, __ldg(r1 + n)); }
+                        if (n + 1 < p.N) { v01 = __fadd_rn(v01, __ldg(r0 + n + 1)); v11 = __fadd_rn(v11, __ldg(r1 + n + 1)); }
+                    }
+                    if (p.out_scale != 1.0f) {
+                        v00 = __fmul_rn(v00, p.out_scale); v01 = __fmul_rn(v01, p.out_scale);
+                        v10 = __fmul_rn(v10, p.out_scale); v11 = __fmul_rn(v11, p.out_scale);
+                    }
+                    const uint32_t a0 = sb + ((static_cast<uint32_t>(c) ^ row_x) << 4);
+                    const uint32_t a1 = a0 + 8 * SW * 2;
+                    if (p.residual) {
+                        const float2 r0 = h2_to_f2(lds32(a0)), r1 = h2_to_f2(lds32(a1));
+                        v00 = __fadd_rn(v00, r0.x); v01 = __fadd_rn(v01, r0.y);
+                        v10 = __fadd_rn(v10, r1.x); v11 = __fadd_rn(v11, r1.y);
+                    }
+                    sts32(a0, pack_h2(v00, v01));
+                    sts32(a1, pack_h2(v10, v11));
+                }
+            }
+            fence_proxy_async_smem();  // the slot is stored by TMA
+            mbar_arrive(&slot_done[sp.slot]);
+        }
+    }
+}
+
+// PP: the ping-pong schedule (gemm_pingpong_consumers); the producer and the epilogue thread are the same for both,
+// only the arrival counts of `empty` and `slot_done` differ (one warpgroup consumes a stage or fills a slot, not two).
+template <bool GEGLU, int BN, bool PP>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
@@ -220,11 +374,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
         for (int i = 0; i < nstages; ++i) {
             mbar_init(&full[i], 1);
-            mbar_init(&empty[i], GEMM_CONSUMERS);
+            mbar_init(&empty[i], PP ? 128 : GEMM_CONSUMERS);
         }
         for (int i = 0; i < p.epi_slots; ++i) {
             mbar_init(&slot_ready[i], 1);
-            mbar_init(&slot_done[i], GEMM_CONSUMERS);
+            mbar_init(&slot_done[i], PP ? 128 : GEMM_CONSUMERS);
         }
         mbar_init(drained, 1);
         fence_barrier_init();
@@ -314,6 +468,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
     // -------------------------------------------------------- consumers: rows [64 wg, 64 wg + 64) of every tile
     setmaxnreg_inc<GEMM_CONSUMER_REGS>();
+    if constexpr (PP) {
+        gemm_pingpong_consumers<GEGLU, BN>(p, ring, full, empty, slot_ready, slot_done, m_tiles, k_iters);
+        return;
+    }
     const int ct = threadIdx.x - 128;  // 0..255
     const int wg = ct >> 7, t = ct & 127;
     const uint32_t ring0 = smem_u32(ring);
@@ -589,16 +747,20 @@ constexpr int GEMM_MAX_AUTO_SPLIT = 8;
 // the batch-8 step (H100 80GB HBM3, 400 W, tools/gemm_classes.py) they took 10-45 % longer than the narrower tiles
 // the model picks on every 1x1 GEMM with K <= 1280 (5-20 k-steps), and 10-40 % less time on the 3x3 convs (45+)
 static constexpr int GEMM_WIDE_MIN_KITERS = 40;
+// Ping-pong tiles (gemm_pingpong_consumers) are offered to launches of whole tiles that all take the TMA epilogue and
+// whose K loop is shorter than this.  One warpgroup runs a whole tile's epilogue, so its per-column cost is twice the
+// cooperative one; a CTA's tiles cost max(K loop, epilogue) each, and the last epilogue is exposed.
+static constexpr int GEMM_PP_MAX_KITERS = GEMM_WIDE_MIN_KITERS;
 static bool g_attr_set = false;
 
-template <bool GEGLU, int BN>
+template <bool GEGLU, int BN, bool PP = false>
 static cudaError_t launch_gemm(dim3 grid, cudaStream_t stream, const CUtensorMap* tm, const GemmKParams& p) {
-    return launch_pdl(gemm_wgmma_kernel<GEGLU, BN>, grid, dim3(GEMM_THREADS), (size_t)GEMM_SMEM_BYTES, stream, tm[0], tm[1],
+    return launch_pdl(gemm_wgmma_kernel<GEGLU, BN, PP>, grid, dim3(GEMM_THREADS), (size_t)GEMM_SMEM_BYTES, stream, tm[0], tm[1],
                       tm[2], tm[3], tm[4], tm[5], tm[6], tm[7], p);
 }
-template <bool GEGLU, int BN>
+template <bool GEGLU, int BN, bool PP = false>
 static bool set_smem_attr() {
-    return cudaFuncSetAttribute(gemm_wgmma_kernel<GEGLU, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM_BYTES) ==
+    return cudaFuncSetAttribute(gemm_wgmma_kernel<GEGLU, BN, PP>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM_BYTES) ==
            cudaSuccess;
 }
 
@@ -629,14 +791,29 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
     const int sms = persistent_sms();
     if (sms <= 0) return CTRLORA_ERR_CUDA;
     const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_b;
+    // ---- which tiles take the TMA epilogue: fp16 row-major outputs and an fp16 (or no) residual that tensor maps can
+    // address.  The segments it serves must come first (q and k of a q | k | V^T launch), so that every CTA runs its
+    // TMA-epilogue tiles before the others; split tiles keep the row-per-thread epilogue (only the CTA that arrives
+    // last knows that it needs the residual).
+    const int n_segs = a->seg_width > 0 ? (p.N + a->seg_width - 1) / a->seg_width : 1;
+    if (n_segs > 3) return CTRLORA_ERR_ARG;
+    auto tma_ok = [](const void* ptr, long long ld) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && ld % 8 == 0; };
+    int tma_segs = 0;
+    while (tma_segs < n_segs && !a->transposed[tma_segs]) ++tma_segs;
+    bool tma_epi = !a->out_f32 && tma_segs > 0 && (!a->residual || (!a->residual_f32 && tma_ok(a->residual, a->ldr)));
+    for (int i = 0; i < n_segs; ++i) {
+        if (i < tma_segs ? !a->out[i] || !tma_ok(a->out[i], a->ldc) : !a->transposed[i]) tma_epi = false;
+    }
     const int k_iters = p.taps * p.kchunks + p.kchunks2;
     // ---- pick the N tile (wgmma N = 32 ... 256 columns; GEGLU tiles carry value + gate) and the split of the tail with
     // a cycle model of the persistent schedule over `sms` CTAs.  A k-step of a 128 x BN tile costs max(MMA: 4 BN cycles
     // at the dense fp16 rate of one SM, operand bytes / GEMM_L2_BPC from L2); a tile adds its epilogue.  Full waves of
     // tiles run whole; the tiles of the last, partial wave may be split along K so that their work units fill it.
     // A plan that does not fit the split-K workspace or counters is not considered.  An explicit block_n / split_k
-    // overrides the model (split_k then splits every tile).
+    // overrides the model (split_k then splits every tile).  Ping-pong plans (GEMM_PP_MAX_KITERS) are priced next to
+    // the cooperative ones; with an explicit block_n a qualifying width runs its whole tiles ping-pong.
     const bool explicit_split = a->split_k > 0;
+    const bool pp_launch = tma_epi && tma_segs == n_segs && k_iters < GEMM_PP_MAX_KITERS && a->split_k <= 1;
     auto plan = [&](int cand, int S, int* s_eff, int* whole) -> double {
         const int bnt = p.geglu ? 2 * cand : cand;
         const long long tiles = (long long)m_tiles * ((p.N + cand - 1) / cand);
@@ -654,7 +831,15 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
         const double t_split = kps * step + epi + GEMM_SPLIT_PER_COL * bnt * (1 + *s_eff);
         return (double)((w + sms - 1) / sms) * t_whole + (double)((tail * *s_eff + sms - 1) / sms) * t_split;
     };
+    auto plan_pp = [&](int cand) -> double {
+        const int bnt = p.geglu ? 2 * cand : cand;
+        const long long per_cta = ((long long)m_tiles * ((p.N + cand - 1) / cand) + sms - 1) / sms;
+        const double step = fmax(4.0 * bnt, (double)(GEMM_A_BYTES + bnt * 128) / GEMM_L2_BPC);
+        const double epi = GEMM_EPI_FIXED + 2.0 * GEMM_EPI_PER_COL * cand;
+        return (double)per_cta * fmax(k_iters * step, epi) + epi;
+    };
     int bn_out = 0, splits = 1, tiles_whole = 0;
+    bool pingpong = false;
     double best_cost = -1;
     // tile widths; GEGLU tiles carry half as many outputs (and have no 80 + 80 tile)
     static const int kWidths[] = {GEMM_MAX_BN, 256, 160, 128, 64, 32};
@@ -667,11 +852,23 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
         // them for split tiles of the 8x8 level, which measured 30-40 % slower than its choice without them
         if (a->block_n <= 0 && kWidths[wi] == 160 && k_iters >= GEMM_WIDE_MIN_KITERS) continue;
         if (a->seg_width > 0 && a->seg_width % cand != 0) continue;
+        // ping-pong widths: 64, 128, 160 columns, GEGLU 64 + 64 (BN accumulators per thread)
+        const bool pp_width = pp_launch && (p.geglu ? cand == 64 : cand >= 64 && cand <= 160);
+        if (pp_width) {
+            const double cost = plan_pp(cand);
+            if (best_cost < 0 || cost < best_cost || a->block_n > 0) {
+                best_cost = cost; bn_out = cand; splits = 1; pingpong = true;
+                tiles_whole = m_tiles * ((p.N + cand - 1) / cand);
+            }
+            if (a->block_n > 0) break;
+        }
         for (int S = explicit_split ? a->split_k : 1; S <= (explicit_split ? a->split_k : GEMM_MAX_AUTO_SPLIT); ++S) {
             int s_eff, whole;
             const double cost = plan(cand, S, &s_eff, &whole);
             if (cost < 0) continue;
-            if (best_cost < 0 || cost < best_cost) { best_cost = cost; bn_out = cand; splits = s_eff; tiles_whole = whole; }
+            if (best_cost < 0 || cost < best_cost) {
+                best_cost = cost; bn_out = cand; splits = s_eff; tiles_whole = whole; pingpong = false;
+            }
         }
     }
     if (bn_out <= 0) {
@@ -690,19 +887,6 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
         p.counters = a->splitk_counters;
     }
     for (int i = 0; i < 3; ++i) { p.out[i] = a->out[i]; p.transposed[i] = a->transposed[i]; }
-    // ---- which tiles take the TMA epilogue: fp16 row-major outputs and an fp16 (or no) residual that tensor maps can
-    // address.  The segments it serves must come first (q and k of a q | k | V^T launch), so that every CTA runs its
-    // TMA-epilogue tiles before the others; split tiles keep the row-per-thread epilogue (only the CTA that arrives
-    // last knows that it needs the residual).
-    const int n_segs = a->seg_width > 0 ? (p.N + a->seg_width - 1) / a->seg_width : 1;
-    if (n_segs > 3) return CTRLORA_ERR_ARG;
-    auto tma_ok = [](const void* ptr, long long ld) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && ld % 8 == 0; };
-    int tma_segs = 0;
-    while (tma_segs < n_segs && !a->transposed[tma_segs]) ++tma_segs;
-    bool tma_epi = !a->out_f32 && tma_segs > 0 && (!a->residual || (!a->residual_f32 && tma_ok(a->residual, a->ldr)));
-    for (int i = 0; i < n_segs; ++i) {
-        if (i < tma_segs ? !a->out[i] || !tma_ok(a->out[i], a->ldc) : !a->transposed[i]) tma_epi = false;
-    }
     if (tma_epi) {
         const long long t = tma_segs == n_segs ? (long long)m_tiles * p.n_tiles : (long long)m_tiles * tma_segs * (a->seg_width / bn_out);
         p.tma_tiles = (int)(t < tiles_whole ? t : tiles_whole);
@@ -785,13 +969,23 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
     if (!g_attr_set) {
         if (!set_smem_attr<false, 32>() || !set_smem_attr<false, 64>() || !set_smem_attr<false, 128>() ||
             !set_smem_attr<false, 160>() || !set_smem_attr<false, 256>() || !set_smem_attr<false, 320>() || !set_smem_attr<true, 64>() ||
-            !set_smem_attr<true, 128>() || !set_smem_attr<true, 256>() || !set_smem_attr<true, 320>())
+            !set_smem_attr<true, 128>() || !set_smem_attr<true, 256>() || !set_smem_attr<true, 320>() ||
+            !set_smem_attr<false, 64, true>() || !set_smem_attr<false, 128, true>() || !set_smem_attr<false, 160, true>() ||
+            !set_smem_attr<true, 128, true>())
             return CTRLORA_ERR_CUDA;
         g_attr_set = true;
     }
     const dim3 grid((unsigned)(p.units < sms ? p.units : sms));
     cudaError_t lrc;
-    if (p.geglu) lrc = p.BN == 64  ? launch_gemm<true, 64>(grid, stream, tm, p)
+    if (pingpong) {
+        // unreachable (the plan's conditions and the slot count of every ping-pong width), but the schedule relies on it
+        if (p.tma_tiles != p.units || p.splits != 1 || p.epi_slots < 2 || p.epi_slots < bn_out / slab_cols)
+            return CTRLORA_ERR_ARG;
+        lrc = p.geglu      ? launch_gemm<true, 128, true>(grid, stream, tm, p)
+            : p.BN == 64  ? launch_gemm<false, 64, true>(grid, stream, tm, p)
+            : p.BN == 128 ? launch_gemm<false, 128, true>(grid, stream, tm, p)
+                          : launch_gemm<false, 160, true>(grid, stream, tm, p);
+    } else if (p.geglu) lrc = p.BN == 64  ? launch_gemm<true, 64>(grid, stream, tm, p)
                      : p.BN == 128 ? launch_gemm<true, 128>(grid, stream, tm, p)
                      : p.BN == 256 ? launch_gemm<true, 256>(grid, stream, tm, p)
                                    : launch_gemm<true, 320>(grid, stream, tm, p);

@@ -36,6 +36,9 @@ def model_cycles(a, sms, widths, m=MODEL):
     nb = 128 // (bw * bh)
     m_tiles = -(-a.a_w // bw) * -(-a.a_h // bh) * -(-a.a_b // nb)
     k_iters = a.kh * a.kw * -(-a.a_c // 64) + (-(-a.a2_c // 64) if a.a2 else 0)
+    # ping-pong plans: whole tiles that all take the TMA epilogue, K loop under GEMM_PP_MAX_KITERS (40)
+    pp_launch = (not a.out_f32 and not any(a.transposed) and not (a.residual and a.residual_f32) and k_iters < 40
+                 and a.split_k <= 1)
     best = None
     for cand in ([w // 2 for w in widths if w >= 64 and w != 160] if a.geglu else widths):  # no 80 + 80 GEGLU tile
         if a.seg_width and a.seg_width % cand:
@@ -46,6 +49,12 @@ def model_cycles(a, sms, widths, m=MODEL):
             continue
         bnt = 2 * cand if a.geglu else cand
         tiles = m_tiles * -(-a.n // cand)
+        step = max(4.0 * bnt, (16384 + bnt * 128) / m["l2_bpc"])
+        if pp_launch and (cand == 64 if a.geglu else 64 <= cand <= 160):
+            epi = m["epi_fixed"] + 2 * m["epi_per_col"] * cand  # one warpgroup runs the tile's epilogue
+            cost = -(-tiles // sms) * max(k_iters * step, epi) + epi
+            if best is None or cost < best:
+                best = cost
         for S in range(1, 9):
             kps = -(-k_iters // S)
             s_eff = -(-k_iters // kps)
@@ -53,7 +62,6 @@ def model_cycles(a, sms, widths, m=MODEL):
             tail = tiles - w
             if s_eff > 1 and tail == 0:
                 continue
-            step = max(4.0 * bnt, (16384 + bnt * 128) / m["l2_bpc"])
             epi = m["epi_fixed"] + m["epi_per_col"] * cand
             t_whole = k_iters * step + epi
             t_split = kps * step + epi + m["split_per_col"] * bnt * (1 + s_eff)
