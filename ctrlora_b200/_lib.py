@@ -26,6 +26,7 @@ class GemmArgs(C.Structure):
         ("split_k", c_int), ("splitk_ws", c_void_p), ("splitk_ws_bytes", c_ll),
         ("splitk_counters", c_void_p), ("splitk_counters_len", c_int),
         ("dup_out", c_void_p), ("dup_ld", c_int), ("force_single_cta", c_int),
+        ("group_b", c_int), ("w_hi", c_void_p), ("bias_hi", c_void_p), ("rowbias_hi", c_void_p), ("w2_hi", c_void_p),
     ]
 
 
@@ -38,6 +39,7 @@ class GroupNormArgs(C.Structure):
         ("gamma", c_void_p), ("beta", c_void_p), ("eps", c_float), ("silu", c_int),
         ("y", c_void_p), ("raw_out", c_void_p), ("stats_ws", c_void_p), ("stats_prezeroed", c_int),
         ("partial_ws", c_void_p), ("partial_ws_floats", c_ll), ("partial_counters", c_void_p), ("partial_counters_len", c_int),
+        ("gamma_hi", c_void_p), ("beta_hi", c_void_p), ("group_b", c_int),
     ]
 
 
@@ -46,6 +48,7 @@ class CtrloraError(RuntimeError):
 
 
 _STATUS = {1: "bad argument", 2: "CUDA error", 3: "tensor-map encode error", 4: "unsupported"}
+STATUS_UNSUPPORTED = 4
 
 
 def lib_path():
@@ -71,6 +74,7 @@ _ARGTYPES = {
     "ctrlora_gemm_f16_simt": [_P, _P],
     "ctrlora_groupnorm_f16": [_P, _P],
     "ctrlora_layernorm_f16": [_P, _L, _P, _L, _I, _I, _P, _P, _F, _P],
+    "ctrlora_layernorm_grouped_f16": [_P, _L, _P, _L, _I, _I, _P, _P, _P, _P, _I, _F, _P],
     "ctrlora_attention_f16": [_P, _L, _P, _L, _P, _I, _P, _L, _P, _I, _I, _I, _I, _I, _P],
     "ctrlora_attention_bwd_f16": [_P, _L, _P, _L, _P, _L, _P, _L, _P, _L, _P, _P, _P, _L, _P, _L, _P, _L, _I, _I, _I, _I, _I, _P],
     "ctrlora_nchw_f32_to_nhwc_f16": [_P, _P, _I, _I, _I, _I, _P],
@@ -146,6 +150,7 @@ EXPORTS = [
     "ctrlora_gemm_f16_simt",
     "ctrlora_groupnorm_f16",
     "ctrlora_layernorm_f16",
+    "ctrlora_layernorm_grouped_f16",
     "ctrlora_attention_f16",
     "ctrlora_nchw_f32_to_nhwc_f16",
     "ctrlora_nhwc_to_nchw_f32",

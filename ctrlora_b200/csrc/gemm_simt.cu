@@ -61,6 +61,7 @@ __global__ void gemm_simt_kernel(ctrlora_gemm_args a, int M, int rows_per_img) {
 
 extern "C" int ctrlora_gemm_f16_simt(const ctrlora_gemm_args* a, void* stream_) {
     if (!a || !a->a || !a->w || !a->out[0]) return CTRLORA_ERR_ARG;
+    if (a->group_b > 0) return CTRLORA_ERR_UNSUPPORTED;
     const long long M = static_cast<long long>(a->a_b) * a->a_h * a->a_w;
     const long long total = M * a->n;
     const int rows = a->rows_per_img > 0 ? a->rows_per_img : a->a_h * a->a_w;

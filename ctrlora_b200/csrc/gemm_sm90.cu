@@ -27,15 +27,16 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
 }
 
 // One CW-column chunk (CW = 16 or 32) of the epilogue for one output row, after bias (and GEGLU): time-embedding row
-// term, scale, residual, then the store (row-major fp16 / fp32, or the transposed V^T layout).
+// term (of the tile's group: `hi`), scale, residual, then the store (row-major fp16 / fp32, or the transposed V^T
+// layout).
 template <int CW>
 __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, float* v, int c, int bn_out, int n0, bool row_ok,
-                                               long long m, int img, int tok) {
+                                               long long m, int img, int tok, bool hi) {
     const int nbase = n0 + c;
     const bool full_chunk = (c + CW <= bn_out) && (nbase + CW <= p.N);
     if (!row_ok) return;
     if (p.rowbias) {
-        const float* rb = p.rowbias + static_cast<long long>(img) * p.rowbias_ld + nbase;
+        const float* rb = p.rowbias_g[hi] + static_cast<long long>(img - hi * p.rb_img_off) * p.rowbias_ld + nbase;
         if (full_chunk && aligned16(rb)) {
 #pragma unroll
             for (int q = 0; q < CW / 4; ++q) {
@@ -129,6 +130,11 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, float* v, i
                 if (c + j < bn_out && nbase + j < p.N) o[j] = __float2half_rn(v[j]);
         }
     }
+}
+
+// Grouped launch: does m tile mt hold images of the second group (its weights, bias and row term)?
+__device__ __forceinline__ bool tile_hi(const GemmKParams& p, int mt) {
+    return p.group_b > 0 && (mt / (p.tiles_w * p.tiles_h)) * p.nb >= p.group_b;
 }
 
 // One work unit: an output tile (m tile, n tile) and its k-iteration range.  `slot` >= 0 marks a split tile: its
@@ -253,14 +259,16 @@ __device__ __forceinline__ void gemm_pingpong_consumers(const GemmKParams& p, ui
         // ---- the TMA epilogue of the cooperative schedule, over both row halves: h = 0 holds rows fr, fr + 8 of the
         // tile in acc[0, HALF), h = 1 rows 64 + fr, 72 + fr in acc[HALF, BN)
         const int n0 = nt * BN_OUT;
+        const bool hi = tile_hi(p, mt);
+        const float* bias = p.bias_g[hi];  // once per tile: a per-chunk lookup slows the short-K epilogues
         auto bias_geglu = [&](float* a, int i) {
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
                 const int n = n0 + 8 * i + cq + e;
                 float bv = 0.f, bg = 0.f;
-                if (p.bias && n < p.N) {
-                    bv = __ldg(p.bias + n);
-                    if (GEGLU) bg = __ldg(p.bias + p.N + n);
+                if (bias && n < p.N) {
+                    bv = __ldg(bias + n);
+                    if (GEGLU) bg = __ldg(bias + p.N + n);
                 }
                 a[4 * i + e] += bv;
                 a[4 * i + 2 + e] += bv;
@@ -280,14 +288,16 @@ __device__ __forceinline__ void gemm_pingpong_consumers(const GemmKParams& p, ui
         const uint32_t row_x = SW == 64 ? (fr & 7) : ((fr >> 1) & 3);  // the same for rows fr, 64 + fr
         const float* rb[4] = {nullptr, nullptr, nullptr, nullptr};     // rows fr, fr + 8, 64 + fr, 72 + fr
         if (p.rowbias) {
+            const float* rowbias = p.rowbias_g[hi];
+            const int img_off = hi * p.rb_img_off;
             auto row_img = [&](int r) {
                 const int iw = r % p.bw, ih = (r / p.bw) % p.bh, ib = r / (p.bw * p.bh);
                 const int gw = tw * p.bw + iw, gh = th * p.bh + ih, gb = tb * p.nb + ib;
                 if (gw >= p.W || gh >= p.H || gb >= p.Bn) return 0LL;
-                return ((static_cast<long long>(gb) * p.H + gh) * p.W + gw) / p.rows_per_img;
+                return ((static_cast<long long>(gb) * p.H + gh) * p.W + gw) / p.rows_per_img - img_off;
             };
 #pragma unroll
-            for (int r = 0; r < 4; ++r) rb[r] = p.rowbias + row_img((r >> 1) * 64 + fr + (r & 1) * 8) * p.rowbias_ld;
+            for (int r = 0; r < 4; ++r) rb[r] = rowbias + row_img((r >> 1) * 64 + fr + (r & 1) * 8) * p.rowbias_ld;
         }
 #pragma unroll
         for (int j = 0; j < NSLAB_TMA; ++j) {
@@ -343,6 +353,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                   const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
                   const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmO0,
                   const __grid_constant__ CUtensorMap tmO1, const __grid_constant__ CUtensorMap tmO2,
+                  const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmB2h,
                   const __grid_constant__ GemmKParams p) {
     constexpr int BN_OUT = GEGLU ? BN / 2 : BN;
     constexpr int NACC = BN / 2;  // fp32 accumulators per consumer thread (64 rows x BN per warpgroup)
@@ -371,6 +382,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         if (p.kchunks2 > 0) {
             tma_prefetch_desc(&tmA2);
             tma_prefetch_desc(&tmB2);
+        }
+        if (p.group_b > 0) {
+            tma_prefetch_desc(&tmBh);
+            if (p.kchunks2 > 0) tma_prefetch_desc(&tmB2h);
         }
         for (int i = 0; i < nstages; ++i) {
             mbar_init(&full[i], 1);
@@ -401,6 +416,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 const GemmUnit w = gemm_unit(p, u, m_tiles, k_iters);
                 const int tw = w.mt % p.tiles_w, th = (w.mt / p.tiles_w) % p.tiles_h, tb = w.mt / (p.tiles_w * p.tiles_h);
                 const int w0 = tw * p.bw - p.pad, h0 = th * p.bh - p.pad, b0 = tb * p.nb, n0 = w.nt * BN_OUT;
+                const bool hi = p.group_b > 0 && b0 >= p.group_b;  // the tile's weights: the second group's maps
+                const CUtensorMap* mB = hi ? &tmBh : &tmB;
+                const CUtensorMap* mB2 = hi ? &tmB2h : &tmB2;
                 for (int it = w.it0; it < w.it1; ++it) {
                     mbar_wait_nocall(&empty[s], phase ^ 1);
                     uint8_t* dst = ring + s * p.stage_bytes;
@@ -408,14 +426,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     if (it < main_iters) {
                         const int tap = it / p.kchunks, kc = it - tap * p.kchunks, ky = tap / p.kw, kx = tap - ky * p.kw;
                         tma_load_4d(dst, &tmA, &full[s], kc * GEMM_BK, w0 + kx, h0 + ky, b0);
-                        tma_load_3d(dst + GEMM_A_BYTES, &tmB, &full[s], kc * GEMM_BK, tap, n0);
+                        tma_load_3d(dst + GEMM_A_BYTES, mB, &full[s], kc * GEMM_BK, tap, n0);
                         if (BOX < BN)  // GEGLU: the gate rows start at N
-                            tma_load_3d(dst + GEMM_A_BYTES + BOX * 128, &tmB, &full[s], kc * GEMM_BK, tap, GEGLU ? p.N + n0 : n0 + BOX);
+                            tma_load_3d(dst + GEMM_A_BYTES + BOX * 128, mB, &full[s], kc * GEMM_BK, tap, GEGLU ? p.N + n0 : n0 + BOX);
                     } else {  // second operand pair (fused 1x1 skip convolution)
                         const int c0 = (it - main_iters) * GEMM_BK;
                         tma_load_4d(dst, &tmA2, &full[s], c0, w0 + p.pad, h0 + p.pad, b0);
-                        tma_load_3d(dst + GEMM_A_BYTES, &tmB2, &full[s], c0, 0, n0);
-                        if (BOX < BN) tma_load_3d(dst + GEMM_A_BYTES + BOX * 128, &tmB2, &full[s], c0, 0, n0 + BOX);
+                        tma_load_3d(dst + GEMM_A_BYTES, mB2, &full[s], c0, 0, n0);
+                        if (BOX < BN) tma_load_3d(dst + GEMM_A_BYTES + BOX * 128, mB2, &full[s], c0, 0, n0 + BOX);
                     }
                     if (++s == nstages) { s = 0; phase ^= 1; }
                 }
@@ -544,14 +562,18 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
         // ---- bias and GEGLU on the fragment: a thread holds value column c and its gate column c + BN_OUT
         const int n0 = w.nt * BN_OUT;
+        const bool hi = tile_hi(p, w.mt);
+        // the group's bias: looked up once per tile, except in the 320-column tiles, which have no register to hold it
+        const float* bias_tile = BN > 256 ? nullptr : p.bias_g[hi];
         auto bias_geglu = [&](int i) {
+            const float* bias = BN > 256 ? p.bias_g[hi] : bias_tile;
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
                 const int n = n0 + 8 * i + cq + e;
                 float bv = 0.f, bg = 0.f;
-                if (p.bias && n < p.N) {
-                    bv = __ldg(p.bias + n);
-                    if (GEGLU) bg = __ldg(p.bias + p.N + n);
+                if (bias && n < p.N) {
+                    bv = __ldg(bias + n);
+                    if (GEGLU) bg = __ldg(bias + p.N + n);
                 }
                 acc[4 * i + e] += bv;
                 acc[4 * i + 2 + e] += bv;
@@ -575,15 +597,17 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             const uint32_t row_off = (wg * 64 + fr) * (SW * 2) + cq * 2, row_x = SW == 64 ? (fr & 7) : ((fr >> 1) & 3);
             const float* rb0 = nullptr;
             const float* rb1 = nullptr;
-            if (p.rowbias) {
-                auto row_img = [&](int r) {  // image of tile row r (a tile can span several); 0 for rows past the end
+            const float* rowbias = p.rowbias_g[hi];
+            const int img_off = hi * p.rb_img_off;
+            if (rowbias) {
+                auto row_img = [&](int r) {  // row term row of tile row r (a tile can span several images); 0 past the end
                     const int iw = r % p.bw, ih = (r / p.bw) % p.bh, ib = r / (p.bw * p.bh);
                     const int gw = tw * p.bw + iw, gh = th * p.bh + ih, gb = tb * p.nb + ib;
                     if (gw >= p.W || gh >= p.H || gb >= p.Bn) return 0LL;
-                    return ((static_cast<long long>(gb) * p.H + gh) * p.W + gw) / p.rows_per_img;
+                    return ((static_cast<long long>(gb) * p.H + gh) * p.W + gw) / p.rows_per_img - img_off;
                 };
-                rb0 = p.rowbias + row_img(wg * 64 + fr) * p.rowbias_ld;
-                rb1 = p.rowbias + row_img(wg * 64 + fr + 8) * p.rowbias_ld;
+                rb0 = rowbias + row_img(wg * 64 + fr) * p.rowbias_ld;
+                rb1 = rowbias + row_img(wg * 64 + fr + 8) * p.rowbias_ld;
             }
 #pragma unroll
             for (int j = 0; j < NSLAB_TMA; ++j) {
@@ -661,7 +685,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                         const float4 x = lds128f(epi_addr(stg, er, 32 * eh + c1 + 4 * q));
                         v[4 * q] = x.x; v[4 * q + 1] = x.y; v[4 * q + 2] = x.z; v[4 * q + 3] = x.w;
                     }
-                    epilogue_chunk<CW>(p, v, c, BN_OUT, n0, row_ok, m, img, tok);
+                    epilogue_chunk<CW>(p, v, c, BN_OUT, n0, row_ok, m, img, tok, hi);
                 }
             }
             named_bar_sync(2 + wg, 128);  // the slab is free for the next one
@@ -756,7 +780,7 @@ static bool g_attr_set = false;
 template <bool GEGLU, int BN, bool PP = false>
 static cudaError_t launch_gemm(dim3 grid, cudaStream_t stream, const CUtensorMap* tm, const GemmKParams& p) {
     return launch_pdl(gemm_wgmma_kernel<GEGLU, BN, PP>, grid, dim3(GEMM_THREADS), (size_t)GEMM_SMEM_BYTES, stream, tm[0], tm[1],
-                      tm[2], tm[3], tm[4], tm[5], tm[6], tm[7], p);
+                      tm[2], tm[3], tm[4], tm[5], tm[6], tm[7], tm[8], tm[9], p);
 }
 template <bool GEGLU, int BN, bool PP = false>
 static bool set_smem_attr() {
@@ -788,6 +812,13 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
     p.kchunks = (a->a_c + GEMM_BK - 1) / GEMM_BK;
     p.kchunks2 = a->a2 ? (a->a2_c + GEMM_BK - 1) / GEMM_BK : 0;
     p.geglu = a->geglu;
+    if (a->group_b > 0) {
+        // a grouped launch: every tile's images lie on one side of group_b (the tile model plans on the whole batch)
+        if (!a->w_hi || a->group_b >= p.Bn || (a->a2 && !a->w2_hi) || (a->bias && !a->bias_hi) || (a->rowbias && !a->rowbias_hi))
+            return CTRLORA_ERR_ARG;
+        if (a->group_b % p.nb != 0) return CTRLORA_ERR_UNSUPPORTED;
+        p.group_b = a->group_b;
+    }
     const int sms = persistent_sms();
     if (sms <= 0) return CTRLORA_ERR_CUDA;
     const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_b;
@@ -905,7 +936,16 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
     p.seg_width = a->seg_width;
     p.ldc = a->ldc; p.out_f32 = a->out_f32;
     p.bias = a->bias; p.rowbias = a->rowbias;
+    p.bias_g[0] = a->bias;
+    p.bias_g[1] = p.group_b > 0 ? a->bias_hi : a->bias;
+    p.rowbias_g[0] = a->rowbias;
+    p.rowbias_g[1] = p.group_b > 0 ? a->rowbias_hi : a->rowbias;
     p.rows_per_img = a->rows_per_img > 0 ? a->rows_per_img : p.W * p.H;
+    if (p.group_b > 0 && p.rowbias) {
+        const long long rows_lo = (long long)p.group_b * p.H * p.W;
+        if (rows_lo % p.rows_per_img != 0) return CTRLORA_ERR_ARG;
+        p.rb_img_off = (int)(rows_lo / p.rows_per_img);
+    }
     p.residual = reinterpret_cast<const __half*>(a->residual); p.ldr = a->ldr;
     p.residual_f32 = a->residual_f32;
     p.rowbias_ld = a->rowbias_ld > 0 ? a->rowbias_ld : a->n;
@@ -914,7 +954,7 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
     p.dup_out = reinterpret_cast<__half*>(a->dup_out); p.dup_ld = a->dup_ld;
 
     const int b_box = p.geglu || p.BN > 256 ? p.BN / 2 : p.BN;  // rows of a B box (the kernel's BOX)
-    CUtensorMap tm[8];  // A, B, A2, B2, residual, out[0..2]
+    CUtensorMap tm[10];  // A, B, A2, B2, residual, out[0..2], B and B2 of the second group
     CUtensorMap &tmA = tm[0], &tmB = tm[1], &tmA2 = tm[2], &tmB2 = tm[3];
     {
         uint64_t dims[4] = {(uint64_t)a->a_c, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)p.Bn};
@@ -928,6 +968,10 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
         uint32_t wb[3] = {GEMM_BK, 1, (uint32_t)b_box};
         rc = make_tmap_f16(&tmB, a->w, 3, wd, ws, wb);
         if (rc) return rc;
+        if (p.group_b > 0) {
+            rc = make_tmap_f16(&tm[8], a->w_hi, 3, wd, ws, wb);
+            if (rc) return rc;
+        }
     }
     if (a->a2) {
         if (!a->w2 || a->a2_c % 8 != 0 || a->a2_ld % 8 != 0 || p.geglu) return CTRLORA_ERR_ARG;
@@ -941,10 +985,16 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
         uint32_t wb[3] = {GEMM_BK, 1, (uint32_t)b_box};
         rc = make_tmap_f16(&tmB2, a->w2, 3, wd, ws, wb);
         if (rc) return rc;
+        if (p.group_b > 0) {
+            rc = make_tmap_f16(&tm[9], a->w2_hi, 3, wd, ws, wb);
+            if (rc) return rc;
+        }
     } else {
         tmA2 = tmA;
         tmB2 = tmB;
     }
+    if (p.group_b == 0) tm[8] = tmB;
+    if (p.group_b == 0 || !a->a2) tm[9] = tmB2;
     for (int i = 4; i < 8; ++i) tm[i] = tmA;
     if (p.tma_tiles > 0) {
         // the residual and the outputs have the geometry of A with C = N (a segment: seg_width): the map clips partial

@@ -64,6 +64,13 @@ struct GemmKParams {
     int head_dim, tok_pad;
     __half* dup_out;               // transposed segments are ALSO stored row-major here (training keeps natural V)
     int dup_ld;
+    // grouped launch: tiles of images >= group_b (0 = off) take the second weight maps, bias_g[1] and rowbias_g[1]
+    // (rows from image img - rb_img_off); [0] are bias and rowbias, and so are [1] when the launch is not grouped.
+    // Indexed in parameter space, so that the 320-column tiles hold no extra pointer in registers.
+    int group_b;
+    int rb_img_off;
+    const float* bias_g[2];
+    const float* rowbias_g[2];
 };
 
 }  // namespace ctrl

@@ -162,11 +162,15 @@ gn_stats_det_kernel(GnSrc s, int C, int HW, int groups, int pix_per_block, float
 
 __global__ void __launch_bounds__(512, 2)  // <= 64 registers: four 240..256-thread blocks per SM, the whole grid in one wave
 gn_apply_kernel(GnSrc s, int C, int HW, int groups, int pix_per_block, const float* __restrict__ stats,
-                const float* __restrict__ gamma, const float* __restrict__ beta, float eps, int silu,
-                __half* __restrict__ y, __half* __restrict__ raw) {
+                const float* __restrict__ gamma_lo, const float* __restrict__ beta_lo, const float* __restrict__ gamma_hi,
+                const float* __restrict__ beta_hi, int group_b, float eps, int silu, __half* __restrict__ y,
+                __half* __restrict__ raw) {
     pdl_launch_dependents();
     pdl_wait();
     const int b = blockIdx.y;
+    const bool hi = group_b > 0 && b >= group_b;  // grouped launch: the second network's affine parameters
+    const float* __restrict__ gamma = hi ? gamma_hi : gamma_lo;
+    const float* __restrict__ beta = hi ? beta_hi : beta_lo;
     const int vecs = C >> 3;
     const int lanes = blockDim.x / vecs;
     const int vec = threadIdx.x % vecs, pl = threadIdx.x / vecs;
@@ -251,8 +255,9 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src, uint32
 // passes differ by 1.6e-3, tools/debug_determinism.py.)
 template <int MODE>  // 0: register-gathered tile, 1: TMA bulk-staged tile, 2: no tile
 __global__ void __launch_bounds__(512, 1)
-gn_cluster_kernel(GnSrc s, int C, int HW, int groups, int ppc, int cs, const float* __restrict__ gamma,
-                  const float* __restrict__ beta, float eps, int silu, __half* __restrict__ y, __half* __restrict__ raw,
+gn_cluster_kernel(GnSrc s, int C, int HW, int groups, int ppc, int cs, const float* __restrict__ gamma_lo,
+                  const float* __restrict__ beta_lo, const float* __restrict__ gamma_hi, const float* __restrict__ beta_hi,
+                  int group_b, float eps, int silu, __half* __restrict__ y, __half* __restrict__ raw,
                   float* __restrict__ stats_out) {
     constexpr bool BULK = MODE == 1;
     constexpr bool TILE = MODE != 2;
@@ -376,6 +381,9 @@ gn_cluster_kernel(GnSrc s, int C, int HW, int groups, int ppc, int cs, const flo
     }
     cluster_sync_all();  // remote reads of this CTA's partials are done (it may exit); mr[] visible to the whole block
     if (pl >= lanes) return;
+    const bool hi = group_b > 0 && b >= group_b;  // grouped launch: the second network's affine parameters
+    const float* __restrict__ gamma = hi ? gamma_hi : gamma_lo;
+    const float* __restrict__ beta = hi ? beta_hi : beta_lo;
     float sc[8], sh[8];
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
@@ -414,12 +422,15 @@ gn_cluster_kernel(GnSrc s, int C, int HW, int groups, int ppc, int cs, const flo
 template <int MAXV>
 __global__ void __launch_bounds__(256)
 layernorm_kernel(const __half* __restrict__ x, long long ldx, __half* __restrict__ y, long long ldy, int M, int C,
-                 const float* __restrict__ gamma, const float* __restrict__ beta, float eps) {
+                 const float* __restrict__ gamma_lo, const float* __restrict__ beta_lo, const float* __restrict__ gamma_hi,
+                 const float* __restrict__ beta_hi, int split_rows, float eps) {
     pdl_launch_dependents();
     pdl_wait();
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (row >= M) return;
+    const float* __restrict__ gamma = row >= split_rows ? gamma_hi : gamma_lo;
+    const float* __restrict__ beta = row >= split_rows ? beta_hi : beta_lo;
     const int vecs = C >> 3;
     float v[MAXV][8];
     float sum = 0.f;
@@ -475,6 +486,9 @@ using namespace ctrl;
 extern "C" int ctrlora_groupnorm_f16(const ctrlora_groupnorm_args* a, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     if (!a || !a->x1 || !a->y || !a->stats_ws || !a->gamma || !a->beta) return CTRLORA_ERR_ARG;
+    if (a->group_b < 0 || a->group_b >= a->batch || (a->group_b > 0 && (!a->gamma_hi || !a->beta_hi))) return CTRLORA_ERR_ARG;
+    const float* gamma_hi = a->group_b > 0 ? a->gamma_hi : a->gamma;
+    const float* beta_hi = a->group_b > 0 ? a->beta_hi : a->beta;
     const int C = a->c1 + (a->x2 ? a->c2 : 0);
     if (C % 8 != 0 || a->c1 % 8 != 0 || C % a->groups != 0 || C / 8 > 512) return CTRLORA_ERR_ARG;
     if (a->ld1 % 8 != 0 || (a->x2 && a->ld2 % 8 != 0)) return CTRLORA_ERR_ARG;
@@ -551,15 +565,18 @@ extern "C" int ctrlora_groupnorm_f16(const ctrlora_groupnorm_args* a, void* stre
             const cudaError_t rc = launch_cluster_pdl(mode == 1 ? gn_cluster_kernel<1> : mode == 2 ? gn_cluster_kernel<2> : gn_cluster_kernel<0>,
                                                       dim3(cs, B),
                                                       dim3(threads), smem, stream, (unsigned)cs, s, C, HW, (int)a->groups, ppc, cs,
-                                                      a->gamma, a->beta, a->eps, (int)a->silu, reinterpret_cast<__half*>(a->y),
+                                                      a->gamma, a->beta, gamma_hi, beta_hi, (int)a->group_b, a->eps,
+                                                      (int)a->silu, reinterpret_cast<__half*>(a->y),
                                                       reinterpret_cast<__half*>(a->raw_out), reinterpret_cast<float*>(a->stats_ws));
             if (rc == cudaSuccess) return cudaGetLastError() == cudaSuccess ? CTRLORA_OK : CTRLORA_ERR_CUDA;
             (void)cudaGetLastError();  // fall through to the two-pass pair
         }
     }
 two_pass:
-    // ~4 blocks per SM in total, at least 8 pixels per block
-    int chunks = (592 + B - 1) / B;
+    // ~4 blocks per SM in total, at least 8 pixels per block; a grouped launch splits each image as a call over the
+    // larger group would, so that its statistics are summed in the same order
+    const int B_split = a->group_b > 0 ? (a->group_b > B - a->group_b ? a->group_b : B - a->group_b) : B;
+    int chunks = (592 + B_split - 1) / B_split;
     int ppb = (HW + chunks - 1) / chunks;
     if (ppb < 8) ppb = 8;
     chunks = (HW + ppb - 1) / ppb;
@@ -583,23 +600,32 @@ two_pass:
         gn_stats_kernel<<<grid, threads, 2 * C * sizeof(float), stream>>>(s, C, HW, a->groups, ppb,
                                                                      reinterpret_cast<float*>(a->stats_ws));
     launch_pdl(gn_apply_kernel, grid, dim3(threads), (size_t)0, stream, s, C, HW, (int)a->groups, ppb,
-               reinterpret_cast<const float*>(a->stats_ws), a->gamma, a->beta, a->eps, (int)a->silu,
-               reinterpret_cast<__half*>(a->y), reinterpret_cast<__half*>(a->raw_out));
+               reinterpret_cast<const float*>(a->stats_ws), a->gamma, a->beta, gamma_hi, beta_hi, (int)a->group_b, a->eps,
+               (int)a->silu, reinterpret_cast<__half*>(a->y), reinterpret_cast<__half*>(a->raw_out));
+    return cudaGetLastError() == cudaSuccess ? CTRLORA_OK : CTRLORA_ERR_CUDA;
+}
+
+extern "C" int ctrlora_layernorm_grouped_f16(const void* x, long long ldx, void* y, long long ldy, int rows, int cols,
+                                             const float* gamma, const float* beta, const float* gamma_hi,
+                                             const float* beta_hi, int split_rows, float eps, void* stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    if (!x || !y || cols % 8 != 0 || cols > 2048 || ldx % 8 != 0 || ldy % 8 != 0) return CTRLORA_ERR_ARG;
+    if (split_rows < 0 || (split_rows < rows && (!gamma_hi || !beta_hi))) return CTRLORA_ERR_ARG;
+    const int grid = (rows + 7) / 8;
+    const __half* xp = reinterpret_cast<const __half*>(x);
+    __half* yp = reinterpret_cast<__half*>(y);
+    const float* gh = split_rows < rows ? gamma_hi : gamma;
+    const float* bh = split_rows < rows ? beta_hi : beta;
+    if (cols <= 512) launch_pdl(layernorm_kernel<2>, dim3(grid), dim3(256), (size_t)0, stream, xp, ldx, yp, ldy, rows, cols, gamma, beta, gh, bh, split_rows, eps);
+    else if (cols <= 768) launch_pdl(layernorm_kernel<3>, dim3(grid), dim3(256), (size_t)0, stream, xp, ldx, yp, ldy, rows, cols, gamma, beta, gh, bh, split_rows, eps);
+    else if (cols <= 1280) launch_pdl(layernorm_kernel<5>, dim3(grid), dim3(256), (size_t)0, stream, xp, ldx, yp, ldy, rows, cols, gamma, beta, gh, bh, split_rows, eps);
+    else launch_pdl(layernorm_kernel<8>, dim3(grid), dim3(256), (size_t)0, stream, xp, ldx, yp, ldy, rows, cols, gamma, beta, gh, bh, split_rows, eps);
     return cudaGetLastError() == cudaSuccess ? CTRLORA_OK : CTRLORA_ERR_CUDA;
 }
 
 extern "C" int ctrlora_layernorm_f16(const void* x, long long ldx, void* y, long long ldy, int rows, int cols,
-                                     const float* gamma, const float* beta, float eps, void* stream_) {
-    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    if (!x || !y || cols % 8 != 0 || cols > 2048 || ldx % 8 != 0 || ldy % 8 != 0) return CTRLORA_ERR_ARG;
-    const int grid = (rows + 7) / 8;
-    const __half* xp = reinterpret_cast<const __half*>(x);
-    __half* yp = reinterpret_cast<__half*>(y);
-    if (cols <= 512) launch_pdl(layernorm_kernel<2>, dim3(grid), dim3(256), (size_t)0, stream, xp, ldx, yp, ldy, rows, cols, gamma, beta, eps);
-    else if (cols <= 768) launch_pdl(layernorm_kernel<3>, dim3(grid), dim3(256), (size_t)0, stream, xp, ldx, yp, ldy, rows, cols, gamma, beta, eps);
-    else if (cols <= 1280) launch_pdl(layernorm_kernel<5>, dim3(grid), dim3(256), (size_t)0, stream, xp, ldx, yp, ldy, rows, cols, gamma, beta, eps);
-    else launch_pdl(layernorm_kernel<8>, dim3(grid), dim3(256), (size_t)0, stream, xp, ldx, yp, ldy, rows, cols, gamma, beta, eps);
-    return cudaGetLastError() == cudaSuccess ? CTRLORA_OK : CTRLORA_ERR_CUDA;
+                                     const float* gamma, const float* beta, float eps, void* stream) {
+    return ctrlora_layernorm_grouped_f16(x, ldx, y, ldy, rows, cols, gamma, beta, nullptr, nullptr, rows, eps, stream);
 }
 
 // ================================================================================================ backward (training)
@@ -972,6 +998,7 @@ extern "C" int ctrlora_groupnorm_bwd_f16(const ctrlora_groupnorm_args* a, const 
                                          const void* res, long long ldres, float* dgamma, float* dbeta, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     if (!a || !a->x1 || !dy || !fwd_stats || !a->stats_ws || !a->gamma || !a->beta) return CTRLORA_ERR_ARG;
+    if (a->group_b != 0) return CTRLORA_ERR_UNSUPPORTED;
     const int C = a->c1 + (a->x2 ? a->c2 : 0);
     if (C % 8 != 0 || a->c1 % 8 != 0 || C % a->groups != 0 || C / 8 > 512) return CTRLORA_ERR_ARG;
     GnSrc s;

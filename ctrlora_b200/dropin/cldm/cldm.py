@@ -6,7 +6,16 @@ Data flow of one `apply_model` (reference :329-344 and cldm_ctrlora_finetune.py:
     UNet: encoder + middle, then for each decoder block the next ResBlock's GroupNorm kernel reads
     [h (+ s*c_mid) | hs_i + s_i*c_i] in place: the residual adds, the control_scales multiply and torch.cat of the
     reference (:34-42, finetune :79) are not separate passes over HBM.
+
+Twin pass (ControlLDM._control_and_unet): the ControlNet and the UNet encoder have the same shapes layer for layer and
+do not depend on each other, so sampling runs them as one batch-2B pass: images [0, B) are the hint's, [B, 2B) x's, and
+each launch takes the ControlNet's weights for the lower half and the UNet's for the upper half (grouped GEMM, GroupNorm
+and LayerNorm launches).  The zero-convs read the lower half, the decoder's skips are views of the upper half.
+Environment: CTRLORA_TWIN_ENCODER=0 runs the two networks one after the other; CTRLORA_TWIN_FROM=L (0-3) runs the
+blocks above resolution level L at batch B per network and starts the twin pass at level L.
 """
+import os
+
 import torch
 import torch.nn as nn
 
@@ -15,7 +24,7 @@ from ctrlora_b200.runtime import CatSpec, Scaled, nchw_view, pixel_major, to_f16
 from ldm.models.diffusion.ddpm import LatentDiffusion
 from ldm.modules.attention import SpatialTransformer
 from ldm.modules.diffusionmodules.openaimodel import (Downsample, ResBlock, TimestepEmbedSequential, UNetModel,  # noqa: F401
-                                                      _conv2d)
+                                                      _Conv, _conv2d)
 from ldm.modules.diffusionmodules.util import conv_nd, linear, timestep_embedding, zero_module  # noqa: F401
 from ldm.util import exists, instantiate_from_config  # noqa: F401
 
@@ -43,6 +52,10 @@ class ControlledForward:
                 h = module(h, emb, ctx)
                 hs.append(h)
             h = self.middle_block(h, emb, ctx)
+        return self.decode(h, hs, emb, ctx, control, only_mid_control)
+
+    def decode(self, h, hs, emb, ctx, control, only_mid_control):
+        """the decoder half of forward: middle-block output h, encoder skips hs (consumed)"""
         add_mid, s_mid = (None, 1.0)
         if control is not None:
             add_mid, s_mid = unwrap_scaled(control.pop())
@@ -179,6 +192,17 @@ class ControlNet(nn.Module):
         return self._encode(hint, emb, _ctx16(context))
 
 
+TWIN_FROM_DEFAULT = 1  # CTRLORA_TWIN_FROM when unset
+
+
+def twin_from_level():
+    """CTRLORA_TWIN_FROM: the resolution level (0-3) at which the twin pass starts"""
+    v = os.environ.get("CTRLORA_TWIN_FROM", str(TWIN_FROM_DEFAULT)).strip()
+    if v not in ("0", "1", "2", "3"):
+        raise ValueError(f"CTRLORA_TWIN_FROM={v!r}: expected a resolution level 0, 1, 2 or 3")
+    return int(v)
+
+
 class ControlLDM(LatentDiffusion):
     def __init__(self, control_stage_config, control_key, only_mid_control, global_average_pooling=False, *args, **kwargs):
         super().__init__(*args, **kwargs)
@@ -233,10 +257,155 @@ class ControlLDM(LatentDiffusion):
         ctx16 = reg["ctx16"]
         key = reg["epoch"]
         ctx2d, nk = ctx16.view(-1, ctx16.shape[-1]), ctx16.shape[1]
+        pairs = {}  # twin pass: a ControlNet layer and its UNet partner keep their K / V^T in one batch-2B buffer pair
+        if self._twin_pairs() is not None:
+            for ca, cb in self._twin_pairs()["cross"]:
+                b, inner = ctx16.shape[0], ca.to_q.out_features
+                nk_pad = (nk + 7) // 8 * 8
+                buf = ca.__dict__.get("_kv_twin")
+                if buf is None or buf[0].shape != (2 * b * nk, inner) or buf[0].device != ctx16.device:
+                    buf = (torch.empty((2 * b * nk, inner), device=ctx16.device, dtype=torch.float16),
+                           ops.zeros((2 * b, ca.heads, inner // ca.heads, nk_pad), ctx16.device))
+                    ca.__dict__["_kv_twin"] = buf
+                pairs[id(ca)] = (buf[0][:b * nk], buf[1][:b])
+                pairs[id(cb)] = (buf[0][b * nk:], buf[1][b:])
         for net in (self.control_model, self.model.diffusion_model):
             for m in net.modules():
                 if isinstance(m, CrossAttention) and m.to_k.in_features == ctx16.shape[-1] and m.to_k.in_features != m.to_q.in_features:
-                    m.project_context(ctx2d, ctx16.shape[0], nk, key)
+                    m.project_context(ctx2d, ctx16.shape[0], nk, key, out=pairs.get(id(m)))
+
+    def _twin_pairs(self):
+        """The layer pairs of the twin pass, or None when the ControlNet and the UNet encoder differ in structure (the
+        style variant's IP-Adapter UNet, say).  Checked once per model: "cross" are the cross-attention pairs, "norms"
+        the transformer norm pairs, whose effective layers (switch_lora re-points the inference ControlNet's) must have
+        one eps when the pass runs."""
+        from ldm.modules.attention import BasicTransformerBlock, CrossAttention
+        if "_twin" in self.__dict__:
+            return self.__dict__["_twin"]
+        cn, un = self.control_model, self.model.diffusion_model
+
+        def same(a, b):
+            if type(a) is not type(b):
+                return False
+            if isinstance(a, ResBlock):
+                return (a.channels, a.out_channels, type(a.skip_connection), a.in_layers[0].eps, a.out_layers[0].eps) == \
+                    (b.channels, b.out_channels, type(b.skip_connection), b.in_layers[0].eps, b.out_layers[0].eps)
+            if isinstance(a, SpatialTransformer):
+                blocks = list(zip(a.transformer_blocks, b.transformer_blocks))
+                return (a.in_channels, a.use_linear, len(a.transformer_blocks)) == \
+                    (b.in_channels, b.use_linear, len(b.transformer_blocks)) and not a.use_linear and all(
+                        type(x) is BasicTransformerBlock and type(y) is BasicTransformerBlock and not x.disable_self_attn and
+                        not y.disable_self_attn and type(x.attn1) is CrossAttention and type(y.attn1) is CrossAttention and
+                        type(x.attn2) is CrossAttention and type(y.attn2) is CrossAttention and
+                        (x.attn1.heads, x.attn1.to_q.out_features, x.attn2.to_k.in_features) ==
+                        (y.attn1.heads, y.attn1.to_q.out_features, y.attn2.to_k.in_features)
+                        for x, y in blocks)
+            if isinstance(a, Downsample):
+                return (a.channels, a.out_channels) == (b.channels, b.out_channels)
+            if isinstance(a, _Conv):
+                return (a.in_channels, a.out_channels, a.kernel_size) == (b.in_channels, b.out_channels, b.kernel_size)
+            return False
+
+        seqs = list(zip(cn.input_blocks, un.input_blocks)) + [(cn.middle_block, un.middle_block)]
+        ok = isinstance(un, ControlledForward) and len(cn.input_blocks) == len(un.input_blocks) and \
+            cn.model_channels == un.model_channels and all(
+                len(a) == len(b) and all(same(x, y) for x, y in zip(a, b)) for a, b in seqs)
+        res = None
+        if ok:
+            sts = [(la, lb) for a, b in seqs for la, lb in zip(a, b) if isinstance(la, SpatialTransformer)]
+            blocks = [(x, y) for la, lb in sts for x, y in zip(la.transformer_blocks, lb.transformer_blocks)]
+            res = {"cross": [(x.attn2, y.attn2) for x, y in blocks],
+                   "norms": [(la.norm, lb.norm) for la, lb in sts] +
+                            [(getattr(x, n), getattr(y, n)) for x, y in blocks for n in ("norm1", "norm2", "norm3")]}
+        self.__dict__["_twin"] = res
+        return res
+
+    def twin_enabled(self):
+        """Whether apply_model runs the ControlNet and the UNet encoder as one pass (the module docstring): inference
+        only, on structurally equal networks, unless CTRLORA_TWIN_ENCODER=0."""
+        if os.environ.get("CTRLORA_TWIN_ENCODER", "1") == "0" or self.training or torch.is_grad_enabled():
+            return False
+        pairs = self._twin_pairs()
+        eff = prepare.effective
+        return pairs is not None and all(eff(a).eps == eff(b).eps for a, b in pairs["norms"])
+
+    @torch.no_grad()
+    def _control_and_unet(self, x, hint, t, context):
+        """The ControlNet's 13 control residuals and the UNet encoder + middle block as one batch-2B pass.
+        Returns (control, h, hs, emb, ctx) for ControlledForward.decode."""
+        cn, un = self.control_model, self.model.diffusion_model
+        b = x.shape[0]
+        # each network's time embedding, in rows of one common stride: a grouped GEMM reads both with one row stride
+        wc = sum(r.out_channels for r in cn._resblocks())
+        wu = sum(r.out_channels for r in un._resblocks())
+        ld = max(wc, wu)
+        emb_c = cn.embed(t, out_all=torch.empty((b, ld), device=x.device, dtype=torch.float32)[:, :wc])
+        emb_u = un.embed(t, out_all=torch.empty((b, ld), device=x.device, dtype=torch.float32)[:, :wu])
+        ctx = _ctx16(context)
+        ctx2d, nk = ctx.reshape(-1, ctx.shape[-1]), ctx.shape[1]
+        # below the fork level each network runs its blocks at batch b; the last of them (a Downsample) writes its
+        # output into that network's half of the batch-2b buffer
+        level = twin_from_level()
+        downs = [i for i, m in enumerate(cn.input_blocks) if isinstance(m[0], Downsample)]
+        fork = downs[level - 1] + 1 if 0 < level <= len(downs) else 0
+        control, hs = [], []
+        hc, hu = hint, x
+        for i in range(fork):
+            if i < fork - 1:
+                hc = cn.input_blocks[i](hc, emb_c, ctx)
+                hu = un.input_blocks[i](hu, emb_u, ctx)
+            else:
+                dc, du = cn.input_blocks[i][0], un.input_blocks[i][0]
+                xc, xu = pixel_major(hc), pixel_major(hu)
+                h16 = torch.empty((2 * b, xc.shape[1] // 2, xc.shape[2] // 2, dc.out_channels), device=x.device,
+                                  dtype=torch.float16)
+                dc.run(xc, out=h16[:b])
+                du.run(xu, out=h16[b:])
+                hc, hu = nchw_view(h16[:b]), nchw_view(h16[b:])
+            control.append(cn._zero_conv(cn.zero_convs[i], hc))
+            hs.append(hu)
+        start = fork
+        if fork == 0:
+            ca, cu = cn.input_blocks[0][0], un.input_blocks[0][0]
+            c_pad = (ca.in_channels + 7) // 8 * 8
+            xin = torch.empty((2 * b, x.shape[2], x.shape[3], c_pad), device=x.device, dtype=torch.float16)
+            ops.nchw_to_nhwc_f16(hint.float().contiguous(), c_pad, out=xin[:b])
+            ops.nchw_to_nhwc_f16(x.float().contiguous(), c_pad, out=xin[b:])
+            pad = c_pad if c_pad != ca.in_channels else None
+            h16 = ops.gemm(xin, ca.kernel_weight(pad_in=pad), ksize=3, bias=prepare.bias_f32(ca.bias),
+                           hi={"w": cu.kernel_weight(pad_in=pad), "bias": prepare.bias_f32(cu.bias)})
+            control.append(cn._zero_conv(cn.zero_convs[0], nchw_view(h16[:b])))
+            hs.append(nchw_view(h16[b:]))
+            start = 1
+
+        def twin_block(sa, sb, h16):
+            for la, lb in zip(sa, sb):
+                if isinstance(la, ResBlock):
+                    h16 = la.forward_twin(lb, h16, emb_c, emb_u)
+                elif isinstance(la, SpatialTransformer):
+                    h16 = la.forward_twin(lb, h16, ctx2d, nk)
+                else:
+                    h16 = la.run(h16, other=lb)
+            return h16
+
+        for i in range(start, len(cn.input_blocks)):
+            h16 = twin_block(cn.input_blocks[i], un.input_blocks[i], h16)
+            control.append(cn._zero_conv(cn.zero_convs[i], nchw_view(h16[:b])))
+            hs.append(nchw_view(h16[b:]))
+        h16 = twin_block(cn.middle_block, un.middle_block, h16)
+        control.append(cn._zero_conv(cn.middle_block_out, nchw_view(h16[:b])))
+        return control, nchw_view(h16[b:]), hs, emb_u, ctx
+
+    def control_and_unet(self, x, hint, t, cond_txt, control_of):
+        """apply_model's body for one ControlNet pass: the twin pass when twin_enabled(), else the ControlNet then the
+        UNet.  control_of(residuals) -> the control list the decoder consumes."""
+        diffusion_model = self.model.diffusion_model
+        if self.twin_enabled():
+            control, h, hs, emb, ctx = self._control_and_unet(x, hint, t, cond_txt)
+            return diffusion_model.decode(h, hs, emb, ctx, control_of(control), self.only_mid_control)
+        control = self.control_model(hint=hint, timesteps=t, context=cond_txt)
+        return diffusion_model(x=x, timesteps=t, context=cond_txt, control=control_of(control),
+                               only_mid_control=self.only_mid_control)
 
     def scaled_control(self, control):
         return [Scaled(c, s) for c, s in zip(control, self.control_scales)]

@@ -69,9 +69,7 @@ class ControlFinetuneLDM(ControlLDM):
             return diffusion_model(x=x_noisy, timesteps=t, context=cond_txt, control=None,
                                    only_mid_control=self.only_mid_control)
         hint = self.hint_latent(cond['c_concat'])
-        control = self.control_model(hint=hint, timesteps=t, context=cond_txt)
-        return diffusion_model(x=x_noisy, timesteps=t, context=cond_txt, control=self.scaled_control(control),
-                               only_mid_control=self.only_mid_control)
+        return self.control_and_unet(x_noisy, hint, t, cond_txt, self.scaled_control)
 
     def configure_optimizers(self):
         picked = trainable_parameters(self.control_model, './tmp/finetune_trainable_params.txt')

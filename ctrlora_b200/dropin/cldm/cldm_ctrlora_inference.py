@@ -187,7 +187,12 @@ class ControlInferenceLDM(ControlLDM):
         diffusion_model = self.model.diffusion_model
         cc = conds[0]['c_crossattn']
         cond_txt = cc[0] if len(cc) == 1 else torch.cat(cc, 1)
-        if len(conds) > 1 and getattr(self, "grouped_multi_lora", True):
+        if len(conds) == 1:
+            self.control_model.switch_lora(0)
+            hint = self.hint_latent(conds[0]['c_concat'])
+            return self.control_and_unet(x_noisy, hint, t, cond_txt, lambda st: [
+                Scaled(c, s * self.lora_weights[0]) for c, s in zip(st, self.control_scales)])
+        if getattr(self, "grouped_multi_lora", True):
             # all LoRA sets in one ControlNet pass (convs and ResBlock norms batched over the sets)
             hints = [self.hint_latent(cond['c_concat']) for cond in conds]
             stacks = self.control_model.forward_grouped(hints, t, cond_txt)
@@ -197,11 +202,8 @@ class ControlInferenceLDM(ControlLDM):
                 self.control_model.switch_lora(i)
                 hint = self.hint_latent(cond['c_concat'])
                 stacks.append(self.control_model(hint=hint, timesteps=t, context=cond_txt))
-        if len(stacks) == 1:
-            control = [Scaled(c, s * self.lora_weights[0]) for c, s in zip(stacks[0], self.control_scales)]
-        else:
-            # sum_i w_i * scale_j * control_i[j]  (reference :172-176): one n-ary kernel per residual, fp32 accumulate
-            control = [ops.weighted_sum([st[j] for st in stacks], [s * w for w in self.lora_weights])
-                       for j, s in enumerate(self.control_scales)]
+        # sum_i w_i * scale_j * control_i[j]  (reference :172-176): one n-ary kernel per residual, fp32 accumulate
+        control = [ops.weighted_sum([st[j] for st in stacks], [s * w for w in self.lora_weights])
+                   for j, s in enumerate(self.control_scales)]
         return diffusion_model(x=x_noisy, timesteps=t, context=cond_txt, control=control,
                                only_mid_control=self.only_mid_control)

@@ -68,15 +68,23 @@ class FeedForward(nn.Module):
         self.net = nn.Sequential(GEGLU(dim, inner_dim), nn.Dropout(dropout), nn.Linear(inner_dim, dim_out))
         self._prep = prepare.PrepCache()
 
-    def run(self, x2d, residual=None, out=None):
-        """x2d fp16 [M, dim] -> fp16 [M, dim_out] (+ residual)."""
-        out_buf = out
+    def _kernel_params(self):
         proj, out = self.net[0].proj, self.net[2]
         lk = prepare.lora_key
         w1 = self._prep.get(("w1", lk(proj)), prepare.linear_params(proj), lambda: prepare.effective_linear_weight(proj))
         w2 = self._prep.get(("w2", lk(out)), prepare.linear_params(out), lambda: prepare.effective_linear_weight(out))
-        g = ops.gemm(x2d, w1, bias=prepare.bias_f32(proj.bias), geglu=True)
-        return ops.gemm(g, w2, bias=prepare.bias_f32(out.bias), residual=residual, out=out_buf)
+        return w1, prepare.bias_f32(proj.bias), w2, prepare.bias_f32(out.bias)
+
+    def run(self, x2d, residual=None, out=None, other=None):
+        """x2d fp16 [M, dim] -> fp16 [M, dim_out] (+ residual).  other: the same layer of a second network, applied to
+        the upper half of the rows in the same launches."""
+        w1, b1, w2, b2 = self._kernel_params()
+        h1 = h2 = None
+        if other is not None:
+            ow1, ob1, ow2, ob2 = other._kernel_params()
+            h1, h2 = {"w": ow1, "bias": ob1}, {"w": ow2, "bias": ob2}
+        g = ops.gemm(x2d, w1, bias=b1, geglu=True, hi=h1)
+        return ops.gemm(g, w2, bias=b2, residual=residual, out=out, hi=h2)
 
     def forward(self, x):
         shp = x.shape
@@ -105,16 +113,19 @@ class CrossAttention(nn.Module):
         lins = [self.to_k, self.to_v]
         return prepare._ver(*[p for lin in lins for p in prepare.linear_params(lin)]) + prepare.lora_key(*lins)
 
-    def project_context(self, ctx2d, batch, nk, ctx_key):
-        """K and V^T of a step-invariant context, into persistent buffers (see ControlLDM.prepare_context)."""
+    def project_context(self, ctx2d, batch, nk, ctx_key, out=None):
+        """K and V^T of a step-invariant context, into persistent buffers (see ControlLDM.prepare_context); `out`:
+        the (K, V^T) buffers to use."""
         inner = self.to_q.out_features
         h, d = self.heads, inner // self.heads
         nk_pad = (nk + 7) // 8 * 8
         token = (ctx_key, ctx2d.data_ptr(), self._kv_weight_token())
         hit = self.__dict__.get("_kv_cache")
-        if hit is not None and hit[0] == token:
+        if hit is not None and hit[0] == token and (out is None or hit[1].data_ptr() == out[0].data_ptr()):
             return
-        if hit is not None and hit[1].shape == (batch * nk, inner) and hit[2].shape == (batch, h, d, nk_pad):
+        if out is not None:
+            k, vt = out
+        elif hit is not None and hit[1].shape == (batch * nk, inner) and hit[2].shape == (batch, h, d, nk_pad):
             k, vt = hit[1], hit[2]  # same addresses: captured graphs keep reading them
         else:
             k = torch.empty((batch * nk, inner), device=ctx2d.device, dtype=torch.float16)
@@ -122,6 +133,55 @@ class CrossAttention(nn.Module):
         w = self._cat_weight("kv", [self.to_k, self.to_v])
         ops.gemm(ctx2d, w, seg_outs=[k, vt], seg_width=inner, transposed=(0, 1, 0), rows_per_img=nk, head_dim=d, tok_pad=nk_pad)
         self.__dict__["_kv_cache"] = (token, k, vt)
+
+    def _kv_hit(self, ctx2d, batch, nk):
+        """(K, V^T) that project_context computed for this context and these weights, or None"""
+        hit = self.__dict__.get("_kv_cache")
+        if hit is not None and hit[0][1] == ctx2d.data_ptr() and hit[0][2] == self._kv_weight_token() and \
+                hit[1].shape[0] == batch * nk:
+            return hit[1], hit[2]
+        return None
+
+    def run_twin(self, other, x2d, batch, nq, ctx2d=None, nk=None, residual=None):
+        """run() of this layer on the lower half of the batch and of `other` (the same layer of a second network) on
+        the upper half: grouped projections, one batch-`batch` attention launch.  Cross-attention reads both layers'
+        K / V^T of the (shared) context from one buffer pair, the one ControlLDM.prepare_context filled, or from
+        projections computed here."""
+        inner = self.to_q.out_features
+        h, d = self.heads, inner // self.heads
+        dev = x2d.device
+        if ctx2d is None:
+            nk = nq
+            nk_pad = (nk + 7) // 8 * 8
+            q = torch.empty((batch * nq, inner), device=dev, dtype=torch.float16)
+            k = torch.empty_like(q)
+            vt = torch.empty((batch, h, d, nk_pad), device=dev, dtype=torch.float16)
+            lins = [self.to_q, self.to_k, self.to_v]
+            ops.gemm(x2d, self._cat_weight("qkv", lins), seg_outs=[q, k, vt], seg_width=inner, transposed=(0, 0, 1),
+                     rows_per_img=nk, head_dim=d, tok_pad=nk_pad,
+                     hi={"w": other._cat_weight("qkv", [other.to_q, other.to_k, other.to_v])})
+        else:
+            half = batch // 2
+            nk_pad = (nk + 7) // 8 * 8
+            q = ops.gemm(x2d, self._q_weight(), hi={"w": other._q_weight()})
+            mine, theirs, shared = self._kv_hit(ctx2d, half, nk), other._kv_hit(ctx2d, half, nk), self.__dict__.get("_kv_twin")
+            if mine is not None and theirs is not None and shared is not None and \
+                    mine[0].data_ptr() == shared[0].data_ptr() and theirs[0].data_ptr() == shared[0][half * nk:].data_ptr():
+                k, vt = shared
+            else:
+                k = torch.empty((batch * nk, inner), device=dev, dtype=torch.float16)
+                vt = ops.zeros((batch, h, d, nk_pad), dev)
+                for m, lo in ((self, True), (other, False)):
+                    rows, imgs = slice(0, half * nk) if lo else slice(half * nk, None), slice(0, half) if lo else slice(half, None)
+                    ops.gemm(ctx2d, m._cat_weight("kv", [m.to_k, m.to_v]), seg_outs=[k[rows], vt[imgs]], seg_width=inner,
+                             transposed=(0, 1, 0), rows_per_img=nk, head_dim=d, tok_pad=nk_pad)
+        o = ops.attention(q, k, vt, batch, h, nq, nk, d)
+        return ops.gemm(o, self._out_weight(), bias=prepare.bias_f32(self.to_out[0].bias), residual=residual,
+                        hi={"w": other._out_weight(), "bias": prepare.bias_f32(other.to_out[0].bias)})
+
+    def _q_weight(self):
+        return self._prep.get(("q", prepare.lora_key(self.to_q)), prepare.linear_params(self.to_q),
+                              lambda: prepare.effective_linear_weight(self.to_q))
 
     def run(self, x2d, batch, nq, ctx2d=None, nk=None, residual=None):
         """x2d fp16 [batch*nq, C]; ctx2d fp16 [batch*nk, Cctx] or None (self-attention). Returns to_out(attn) (+residual)."""
@@ -139,13 +199,10 @@ class CrossAttention(nn.Module):
                      tok_pad=nk_pad)
         else:
             nk_pad = (nk + 7) // 8 * 8
-            wq = self._prep.get(("q", prepare.lora_key(self.to_q)), prepare.linear_params(self.to_q),
-                                lambda: prepare.effective_linear_weight(self.to_q))
-            q = ops.gemm(x2d, wq)
-            hit = self.__dict__.get("_kv_cache")
-            if hit is not None and hit[0][1] == ctx2d.data_ptr() and hit[0][2] == self._kv_weight_token() and \
-                    hit[1].shape[0] == batch * nk:
-                return self._finish(ops.attention(q, hit[1], hit[2], batch, h, nq, nk, d), q, batch, nq, residual)
+            q = ops.gemm(x2d, self._q_weight())
+            hit = self._kv_hit(ctx2d, batch, nk)
+            if hit is not None:
+                return self._finish(ops.attention(q, hit[0], hit[1], batch, h, nq, nk, d), q, batch, nq, residual)
             k = torch.empty((batch * nk, inner), device=dev, dtype=torch.float16)
             # the key padding columns (77 -> 80) are never written by the projection, and ops.attention never reads
             # them: its V^T tensor map ends at key nk, so keys >= nk load as zeros.  The zero fill is not needed for
@@ -196,9 +253,18 @@ class BasicTransformerBlock(nn.Module):
         self.checkpoint = checkpoint
 
     @staticmethod
-    def _ln(norm, x2d):
+    def _ln(norm, x2d, other=None):
+        """LayerNorm `norm` (of the upper half of the rows: `other`, the same layer of a second network)"""
         norm = prepare.effective(norm)
-        return ops.layernorm(x2d, prepare.bias_f32(norm.weight), prepare.bias_f32(norm.bias), norm.eps)
+        hi = {} if other is None else {"gamma_hi": prepare.bias_f32(prepare.effective(other).weight),
+                                       "beta_hi": prepare.bias_f32(prepare.effective(other).bias)}
+        return ops.layernorm(x2d, prepare.bias_f32(norm.weight), prepare.bias_f32(norm.bias), norm.eps, **hi)
+
+    def run_twin(self, other, x2d, batch, n, ctx2d, nk):
+        """run() of this block on the lower half of the batch and of `other` on the upper half (self-attention blocks)"""
+        x2d = self.attn1.run_twin(other.attn1, self._ln(self.norm1, x2d, other.norm1), batch, n, residual=x2d)
+        x2d = self.attn2.run_twin(other.attn2, self._ln(self.norm2, x2d, other.norm2), batch, n, ctx2d, nk, residual=x2d)
+        return self.ff.run(self._ln(self.norm3, x2d, other.norm3), residual=x2d, other=other.ff)
 
     def run(self, x2d, batch, n, ctx2d, nk, out=None):
         """x2d fp16 [batch*n, dim] -> same shape (reference _forward :271-275); `out`: optional destination buffer."""
@@ -243,6 +309,22 @@ class SpatialTransformer(nn.Module):
             return self._prep.get((key, prepare.lora_key(mod)), prepare.linear_params(mod),
                                   lambda: prepare.effective_linear_weight(mod))
         return self._prep.get(key, [mod.weight], lambda: prepare.conv_weight(mod.weight))
+
+    def forward_twin(self, other, xp, ctx2d, nk):
+        """This transformer on the lower half of the pixel-major batch `xp` and `other` (the same layer of a second
+        network) on the upper half, one launch per kernel; ctx2d: fp16 [batch/2 * nk, D] context of both halves."""
+        b, h, w, c = xp.shape
+        f32 = prepare.bias_f32
+        gn, ogn = prepare.effective(self.norm), prepare.effective(other.norm)
+        xn = ops.groupnorm(xp, f32(gn.weight), f32(gn.bias), gn.eps, False, groups=gn.num_groups, gamma_hi=f32(ogn.weight),
+                           beta_hi=f32(ogn.bias))
+        y = ops.gemm(xn, self._w("in", self.proj_in), bias=f32(self.proj_in.bias),
+                     hi={"w": other._w("in", other.proj_in), "bias": f32(other.proj_in.bias)})
+        y2d = y.view(b * h * w, -1)
+        for block, oblock in zip(self.transformer_blocks, other.transformer_blocks):
+            y2d = block.run_twin(oblock, y2d, b, h * w, ctx2d, nk)
+        return ops.gemm(y2d.view(b, h, w, -1), self._w("out", self.proj_out), bias=f32(self.proj_out.bias),
+                        residual=xp.view(b * h * w, c), hi={"w": other._w("out", other.proj_out), "bias": f32(other.proj_out.bias)})
 
     def forward_grouped(self, x, context, n_groups, attach):
         """One pass over a batch made of `n_groups` equal slices that use DIFFERENT LoRA / norm sets (multi-LoRA inference,

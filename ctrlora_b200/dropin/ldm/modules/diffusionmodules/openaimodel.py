@@ -111,14 +111,20 @@ class Downsample(nn.Module):
         self.op = nn.Conv2d(self.channels, self.out_channels, 3, stride=2, padding=padding)
         self._prep = prepare.PrepCache()
 
+    def _weight(self):
+        return self._prep.get("w", [self.op.weight],
+                              lambda: prepare.conv_weight(self.op.weight).view(self.out_channels, 1, 9 * self.channels))
+
+    def run(self, xp, out=None, other=None):
+        """pixel-major fp16 [B, H, W, C] -> [B, H/2, W/2, Cout] (into `out` if given); `other`: the same layer of a
+        second network, applied to the upper half of the batch in the same launch."""
+        col = ops.im2col_s2(xp.contiguous())  # [B, H/2, W/2, 9*C]
+        hi = None if other is None else {"w": other._weight(), "bias": prepare.bias_f32(other.op.bias)}
+        return ops.gemm(col, self._weight(), bias=prepare.bias_f32(self.op.bias), out=out, hi=hi)
+
     def forward(self, x):
         assert x.shape[1] == self.channels
-        xp = pixel_major(x).contiguous()
-        b, h, w, c = xp.shape
-        col = ops.im2col_s2(xp)  # [B, H/2, W/2, 9*C]
-        wk = self._prep.get("w", [self.op.weight],
-                            lambda: prepare.conv_weight(self.op.weight).view(self.out_channels, 1, 9 * c))
-        return nchw_view(ops.gemm(col, wk, bias=prepare.bias_f32(self.op.bias)))
+        return nchw_view(self.run(pixel_major(x)))
 
 
 class ResBlock(TimestepBlock):
@@ -149,30 +155,23 @@ class ResBlock(TimestepBlock):
             self.skip_connection = nn.Conv2d(channels, self.out_channels, 1)
         self._prep = prepare.PrepCache()
 
-    def emb_weight(self):
-        lin = self.emb_layers[1]
-        return self._prep.get("emb", prepare.linear_params(lin),
-                              lambda: prepare.effective_linear_weight(lin).view(lin.out_features, lin.in_features))
-
-    def forward(self, x, emb):
+    def _kernel_params(self):
+        """the prepared operands of the block's kernels: GroupNorm affines, conv weights and biases"""
         f32 = prepare.bias_f32
         gn1, conv1 = self.in_layers[0], self.in_layers[2]
         gn2, conv2 = self.out_layers[0], self.out_layers[3]
-        has_skip_conv = not isinstance(self.skip_connection, nn.Identity)
-        if isinstance(x, CatSpec):
-            x1 = pixel_major(x.x1)
-            res = ops.groupnorm(x1, f32(gn1.weight), f32(gn1.bias), gn1.eps, True,
-                                add1=None if x.add1 is None else pixel_major(x.add1), add1_scale=x.s1,
-                                x2=None if x.x2 is None else pixel_major(x.x2),
-                                add2=None if x.add2 is None else pixel_major(x.add2), add2_scale=x.s2,
-                                want_raw=True)
-            a, xp = res
-        else:
-            xp = pixel_major(x)
-            a = ops.groupnorm(xp, f32(gn1.weight), f32(gn1.bias), gn1.eps, True)
-        b, h, w, cin = xp.shape
-        assert cin == self.channels, (cin, self.channels)
-        # time-embedding term: a slice of the network's batched GEMV, or this block's own small linear
+        k = {"gn1": (f32(gn1.weight), f32(gn1.bias), gn1.eps), "gn2": (f32(gn2.weight), f32(gn2.bias), gn2.eps),
+             "w1": self._prep.get("w1", [conv1.weight], lambda: prepare.conv_weight(conv1.weight)), "b1": f32(conv1.bias),
+             "w2": self._prep.get("w2", [conv2.weight], lambda: prepare.conv_weight(conv2.weight)), "wsk": None,
+             "b2": f32(conv2.bias)}
+        if not isinstance(self.skip_connection, nn.Identity):
+            sk = self.skip_connection
+            k["wsk"] = self._prep.get("wsk", [sk.weight], lambda: prepare.conv_weight(sk.weight).view(self.out_channels, -1))
+            k["b2"] = self._prep.get("bsum", [conv2.bias, sk.bias], lambda: (conv2.bias.float() + sk.bias.float()).contiguous())
+        return k
+
+    def _rowbias(self, emb):
+        """time-embedding term: a slice of the network's batched GEMV, or this block's own small linear"""
         if isinstance(emb, EmbPack):
             rowbias = emb.slices.get(id(self))
             raw = emb.raw
@@ -180,18 +179,50 @@ class ResBlock(TimestepBlock):
             rowbias, raw = None, emb
         if rowbias is None:
             lin = self.emb_layers[1]
-            rowbias = ops.small_linear(raw.float().contiguous(), self.emb_weight(), f32(lin.bias), silu_in=True)
-        w1 = self._prep.get("w1", [conv1.weight], lambda: prepare.conv_weight(conv1.weight))
-        hmid = ops.gemm(a, w1, ksize=3, bias=f32(conv1.bias), rowbias=rowbias)
-        c = ops.groupnorm(hmid, f32(gn2.weight), f32(gn2.bias), gn2.eps, True)
-        w2 = self._prep.get("w2", [conv2.weight], lambda: prepare.conv_weight(conv2.weight))
-        if has_skip_conv:
-            sk = self.skip_connection
-            wsk = self._prep.get("wsk", [sk.weight], lambda: prepare.conv_weight(sk.weight).view(self.out_channels, cin))
-            bsum = self._prep.get("bsum", [conv2.bias, sk.bias], lambda: (conv2.bias.float() + sk.bias.float()).contiguous())
-            out = ops.gemm(c, w2, ksize=3, bias=bsum, a2=xp, w2=wsk)
+            rowbias = ops.small_linear(raw.float().contiguous(), self.emb_weight(), prepare.bias_f32(lin.bias), silu_in=True)
+        return rowbias
+
+    def forward_twin(self, other, xp, emb, emb_other):
+        """This block on the lower half of the pixel-major batch `xp` and `other` (the same block of a second network)
+        on the upper half, one launch per kernel; emb / emb_other: each network's time embedding."""
+        k, o = self._kernel_params(), other._kernel_params()
+        a = ops.groupnorm(xp, k["gn1"][0], k["gn1"][1], k["gn1"][2], True, gamma_hi=o["gn1"][0], beta_hi=o["gn1"][1])
+        hmid = ops.gemm(a, k["w1"], ksize=3, bias=k["b1"], rowbias=self._rowbias(emb),
+                        hi={"w": o["w1"], "bias": o["b1"], "rowbias": other._rowbias(emb_other)})
+        c = ops.groupnorm(hmid, k["gn2"][0], k["gn2"][1], k["gn2"][2], True, gamma_hi=o["gn2"][0], beta_hi=o["gn2"][1])
+        if k["wsk"] is not None:
+            return ops.gemm(c, k["w2"], ksize=3, bias=k["b2"], a2=xp, w2=k["wsk"],
+                            hi={"w": o["w2"], "bias": o["b2"], "w2": o["wsk"]})
+        b, h, w, cin = xp.shape
+        return ops.gemm(c, k["w2"], ksize=3, bias=k["b2"], residual=xp.view(b * h * w, cin), hi={"w": o["w2"], "bias": o["b2"]})
+
+    def emb_weight(self):
+        lin = self.emb_layers[1]
+        return self._prep.get("emb", prepare.linear_params(lin),
+                              lambda: prepare.effective_linear_weight(lin).view(lin.out_features, lin.in_features))
+
+    def forward(self, x, emb):
+        k = self._kernel_params()
+        (g1, b1, eps1), (g2, b2, eps2) = k["gn1"], k["gn2"]
+        if isinstance(x, CatSpec):
+            x1 = pixel_major(x.x1)
+            res = ops.groupnorm(x1, g1, b1, eps1, True,
+                                add1=None if x.add1 is None else pixel_major(x.add1), add1_scale=x.s1,
+                                x2=None if x.x2 is None else pixel_major(x.x2),
+                                add2=None if x.add2 is None else pixel_major(x.add2), add2_scale=x.s2,
+                                want_raw=True)
+            a, xp = res
         else:
-            out = ops.gemm(c, w2, ksize=3, bias=f32(conv2.bias), residual=xp.view(b * h * w, cin))
+            xp = pixel_major(x)
+            a = ops.groupnorm(xp, g1, b1, eps1, True)
+        b, h, w, cin = xp.shape
+        assert cin == self.channels, (cin, self.channels)
+        hmid = ops.gemm(a, k["w1"], ksize=3, bias=k["b1"], rowbias=self._rowbias(emb))
+        c = ops.groupnorm(hmid, g2, b2, eps2, True)
+        if k["wsk"] is not None:
+            out = ops.gemm(c, k["w2"], ksize=3, bias=k["b2"], a2=xp, w2=k["wsk"])
+        else:
+            out = ops.gemm(c, k["w2"], ksize=3, bias=k["b2"], residual=xp.view(b * h * w, cin))
         return nchw_view(out)
 
 

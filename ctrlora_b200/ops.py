@@ -138,13 +138,22 @@ def _as_bhwc(a):
 def gemm(a, w, *, ksize=1, bias=None, rowbias=None, rows_per_img=0, rowbias_ld=0, residual=None, out_scale=1.0, a2=None,
          w2=None,
          geglu=False, out=None, out_f32=False, seg_outs=None, seg_width=0, transposed=(0, 0, 0), head_dim=0,
-         tok_pad=0, block_n=0, split_k=0, dup_out=None, single_cta=False, simt=False):
+         tok_pad=0, block_n=0, split_k=0, dup_out=None, single_cta=False, simt=False, hi=None):
     """out = epilogue(conv_or_linear(a, w) [+ a2 @ w2^T]); see `ctrlora_gemm_f16` in include/ctrlora_b200.h.
 
     a: fp16 [B,H,W,C] or [M,K]; w: fp16 [N(2N), ksize*ksize, C]; returns the output tensor ([..., N]).
+    hi: grouped launch of two same-shaped layers over the two halves of the batch (images of a [B,H,W,C] `a`, rows of
+    an [M,K] one): a dict with the upper half's "w" and, as the call has them, "bias", "rowbias" (indexed from the
+    half's first image) and "w2".  A batch whose halves cannot be tiled apart runs as two launches.
     """
     _require_cuda(a, w)
     assert a.dtype == torch.float16 and w.dtype == torch.float16 and w.is_contiguous()
+    if hi is not None:
+        return _gemm_grouped(a, w, hi, dict(ksize=ksize, bias=bias, rowbias=rowbias, rows_per_img=rows_per_img,
+                                            rowbias_ld=rowbias_ld, residual=residual, out_scale=out_scale, a2=a2, w2=w2,
+                                            geglu=geglu, out=out, out_f32=out_f32, seg_outs=seg_outs, seg_width=seg_width,
+                                            transposed=transposed, head_dim=head_dim, tok_pad=tok_pad, block_n=block_n,
+                                            split_k=split_k))
     b, h, wd, c, ld = _as_bhwc(a)
     n_rows = w.shape[0]
     n = n_rows // 2 if geglu else n_rows
@@ -193,6 +202,20 @@ def gemm(a, w, *, ksize=1, bias=None, rowbias=None, rows_per_img=0, rowbias_ld=0
     args.force_single_cta = int(single_cta)
     lib = _lib.load()
     fn = lib.ctrlora_gemm_f16_simt if simt else lib.ctrlora_gemm_f16
+    if _GROUP is not None:
+        group_b, g = _GROUP
+        args.group_b, args.w_hi, args.w2_hi = group_b, _ptr(g["w"]), _ptr(g.get("w2"))
+        args.bias_hi, args.rowbias_hi = _ptr(g.get("bias")), _ptr(g.get("rowbias"))
+        rc = fn(C.addressof(args), _sp())
+        if rc == _lib.STATUS_UNSUPPORTED:
+            return None  # a tile would straddle the halves: the caller launches them one by one
+        check(rc, "ctrlora_gemm_f16 (grouped)")
+        _count()
+        if _GEMM_RECORD is not None:
+            ktot = ksize * ksize * c + (args.a2_c if a2 is not None else 0)
+            _GEMM_RECORD.append((args, 2.0 * M * n_rows * ktot,
+                                 (a, w, a2, w2, bias, rowbias, residual, out, seg_outs, dup_out, ws, cnt, g)))
+        return ret
     _count()
     if _GEMM_RECORD is not None and not simt:
         ktot = ksize * ksize * c + (args.a2_c if a2 is not None else 0)
@@ -212,6 +235,53 @@ def gemm(a, w, *, ksize=1, bias=None, rowbias=None, rows_per_img=0, rowbias_ld=0
         return ret
     check(fn(C.addressof(args), _sp()), "ctrlora_gemm_f16")
     return ret
+
+
+_GROUP = None  # (group_b, upper half's operands) while _gemm_grouped issues its launch
+
+
+def _gemm_grouped(a, w, hi, kw):
+    """One launch over both halves of the batch (see gemm's `hi`), or one launch per half where a tile would straddle
+    them.  An [M, K] `a` is viewed as two images of M/2 rows."""
+    global _GROUP
+    assert a.shape[0] % 2 == 0
+    half = a.shape[0] // 2
+    a4 = a.view(2, 1, half, a.shape[1]) if a.dim() == 2 else a
+    out = kw.pop("out")
+    if out is None and kw["seg_outs"] is None:
+        out = torch.empty(a.shape[:-1] + (w.shape[0] // 2 if kw["geglu"] else w.shape[0],), device=a.device,
+                          dtype=torch.float32 if kw["out_f32"] else torch.float16)
+    out4 = out.view(a4.shape[:3] + (out.shape[-1],)) if out is not None and a.dim() == 2 else out
+    g = {k: v for k, v in hi.items() if v is not None}
+    if "rowbias" in g:  # the kernel reads both halves' row terms with the lower half's row stride
+        assert kw["rowbias"] is not None and g["rowbias"].stride(0) == kw["rowbias"].stride(0) and \
+            g["rowbias"].stride(-1) == 1, "the two halves' row terms need one row stride"
+    _GROUP = (a4.shape[0] // 2, g)
+    try:
+        ret = gemm(a4, w, out=out4, **kw)
+    finally:
+        _GROUP = None
+    if ret is not None:
+        return kw["seg_outs"] if kw["seg_outs"] is not None else out
+    # two plain launches: rows of the row-indexed operands, images of the V^T-layout segments
+    rows = half if a.dim() == 2 else half * a.shape[1] * a.shape[2]
+    imgs = rows // (kw["rows_per_img"] or rows)
+
+    def cut(t, lo, by_image=False):
+        if t is None:
+            return None
+        n = imgs if by_image else (half if t.dim() == 4 else rows)
+        return t[:n] if lo else t[n:]
+
+    for lo in (True, False):
+        k = dict(kw)
+        k["residual"], k["a2"] = cut(kw["residual"], lo), cut(kw["a2"], lo)
+        if kw["seg_outs"] is not None:
+            k["seg_outs"] = [cut(o, lo, by_image=bool(t)) for o, t in zip(kw["seg_outs"], kw["transposed"])]
+        if not lo:
+            k["bias"], k["rowbias"], k["w2"] = hi.get("bias"), hi.get("rowbias"), hi.get("w2")
+        gemm(cut(a, lo), w if lo else hi["w"], out=cut(out, lo), **k)
+    return kw["seg_outs"] if kw["seg_outs"] is not None else out
 
 
 def _dp(t):
@@ -297,8 +367,9 @@ def _gn_partial_buffers(device):
 
 
 def groupnorm(x1, gamma, beta, eps, silu, *, add1=None, add1_scale=1.0, x2=None, add2=None, add2_scale=1.0,
-              groups=32, want_raw=False, stats_ws=None, want_stats=False, out=None):
-    """GroupNorm(+SiLU) over [x1 (+s1*add1) | x2 (+s2*add2)], pixel-major fp16 [B,H,W,C*]; returns y (and raw concat)."""
+              groups=32, want_raw=False, stats_ws=None, want_stats=False, out=None, gamma_hi=None, beta_hi=None):
+    """GroupNorm(+SiLU) over [x1 (+s1*add1) | x2 (+s2*add2)], pixel-major fp16 [B,H,W,C*]; returns y (and raw concat).
+    gamma_hi / beta_hi: the affine parameters of the upper half of the batch (two networks' layers in one launch)."""
     _require_cuda(x1, x2, add1, add2)
     b, h, w, c1, ld1 = _as_bhwc(x1)
     c2, ld2 = 0, 0
@@ -322,6 +393,9 @@ def groupnorm(x1, gamma, beta, eps, silu, *, add1=None, add1_scale=1.0, x2=None,
     a.batch, a.hw, a.groups = b, h * w, groups
     assert gamma.dtype == torch.float32 and beta.dtype == torch.float32 and gamma.numel() == ctot
     a.gamma, a.beta, a.eps, a.silu = _dp(gamma), _dp(beta), float(eps), int(silu)
+    if gamma_hi is not None:
+        assert b % 2 == 0 and gamma_hi.numel() == ctot and beta_hi.numel() == ctot
+        a.gamma_hi, a.beta_hi, a.group_b = _dp(gamma_hi), _dp(beta_hi), b // 2
     a.y, a.raw_out, a.stats_ws = _dp(y), _dp(raw), _dp(stats_ws)
     if not torch.cuda.is_current_stream_capturing() or x1.device.index in _GN_PARTIAL or torch.cuda.current_device() in _GN_PARTIAL:
         pws, pcnt = _gn_partial_buffers(x1.device)  # (never first allocated inside a capture)
@@ -341,13 +415,20 @@ def zeros(shape, device, dtype=torch.float16):
     return t
 
 
-def layernorm(x, gamma, beta, eps=1e-5):
-    """x fp16 [..., C] with contiguous last dim and uniform row stride."""
+def layernorm(x, gamma, beta, eps=1e-5, gamma_hi=None, beta_hi=None):
+    """x fp16 [..., C] with contiguous last dim and uniform row stride.  gamma_hi / beta_hi: the affine parameters of the
+    upper half of the rows (two networks' layers in one launch)."""
     _require_cuda(x)
     cols = x.shape[-1]
     x2 = x.reshape(-1, cols)
     y = torch.empty((x2.shape[0], cols), device=x.device, dtype=torch.float16)
     _count(1)
+    if gamma_hi is not None:
+        assert x2.shape[0] % 2 == 0
+        check(_lib.load().ctrlora_layernorm_grouped_f16(_dp(x2), x2.stride(0), _dp(y), cols, x2.shape[0], cols, _dp(gamma),
+                                                        _dp(beta), _dp(gamma_hi), _dp(beta_hi), x2.shape[0] // 2,
+                                                        float(eps), _sp()), "ctrlora_layernorm_grouped_f16")
+        return y.view(x.shape)
     check(_lib.load().ctrlora_layernorm_f16(_dp(x2), x2.stride(0), _dp(y), cols, x2.shape[0], cols, _dp(gamma), _dp(beta),
                                             float(eps), _sp()), "ctrlora_layernorm_f16")
     return y.view(x.shape)

@@ -79,6 +79,15 @@ typedef struct ctrlora_gemm_args {
     void* dup_out;          /* optional: transposed segments are also stored row-major here (fp16, row stride dup_ld) */
     int dup_ld;
     int force_single_cta;   /* accepted for ABI compatibility; every tile is one CTA */
+    /* Grouped launch: two same-shaped layers of two networks over one batch (the ControlNet and the UNet encoder run as
+     * one pass).  group_b > 0: images (a_b index) >= group_b take w_hi, w2_hi, bias_hi and rowbias_hi, whose rows are
+     * indexed from image img - group_b * a_h * a_w / rows_per_img.  Every tile must lie in one group: when group_b is
+     * not a multiple of the images one tile covers, the call returns CTRLORA_STATUS_UNSUPPORTED and launches nothing. */
+    int group_b;
+    const void* w_hi;
+    const float* bias_hi;
+    const float* rowbias_hi;
+    const void* w2_hi;
 } ctrlora_gemm_args;
 
 int ctrlora_gemm_f16(const ctrlora_gemm_args* args, void* stream);
@@ -111,12 +120,19 @@ typedef struct ctrlora_groupnorm_args {
     long long partial_ws_floats;
     unsigned int* partial_counters;   /* [>= batch] arrival counters: all zero on entry, left all zero on exit */
     int partial_counters_len;
+    /* Grouped forward (two networks' GroupNorms over one batch): images >= group_b (0 = off) take gamma_hi / beta_hi.
+     * Statistics stay per image and are computed as by a call over images [0, group_b) and one over the rest. */
+    const float* gamma_hi; const float* beta_hi; int group_b;
 } ctrlora_groupnorm_args;
 int ctrlora_groupnorm_f16(const ctrlora_groupnorm_args* args, void* stream);
 
 /* LayerNorm over the last dim (eps 1e-5 in the reference: ldm/modules/attention.py:263-265), fp16 in/out. */
 int ctrlora_layernorm_f16(const void* x, long long ldx, void* y, long long ldy, int rows, int cols,
                           const float* gamma, const float* beta, float eps, void* stream);
+/* The same LayerNorm over the rows of two networks' layers in one launch: rows >= split_rows take gamma_hi / beta_hi. */
+int ctrlora_layernorm_grouped_f16(const void* x, long long ldx, void* y, long long ldy, int rows, int cols,
+                                  const float* gamma, const float* beta, const float* gamma_hi, const float* beta_hi,
+                                  int split_rows, float eps, void* stream);
 
 /* Fused attention forward: out[b, i, h*d:(h+1)*d] = softmax_j(q_i . k_j * d^-1/2) v_j   (fp32 logits / softmax).
  * replaces CrossAttention.forward   ldm/modules/attention.py:163-194 (and MemoryEfficientCrossAttention :197-243).
@@ -239,7 +255,7 @@ int ctrlora_attention_bwd_f16(const void* q, long long ldq, const void* k, long 
                               float* delta_ws, void* dq, long long lddq, void* dk, long long lddk, void* dv, long long lddv,
                               int batch, int heads, int nq, int nk, int head_dim, void* stream);
 
-/* GroupNorm(+SiLU) backward: same source description as the forward (`args`, whose stats_ws is a scratch buffer for the
+/* GroupNorm(+SiLU) backward: same source description as the forward (`args`, not grouped; its stats_ws is a scratch buffer for the
  * backward statistics); fwd_stats = the {sum, sumsq} buffer the forward left in ITS stats_ws.  dx1 / dx2: gradients of
  * the two concat halves (fp16, row strides ldd1 / ldd2, scaled by dx*_scale; dx2 may be NULL).  dgamma/dbeta (fp32 [C],
  * accumulated into) may be NULL. */
