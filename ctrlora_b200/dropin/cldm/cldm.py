@@ -8,11 +8,12 @@ Data flow of one `apply_model` (reference :329-344 and cldm_ctrlora_finetune.py:
     reference (:34-42, finetune :79) are not separate passes over HBM.
 
 Twin pass (ControlLDM._control_and_unet): the ControlNet and the UNet encoder have the same shapes layer for layer and
-do not depend on each other, so sampling runs them as one batch-2B pass: images [0, B) are the hint's, [B, 2B) x's, and
-each launch takes the ControlNet's weights for the lower half and the UNet's for the upper half (grouped GEMM, GroupNorm
-and LayerNorm launches).  The zero-convs read the lower half, the decoder's skips are views of the upper half.
-Environment: CTRLORA_TWIN_ENCODER=0 runs the two networks one after the other; CTRLORA_TWIN_FROM=L (0-3) runs the
-blocks above resolution level L at batch B per network and starts the twin pass at level L.
+do not depend on each other, so sampling runs them as one batch-2B pass from the first Downsample on: images [0, B) are
+the hint's, [B, 2B) x's, and each launch takes the ControlNet's weights for the lower half and the UNet's for the upper
+half (grouped GEMM, GroupNorm and LayerNorm launches).  Every layer has one forward body; the UNet's layer, passed as
+`other`, turns its launches into grouped ones.  The full-resolution blocks run at batch B per network.  The zero-convs
+read the lower half, the decoder's skips are views of the upper half.  CTRLORA_TWIN_ENCODER=0 runs the two networks one
+after the other.
 """
 import os
 
@@ -192,17 +193,6 @@ class ControlNet(nn.Module):
         return self._encode(hint, emb, _ctx16(context))
 
 
-TWIN_FROM_DEFAULT = 1  # CTRLORA_TWIN_FROM when unset
-
-
-def twin_from_level():
-    """CTRLORA_TWIN_FROM: the resolution level (0-3) at which the twin pass starts"""
-    v = os.environ.get("CTRLORA_TWIN_FROM", str(TWIN_FROM_DEFAULT)).strip()
-    if v not in ("0", "1", "2", "3"):
-        raise ValueError(f"CTRLORA_TWIN_FROM={v!r}: expected a resolution level 0, 1, 2 or 3")
-    return int(v)
-
-
 class ControlLDM(LatentDiffusion):
     def __init__(self, control_stage_config, control_key, only_mid_control, global_average_pooling=False, *args, **kwargs):
         super().__init__(*args, **kwargs)
@@ -278,7 +268,7 @@ class ControlLDM(LatentDiffusion):
         """The layer pairs of the twin pass, or None when the ControlNet and the UNet encoder differ in structure (the
         style variant's IP-Adapter UNet, say).  Checked once per model: "cross" are the cross-attention pairs, "norms"
         the transformer norm pairs, whose effective layers (switch_lora re-points the inference ControlNet's) must have
-        one eps when the pass runs."""
+        one eps when the pass runs.  The pass starts after the first Downsample, so a network without one has none."""
         from ldm.modules.attention import BasicTransformerBlock, CrossAttention
         if "_twin" in self.__dict__:
             return self.__dict__["_twin"]
@@ -308,7 +298,7 @@ class ControlLDM(LatentDiffusion):
 
         seqs = list(zip(cn.input_blocks, un.input_blocks)) + [(cn.middle_block, un.middle_block)]
         ok = isinstance(un, ControlledForward) and len(cn.input_blocks) == len(un.input_blocks) and \
-            cn.model_channels == un.model_channels and all(
+            cn.model_channels == un.model_channels and any(isinstance(m[0], Downsample) for m in cn.input_blocks) and all(
                 len(a) == len(b) and all(same(x, y) for x, y in zip(a, b)) for a, b in seqs)
         res = None
         if ok:
@@ -342,59 +332,32 @@ class ControlLDM(LatentDiffusion):
         emb_c = cn.embed(t, out_all=torch.empty((b, ld), device=x.device, dtype=torch.float32)[:, :wc])
         emb_u = un.embed(t, out_all=torch.empty((b, ld), device=x.device, dtype=torch.float32)[:, :wu])
         ctx = _ctx16(context)
-        ctx2d, nk = ctx.reshape(-1, ctx.shape[-1]), ctx.shape[1]
-        # below the fork level each network runs its blocks at batch b; the last of them (a Downsample) writes its
-        # output into that network's half of the batch-2b buffer
-        level = twin_from_level()
-        downs = [i for i, m in enumerate(cn.input_blocks) if isinstance(m[0], Downsample)]
-        fork = downs[level - 1] + 1 if 0 < level <= len(downs) else 0
+        # the full-resolution blocks run at batch b per network (measured no faster twinned); the first Downsample
+        # writes each network's output into its half of the batch-2b buffer, and the twin pass takes over from there
+        down = next(i for i, m in enumerate(cn.input_blocks) if isinstance(m[0], Downsample))
         control, hs = [], []
         hc, hu = hint, x
-        for i in range(fork):
-            if i < fork - 1:
+        for i in range(down + 1):
+            if i < down:
                 hc = cn.input_blocks[i](hc, emb_c, ctx)
                 hu = un.input_blocks[i](hu, emb_u, ctx)
             else:
-                dc, du = cn.input_blocks[i][0], un.input_blocks[i][0]
                 xc, xu = pixel_major(hc), pixel_major(hu)
-                h16 = torch.empty((2 * b, xc.shape[1] // 2, xc.shape[2] // 2, dc.out_channels), device=x.device,
-                                  dtype=torch.float16)
-                dc.run(xc, out=h16[:b])
-                du.run(xu, out=h16[b:])
-                hc, hu = nchw_view(h16[:b]), nchw_view(h16[b:])
+                h16 = torch.empty((2 * b, xc.shape[1] // 2, xc.shape[2] // 2, cn.input_blocks[i][0].out_channels),
+                                  device=x.device, dtype=torch.float16)
+                cn.input_blocks[i][0].run(xc, out=h16[:b])
+                un.input_blocks[i][0].run(xu, out=h16[b:])
+                h = nchw_view(h16)
+                hc, hu = h[:b], h[b:]
             control.append(cn._zero_conv(cn.zero_convs[i], hc))
             hs.append(hu)
-        start = fork
-        if fork == 0:
-            ca, cu = cn.input_blocks[0][0], un.input_blocks[0][0]
-            c_pad = (ca.in_channels + 7) // 8 * 8
-            xin = torch.empty((2 * b, x.shape[2], x.shape[3], c_pad), device=x.device, dtype=torch.float16)
-            ops.nchw_to_nhwc_f16(hint.float().contiguous(), c_pad, out=xin[:b])
-            ops.nchw_to_nhwc_f16(x.float().contiguous(), c_pad, out=xin[b:])
-            pad = c_pad if c_pad != ca.in_channels else None
-            h16 = ops.gemm(xin, ca.kernel_weight(pad_in=pad), ksize=3, bias=prepare.bias_f32(ca.bias),
-                           hi={"w": cu.kernel_weight(pad_in=pad), "bias": prepare.bias_f32(cu.bias)})
-            control.append(cn._zero_conv(cn.zero_convs[0], nchw_view(h16[:b])))
-            hs.append(nchw_view(h16[b:]))
-            start = 1
-
-        def twin_block(sa, sb, h16):
-            for la, lb in zip(sa, sb):
-                if isinstance(la, ResBlock):
-                    h16 = la.forward_twin(lb, h16, emb_c, emb_u)
-                elif isinstance(la, SpatialTransformer):
-                    h16 = la.forward_twin(lb, h16, ctx2d, nk)
-                else:
-                    h16 = la.run(h16, other=lb)
-            return h16
-
-        for i in range(start, len(cn.input_blocks)):
-            h16 = twin_block(cn.input_blocks[i], un.input_blocks[i], h16)
-            control.append(cn._zero_conv(cn.zero_convs[i], nchw_view(h16[:b])))
-            hs.append(nchw_view(h16[b:]))
-        h16 = twin_block(cn.middle_block, un.middle_block, h16)
-        control.append(cn._zero_conv(cn.middle_block_out, nchw_view(h16[:b])))
-        return control, nchw_view(h16[b:]), hs, emb_u, ctx
+        for i in range(down + 1, len(cn.input_blocks)):
+            h = cn.input_blocks[i](h, emb_c, ctx, other=un.input_blocks[i], emb_other=emb_u)
+            control.append(cn._zero_conv(cn.zero_convs[i], h[:b]))
+            hs.append(h[b:])
+        h = cn.middle_block(h, emb_c, ctx, other=un.middle_block, emb_other=emb_u)
+        control.append(cn._zero_conv(cn.middle_block_out, h[:b]))
+        return control, h[b:], hs, emb_u, ctx
 
     def control_and_unet(self, x, hint, t, cond_txt, control_of):
         """apply_model's body for one ControlNet pass: the twin pass when twin_enabled(), else the ControlNet then the

@@ -8,6 +8,8 @@ Kernel sequence of one SpatialTransformer (reference :321-340 and :271-275), all
       layernorm -> gemm q ; gemm [k|v](context) -> attention -> gemm to_out (+bias +residual) ->
       layernorm -> gemm GEGLU (value*gelu(gate) in the epilogue) -> gemm ff.net.2 (+bias +residual)
     -> gemm proj_out (+bias + x_in)
+Each layer has one body.  Its optional `other`, the same layer of a second network, turns every launch into a grouped
+one over the two halves of the batch (the twin pass of cldm/cldm.py); the attention launch covers the whole batch.
 """
 from inspect import isfunction
 
@@ -142,86 +144,74 @@ class CrossAttention(nn.Module):
             return hit[1], hit[2]
         return None
 
-    def run_twin(self, other, x2d, batch, nq, ctx2d=None, nk=None, residual=None):
-        """run() of this layer on the lower half of the batch and of `other` (the same layer of a second network) on
-        the upper half: grouped projections, one batch-`batch` attention launch.  Cross-attention reads both layers'
-        K / V^T of the (shared) context from one buffer pair, the one ControlLDM.prepare_context filled, or from
-        projections computed here."""
-        inner = self.to_q.out_features
-        h, d = self.heads, inner // self.heads
-        dev = x2d.device
-        if ctx2d is None:
-            nk = nq
-            nk_pad = (nk + 7) // 8 * 8
-            q = torch.empty((batch * nq, inner), device=dev, dtype=torch.float16)
-            k = torch.empty_like(q)
-            vt = torch.empty((batch, h, d, nk_pad), device=dev, dtype=torch.float16)
-            lins = [self.to_q, self.to_k, self.to_v]
-            ops.gemm(x2d, self._cat_weight("qkv", lins), seg_outs=[q, k, vt], seg_width=inner, transposed=(0, 0, 1),
-                     rows_per_img=nk, head_dim=d, tok_pad=nk_pad,
-                     hi={"w": other._cat_weight("qkv", [other.to_q, other.to_k, other.to_v])})
-        else:
-            half = batch // 2
-            nk_pad = (nk + 7) // 8 * 8
-            q = ops.gemm(x2d, self._q_weight(), hi={"w": other._q_weight()})
-            mine, theirs, shared = self._kv_hit(ctx2d, half, nk), other._kv_hit(ctx2d, half, nk), self.__dict__.get("_kv_twin")
-            if mine is not None and theirs is not None and shared is not None and \
-                    mine[0].data_ptr() == shared[0].data_ptr() and theirs[0].data_ptr() == shared[0][half * nk:].data_ptr():
-                k, vt = shared
-            else:
-                k = torch.empty((batch * nk, inner), device=dev, dtype=torch.float16)
-                vt = ops.zeros((batch, h, d, nk_pad), dev)
-                for m, lo in ((self, True), (other, False)):
-                    rows, imgs = slice(0, half * nk) if lo else slice(half * nk, None), slice(0, half) if lo else slice(half, None)
-                    ops.gemm(ctx2d, m._cat_weight("kv", [m.to_k, m.to_v]), seg_outs=[k[rows], vt[imgs]], seg_width=inner,
-                             transposed=(0, 1, 0), rows_per_img=nk, head_dim=d, tok_pad=nk_pad)
-        o = ops.attention(q, k, vt, batch, h, nq, nk, d)
-        return ops.gemm(o, self._out_weight(), bias=prepare.bias_f32(self.to_out[0].bias), residual=residual,
-                        hi={"w": other._out_weight(), "bias": prepare.bias_f32(other.to_out[0].bias)})
-
     def _q_weight(self):
         return self._prep.get(("q", prepare.lora_key(self.to_q)), prepare.linear_params(self.to_q),
                               lambda: prepare.effective_linear_weight(self.to_q))
 
-    def run(self, x2d, batch, nq, ctx2d=None, nk=None, residual=None):
-        """x2d fp16 [batch*nq, C]; ctx2d fp16 [batch*nk, Cctx] or None (self-attention). Returns to_out(attn) (+residual)."""
+    def _context_kv(self, ctx2d, batch, nk, other=None):
+        """K [batch*nk, inner] and V^T [batch, heads, d, nk_pad] of the context: the buffers project_context filled when
+        they are this context's, else projections into new buffers.  With `other` (the same layer of a second network)
+        ctx2d holds batch/2 images' tokens; the lower half of K / V^T is this layer's projection of them, the upper half
+        other's, and the buffers to re-use are the pair's one `_kv_twin` (ControlLDM.prepare_context)."""
+        layers = (self,) if other is None else (self, other)
+        per = batch // len(layers)
+        if other is None:
+            hit = self._kv_hit(ctx2d, batch, nk)
+        else:
+            hit, mine, theirs = self.__dict__.get("_kv_twin"), self._kv_hit(ctx2d, per, nk), other._kv_hit(ctx2d, per, nk)
+            if hit is None or mine is None or theirs is None or mine[0].data_ptr() != hit[0].data_ptr() or \
+                    theirs[0].data_ptr() != hit[0][per * nk:].data_ptr():
+                hit = None
+        if hit is not None:
+            return hit
         inner = self.to_q.out_features
         h, d = self.heads, inner // self.heads
-        dev = x2d.device
+        nk_pad = (nk + 7) // 8 * 8
+        dev = ctx2d.device
+        k = torch.empty((batch * nk, inner), device=dev, dtype=torch.float16)
+        # the key padding columns (77 -> 80) are never written by the projection, and ops.attention never reads
+        # them: its V^T tensor map ends at key nk, so keys >= nk load as zeros.  The zero fill is not needed for
+        # correctness.
+        vt = ops.zeros((batch, h, d, nk_pad), dev) if nk_pad != nk else torch.empty((batch, h, d, nk_pad), device=dev, dtype=torch.float16)
+        for i, m in enumerate(layers):
+            rows, imgs = slice(i * per * nk, (i + 1) * per * nk), slice(i * per, (i + 1) * per)
+            ops.gemm(ctx2d, m._cat_weight("kv", [m.to_k, m.to_v]), seg_outs=[k[rows], vt[imgs]], seg_width=inner,
+                     transposed=(0, 1, 0), rows_per_img=nk, head_dim=d, tok_pad=nk_pad)
+        return k, vt
+
+    def run(self, x2d, batch, nq, ctx2d=None, nk=None, residual=None, other=None, **finish_kw):
+        """x2d fp16 [batch*nq, C]; ctx2d fp16 [batch*nk, Cctx] or None (self-attention). Returns to_out(attn) (+residual).
+        other: the same layer of a second network, applied to the upper half of the batch in the same launches (one
+        attention launch over the whole batch); both halves attend the same context, so ctx2d then holds batch/2
+        images' tokens.  finish_kw: handed on to _finish."""
+        inner = self.to_q.out_features
+        h, d = self.heads, inner // self.heads
         if ctx2d is None:
             nk = nq
             nk_pad = (nk + 7) // 8 * 8
-            q = torch.empty((batch * nq, inner), device=dev, dtype=torch.float16)
+            q = torch.empty((batch * nq, inner), device=x2d.device, dtype=torch.float16)
             k = torch.empty_like(q)
-            vt = torch.empty((batch, h, d, nk_pad), device=dev, dtype=torch.float16)
+            vt = torch.empty((batch, h, d, nk_pad), device=x2d.device, dtype=torch.float16)
             w = self._cat_weight("qkv", [self.to_q, self.to_k, self.to_v])
+            hi = None if other is None else {"w": other._cat_weight("qkv", [other.to_q, other.to_k, other.to_v])}
             ops.gemm(x2d, w, seg_outs=[q, k, vt], seg_width=inner, transposed=(0, 0, 1), rows_per_img=nk, head_dim=d,
-                     tok_pad=nk_pad)
+                     tok_pad=nk_pad, hi=hi)
         else:
-            nk_pad = (nk + 7) // 8 * 8
-            q = ops.gemm(x2d, self._q_weight())
-            hit = self._kv_hit(ctx2d, batch, nk)
-            if hit is not None:
-                return self._finish(ops.attention(q, hit[0], hit[1], batch, h, nq, nk, d), q, batch, nq, residual)
-            k = torch.empty((batch * nk, inner), device=dev, dtype=torch.float16)
-            # the key padding columns (77 -> 80) are never written by the projection, and ops.attention never reads
-            # them: its V^T tensor map ends at key nk, so keys >= nk load as zeros.  The zero fill is not needed for
-            # correctness.
-            vt = ops.zeros((batch, h, d, nk_pad), dev) if nk_pad != nk else torch.empty((batch, h, d, nk_pad), device=dev, dtype=torch.float16)
-            w = self._cat_weight("kv", [self.to_k, self.to_v])
-            ops.gemm(ctx2d, w, seg_outs=[k, vt], seg_width=inner, transposed=(0, 1, 0), rows_per_img=nk, head_dim=d,
-                     tok_pad=nk_pad)
-        return self._finish(ops.attention(q, k, vt, batch, h, nq, nk, d), q, batch, nq, residual)
+            q = ops.gemm(x2d, self._q_weight(), hi=None if other is None else {"w": other._q_weight()})
+            k, vt = self._context_kv(ctx2d, batch, nk, other)
+        return self._finish(ops.attention(q, k, vt, batch, h, nq, nk, d), q, batch, nq, residual, other, **finish_kw)
 
     def _out_weight(self):
         lin = self.to_out[0]
         return self._prep.get(("o", prepare.lora_key(lin)), prepare.linear_params(lin),
                               lambda: prepare.effective_linear_weight(lin))
 
-    def _finish(self, o, q, batch, nq, residual):
+    def _finish(self, o, q, batch, nq, residual, other=None):
         """to_out(attention output) (+ residual); `q` is handed on for variants that attend a second key set
         (ldm/modules/attention_ip.py)."""
-        return ops.gemm(o, self._out_weight(), bias=prepare.bias_f32(self.to_out[0].bias), residual=residual)
+        w, bias = self._out_weight(), prepare.bias_f32(self.to_out[0].bias)
+        hi = None if other is None else {"w": other._out_weight(), "bias": prepare.bias_f32(other.to_out[0].bias)}
+        return ops.gemm(o, w, bias=bias, residual=residual, hi=hi)
 
     def forward(self, x, context=None, mask=None):
         if mask is not None:
@@ -260,18 +250,15 @@ class BasicTransformerBlock(nn.Module):
                                        "beta_hi": prepare.bias_f32(prepare.effective(other).bias)}
         return ops.layernorm(x2d, prepare.bias_f32(norm.weight), prepare.bias_f32(norm.bias), norm.eps, **hi)
 
-    def run_twin(self, other, x2d, batch, n, ctx2d, nk):
-        """run() of this block on the lower half of the batch and of `other` on the upper half (self-attention blocks)"""
-        x2d = self.attn1.run_twin(other.attn1, self._ln(self.norm1, x2d, other.norm1), batch, n, residual=x2d)
-        x2d = self.attn2.run_twin(other.attn2, self._ln(self.norm2, x2d, other.norm2), batch, n, ctx2d, nk, residual=x2d)
-        return self.ff.run(self._ln(self.norm3, x2d, other.norm3), residual=x2d, other=other.ff)
-
-    def run(self, x2d, batch, n, ctx2d, nk, out=None):
-        """x2d fp16 [batch*n, dim] -> same shape (reference _forward :271-275); `out`: optional destination buffer."""
+    def run(self, x2d, batch, n, ctx2d, nk, out=None, other=None, **attn2_kw):
+        """x2d fp16 [batch*n, dim] -> same shape (reference _forward :271-275); `out`: optional destination buffer.
+        other: the same block of a second network, applied to the upper half of the rows in the same launches.
+        attn2_kw: further arguments of attn2.run (the IP-Adapter's image tokens)."""
+        o = (None,) * 6 if other is None else (other.norm1, other.norm2, other.norm3, other.attn1, other.attn2, other.ff)
         c1 = (ctx2d, nk) if self.disable_self_attn else (None, None)
-        x2d = self.attn1.run(self._ln(self.norm1, x2d), batch, n, c1[0], c1[1], residual=x2d)
-        x2d = self.attn2.run(self._ln(self.norm2, x2d), batch, n, ctx2d, nk, residual=x2d)
-        return self.ff.run(self._ln(self.norm3, x2d), residual=x2d, out=out)
+        x2d = self.attn1.run(self._ln(self.norm1, x2d, o[0]), batch, n, c1[0], c1[1], residual=x2d, other=o[3])
+        x2d = self.attn2.run(self._ln(self.norm2, x2d, o[1]), batch, n, ctx2d, nk, residual=x2d, other=o[4], **attn2_kw)
+        return self.ff.run(self._ln(self.norm3, x2d, o[2]), residual=x2d, out=out, other=o[5])
 
     def forward(self, x, context=None):
         b, n, _ = x.shape
@@ -310,22 +297,6 @@ class SpatialTransformer(nn.Module):
                                   lambda: prepare.effective_linear_weight(mod))
         return self._prep.get(key, [mod.weight], lambda: prepare.conv_weight(mod.weight))
 
-    def forward_twin(self, other, xp, ctx2d, nk):
-        """This transformer on the lower half of the pixel-major batch `xp` and `other` (the same layer of a second
-        network) on the upper half, one launch per kernel; ctx2d: fp16 [batch/2 * nk, D] context of both halves."""
-        b, h, w, c = xp.shape
-        f32 = prepare.bias_f32
-        gn, ogn = prepare.effective(self.norm), prepare.effective(other.norm)
-        xn = ops.groupnorm(xp, f32(gn.weight), f32(gn.bias), gn.eps, False, groups=gn.num_groups, gamma_hi=f32(ogn.weight),
-                           beta_hi=f32(ogn.bias))
-        y = ops.gemm(xn, self._w("in", self.proj_in), bias=f32(self.proj_in.bias),
-                     hi={"w": other._w("in", other.proj_in), "bias": f32(other.proj_in.bias)})
-        y2d = y.view(b * h * w, -1)
-        for block, oblock in zip(self.transformer_blocks, other.transformer_blocks):
-            y2d = block.run_twin(oblock, y2d, b, h * w, ctx2d, nk)
-        return ops.gemm(y2d.view(b, h, w, -1), self._w("out", self.proj_out), bias=f32(self.proj_out.bias),
-                        residual=xp.view(b * h * w, c), hi={"w": other._w("out", other.proj_out), "bias": f32(other.proj_out.bias)})
-
     def forward_grouped(self, x, context, n_groups, attach):
         """One pass over a batch made of `n_groups` equal slices that use DIFFERENT LoRA / norm sets (multi-LoRA inference,
         cldm/cldm_ctrlora_inference.py:156-178 runs the ControlNet once per set): `attach(self, g)` re-points this module's
@@ -359,19 +330,32 @@ class SpatialTransformer(nn.Module):
                        residual=xp.view(b * h * w, c))
         return nchw_view(out)
 
-    def forward(self, x, context=None):
+    @staticmethod
+    def block_context(ctx):
+        """a transformer block's context entry -> (ctx2d, nk, further attn2.run arguments)"""
+        return (None, None, {}) if ctx is None else (to_f16_rows(ctx), ctx.shape[1], {})
+
+    def forward(self, x, context=None, other=None):
+        """other: the same layer of a second network, applied to the upper half of the batch in the same launches;
+        `context` then holds the images of one half, which both halves attend."""
         xp = pixel_major(x)  # [B, H, W, C]
         b, h, w, c = xp.shape
         if not isinstance(context, list):
             context = [context]
+        f32 = prepare.bias_f32
         gn = prepare.effective(self.norm)
-        xn = ops.groupnorm(xp, prepare.bias_f32(gn.weight), prepare.bias_f32(gn.bias), gn.eps, False, groups=gn.num_groups)
-        y = ops.gemm(xn, self._w("in", self.proj_in), bias=prepare.bias_f32(self.proj_in.bias))
+        ogn = None if other is None else prepare.effective(other.norm)
+        hi = {} if other is None else {"gamma_hi": f32(ogn.weight), "beta_hi": f32(ogn.bias)}
+        xn = ops.groupnorm(xp, f32(gn.weight), f32(gn.bias), gn.eps, False, groups=gn.num_groups, **hi)
+        wi, bias = self._w("in", self.proj_in), f32(self.proj_in.bias)
+        hi = None if other is None else {"w": other._w("in", other.proj_in), "bias": f32(other.proj_in.bias)}
+        y = ops.gemm(xn, wi, bias=bias, hi=hi)
         y2d = y.view(b * h * w, -1)
         for i, block in enumerate(self.transformer_blocks):
-            ctx = context[i] if i < len(context) else context[-1]
-            ctx2d, nk = (None, None) if ctx is None else (to_f16_rows(ctx), ctx.shape[1])
-            y2d = block.run(y2d, b, h * w, ctx2d, nk)
-        out = ops.gemm(y2d.view(b, h, w, -1), self._w("out", self.proj_out), bias=prepare.bias_f32(self.proj_out.bias),
-                       residual=xp.view(b * h * w, c))
+            ctx2d, nk, attn2_kw = self.block_context(context[i] if i < len(context) else context[-1])
+            y2d = block.run(y2d, b, h * w, ctx2d, nk, other=None if other is None else other.transformer_blocks[i],
+                            **attn2_kw)
+        wo, bias = self._w("out", self.proj_out), f32(self.proj_out.bias)
+        hi = None if other is None else {"w": other._w("out", other.proj_out), "bias": f32(other.proj_out.bias)}
+        out = ops.gemm(y2d.view(b, h, w, -1), wo, bias=bias, residual=xp.view(b * h * w, c), hi=hi)
         return nchw_view(out)

@@ -37,16 +37,19 @@ class TimestepBlock(nn.Module):
 
 
 class TimestepEmbedSequential(nn.Sequential, TimestepBlock):
-    """Sequential that routes (x, emb) to TimestepBlocks and (x, context) to SpatialTransformers (reference :73-87)."""
+    """Sequential that routes (x, emb) to TimestepBlocks and (x, context) to SpatialTransformers (reference :73-87).
+    `other` / `emb_other`: the same block of a second network and that network's time embedding; each layer then runs
+    on the lower half of the batch and its partner in `other` on the upper half, in the same launches."""
 
-    def forward(self, x, emb, context=None):
-        for layer in self:
+    def forward(self, x, emb, context=None, other=None, emb_other=None):
+        for i, layer in enumerate(self):
+            pair = {} if other is None else {"other": other[i]}
             if isinstance(layer, TimestepBlock):
-                x = layer(x, emb)
+                x = layer(x, emb, emb_other=emb_other, **pair)
             elif isinstance(layer, SpatialTransformer):
-                x = layer(x, context)
+                x = layer(x, context, **pair)
             else:
-                x = layer(x)
+                x = layer(x, **pair)
         return x
 
 
@@ -122,9 +125,9 @@ class Downsample(nn.Module):
         hi = None if other is None else {"w": other._weight(), "bias": prepare.bias_f32(other.op.bias)}
         return ops.gemm(col, self._weight(), bias=prepare.bias_f32(self.op.bias), out=out, hi=hi)
 
-    def forward(self, x):
+    def forward(self, x, other=None):
         assert x.shape[1] == self.channels
-        return nchw_view(self.run(pixel_major(x)))
+        return nchw_view(self.run(pixel_major(x), other=other))
 
 
 class ResBlock(TimestepBlock):
@@ -182,47 +185,39 @@ class ResBlock(TimestepBlock):
             rowbias = ops.small_linear(raw.float().contiguous(), self.emb_weight(), prepare.bias_f32(lin.bias), silu_in=True)
         return rowbias
 
-    def forward_twin(self, other, xp, emb, emb_other):
-        """This block on the lower half of the pixel-major batch `xp` and `other` (the same block of a second network)
-        on the upper half, one launch per kernel; emb / emb_other: each network's time embedding."""
-        k, o = self._kernel_params(), other._kernel_params()
-        a = ops.groupnorm(xp, k["gn1"][0], k["gn1"][1], k["gn1"][2], True, gamma_hi=o["gn1"][0], beta_hi=o["gn1"][1])
-        hmid = ops.gemm(a, k["w1"], ksize=3, bias=k["b1"], rowbias=self._rowbias(emb),
-                        hi={"w": o["w1"], "bias": o["b1"], "rowbias": other._rowbias(emb_other)})
-        c = ops.groupnorm(hmid, k["gn2"][0], k["gn2"][1], k["gn2"][2], True, gamma_hi=o["gn2"][0], beta_hi=o["gn2"][1])
-        if k["wsk"] is not None:
-            return ops.gemm(c, k["w2"], ksize=3, bias=k["b2"], a2=xp, w2=k["wsk"],
-                            hi={"w": o["w2"], "bias": o["b2"], "w2": o["wsk"]})
-        b, h, w, cin = xp.shape
-        return ops.gemm(c, k["w2"], ksize=3, bias=k["b2"], residual=xp.view(b * h * w, cin), hi={"w": o["w2"], "bias": o["b2"]})
-
     def emb_weight(self):
         lin = self.emb_layers[1]
         return self._prep.get("emb", prepare.linear_params(lin),
                               lambda: prepare.effective_linear_weight(lin).view(lin.out_features, lin.in_features))
 
-    def forward(self, x, emb):
+    def forward(self, x, emb, other=None, emb_other=None):
+        """`other` / `emb_other`: the same block of a second network and that network's time embedding, applied to the
+        upper half of the batch in the same launches."""
         k = self._kernel_params()
+        o = None if other is None else other._kernel_params()
         (g1, b1, eps1), (g2, b2, eps2) = k["gn1"], k["gn2"]
-        if isinstance(x, CatSpec):
+        hi1, hi2 = ({}, {}) if o is None else ({"gamma_hi": o["gn1"][0], "beta_hi": o["gn1"][1]},
+                                               {"gamma_hi": o["gn2"][0], "beta_hi": o["gn2"][1]})
+        if isinstance(x, CatSpec):  # the decoder's concatenated input, read in place
             x1 = pixel_major(x.x1)
-            res = ops.groupnorm(x1, g1, b1, eps1, True,
-                                add1=None if x.add1 is None else pixel_major(x.add1), add1_scale=x.s1,
-                                x2=None if x.x2 is None else pixel_major(x.x2),
-                                add2=None if x.add2 is None else pixel_major(x.add2), add2_scale=x.s2,
-                                want_raw=True)
-            a, xp = res
+            a, xp = ops.groupnorm(x1, g1, b1, eps1, True,
+                                  add1=None if x.add1 is None else pixel_major(x.add1), add1_scale=x.s1,
+                                  x2=None if x.x2 is None else pixel_major(x.x2),
+                                  add2=None if x.add2 is None else pixel_major(x.add2), add2_scale=x.s2,
+                                  want_raw=True, **hi1)
         else:
             xp = pixel_major(x)
-            a = ops.groupnorm(xp, g1, b1, eps1, True)
+            a = ops.groupnorm(xp, g1, b1, eps1, True, **hi1)
         b, h, w, cin = xp.shape
         assert cin == self.channels, (cin, self.channels)
-        hmid = ops.gemm(a, k["w1"], ksize=3, bias=k["b1"], rowbias=self._rowbias(emb))
-        c = ops.groupnorm(hmid, g2, b2, eps2, True)
+        hmid = ops.gemm(a, k["w1"], ksize=3, bias=k["b1"], rowbias=self._rowbias(emb),
+                        hi=None if o is None else {"w": o["w1"], "bias": o["b1"], "rowbias": other._rowbias(emb_other)})
+        c = ops.groupnorm(hmid, g2, b2, eps2, True, **hi2)
+        hi = None if o is None else {"w": o["w2"], "bias": o["b2"], "w2": o["wsk"]}
         if k["wsk"] is not None:
-            out = ops.gemm(c, k["w2"], ksize=3, bias=k["b2"], a2=xp, w2=k["wsk"])
+            out = ops.gemm(c, k["w2"], ksize=3, bias=k["b2"], a2=xp, w2=k["wsk"], hi=hi)
         else:
-            out = ops.gemm(c, k["w2"], ksize=3, bias=k["b2"], residual=xp.view(b * h * w, cin))
+            out = ops.gemm(c, k["w2"], ksize=3, bias=k["b2"], residual=xp.view(b * h * w, cin), hi=hi)
         return nchw_view(out)
 
 

@@ -148,19 +148,21 @@ def gemm(a, w, *, ksize=1, bias=None, rowbias=None, rows_per_img=0, rowbias_ld=0
     """
     _require_cuda(a, w)
     assert a.dtype == torch.float16 and w.dtype == torch.float16 and w.is_contiguous()
-    if hi is not None:
-        return _gemm_grouped(a, w, hi, dict(ksize=ksize, bias=bias, rowbias=rowbias, rows_per_img=rows_per_img,
-                                            rowbias_ld=rowbias_ld, residual=residual, out_scale=out_scale, a2=a2, w2=w2,
-                                            geglu=geglu, out=out, out_f32=out_f32, seg_outs=seg_outs, seg_width=seg_width,
-                                            transposed=transposed, head_dim=head_dim, tok_pad=tok_pad, block_n=block_n,
-                                            split_k=split_k))
-    b, h, wd, c, ld = _as_bhwc(a)
     n_rows = w.shape[0]
     n = n_rows // 2 if geglu else n_rows
+    if out is None and seg_outs is None:
+        out = torch.empty(a.shape[:-1] + (n,), device=a.device, dtype=torch.float32 if out_f32 else torch.float16)
+    a4, out4 = a, out
+    if hi is not None:
+        assert a.shape[0] % 2 == 0
+        if a.dim() == 2:  # the two halves of the rows are two images
+            a4 = a.view(2, 1, a.shape[0] // 2, a.shape[1])
+            out4 = None if out is None else out.view(a4.shape[:3] + (out.shape[-1],))
+    b, h, wd, c, ld = _as_bhwc(a4)
     assert w.numel() == n_rows * ksize * ksize * c, (w.shape, ksize, c)
     M = b * h * wd
     args = GemmArgs()
-    args.a, args.a_b, args.a_h, args.a_w, args.a_c, args.a_ld = _ptr(a), b, h, wd, c, ld
+    args.a, args.a_b, args.a_h, args.a_w, args.a_c, args.a_ld = _ptr(a4), b, h, wd, c, ld
     args.w, args.kh, args.kw, args.pad = _ptr(w), ksize, ksize, (ksize - 1) // 2
     if a2 is not None:
         b2, h2, w2d, c2, ld2 = _as_bhwc(a2)
@@ -168,19 +170,15 @@ def gemm(a, w, *, ksize=1, bias=None, rowbias=None, rows_per_img=0, rowbias_ld=0
         args.a2, args.a2_c, args.a2_ld, args.w2 = _ptr(a2), c2, ld2, _ptr(w2)
     args.n, args.block_n, args.geglu = n, block_n, int(geglu)
     if seg_outs is not None:
-        outs = list(seg_outs)
         ldc = seg_width
-        for i, o in enumerate(outs):
+        for i, o in enumerate(seg_outs):
             args.out[i] = o.data_ptr()
             args.transposed[i] = int(transposed[i])
-        ret = outs
+        ret = list(seg_outs)
     else:
-        if out is None:
-            shape = (M, n) if a.dim() == 2 else (b, h, wd, n)
-            out = torch.empty(shape, device=a.device, dtype=torch.float32 if out_f32 else torch.float16)
-        assert out.stride(-1) == 1
-        ldc = out.stride(-2)
-        args.out[0] = out.data_ptr()
+        assert out4.stride(-1) == 1
+        ldc = out4.stride(-2)
+        args.out[0] = out4.data_ptr()
         ret = out
     args.seg_width, args.ldc, args.out_f32 = seg_width, ldc, int(out_f32)
     if bias is not None:
@@ -200,72 +198,23 @@ def gemm(a, w, *, ksize=1, bias=None, rowbias=None, rows_per_img=0, rowbias_ld=0
     if dup_out is not None:
         args.dup_out, args.dup_ld = dup_out.data_ptr(), dup_out.stride(0)
     args.force_single_cta = int(single_cta)
+    if hi is not None:
+        if hi.get("rowbias") is not None:  # the kernel reads both halves' row terms with the lower half's row stride
+            assert rowbias is not None and hi["rowbias"].stride(0) == rowbias.stride(0) and \
+                hi["rowbias"].stride(-1) == 1, "the two halves' row terms need one row stride"
+        args.group_b, args.w_hi, args.w2_hi = b // 2, _ptr(hi["w"]), _ptr(hi.get("w2"))
+        args.bias_hi, args.rowbias_hi = _ptr(hi.get("bias")), _ptr(hi.get("rowbias"))
     lib = _lib.load()
-    fn = lib.ctrlora_gemm_f16_simt if simt else lib.ctrlora_gemm_f16
-    if _GROUP is not None:
-        group_b, g = _GROUP
-        args.group_b, args.w_hi, args.w2_hi = group_b, _ptr(g["w"]), _ptr(g.get("w2"))
-        args.bias_hi, args.rowbias_hi = _ptr(g.get("bias")), _ptr(g.get("rowbias"))
-        rc = fn(C.addressof(args), _sp())
-        if rc == _lib.STATUS_UNSUPPORTED:
-            return None  # a tile would straddle the halves: the caller launches them one by one
-        check(rc, "ctrlora_gemm_f16 (grouped)")
-        _count()
-        if _GEMM_RECORD is not None:
-            ktot = ksize * ksize * c + (args.a2_c if a2 is not None else 0)
-            _GEMM_RECORD.append((args, 2.0 * M * n_rows * ktot,
-                                 (a, w, a2, w2, bias, rowbias, residual, out, seg_outs, dup_out, ws, cnt, g)))
+    shape = {"B": b, "H": h, "W": wd, "C": c, "N": n_rows, "ksize": ksize, "geglu": int(geglu),
+             "c2": int(args.a2_c) if a2 is not None else 0, "segs": seg_width, "res": int(residual is not None)}
+    keep = (a, w, a2, w2, bias, rowbias, residual, out, seg_outs, dup_out, ws, cnt, hi)
+    if _launch_gemm(lib.ctrlora_gemm_f16_simt if simt else lib.ctrlora_gemm_f16, args, simt, shape, keep):
         return ret
-    _count()
-    if _GEMM_RECORD is not None and not simt:
-        ktot = ksize * ksize * c + (args.a2_c if a2 is not None else 0)
-        _GEMM_RECORD.append((args, 2.0 * M * n_rows * ktot,
-                             (a, w, a2, w2, bias, rowbias, residual, out, seg_outs, dup_out, ws, cnt)))
-    if _GEMM_PROFILE is not None and not simt:
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        check(fn(C.addressof(args), _sp()), "ctrlora_gemm_f16")
-        e1.record()
-        ktot = ksize * ksize * c + (args.a2_c if a2 is not None else 0)
-        _GEMM_PROFILE.append((2.0 * M * n_rows * ktot, e0, e1))
-        if _GEMM_SHAPES is not None:
-            _GEMM_SHAPES.append({"B": b, "H": h, "W": wd, "C": c, "N": n_rows, "ksize": ksize, "geglu": int(geglu),
-                                 "c2": int(args.a2_c) if a2 is not None else 0, "segs": seg_width,
-                                 "res": int(residual is not None)})
-        return ret
-    check(fn(C.addressof(args), _sp()), "ctrlora_gemm_f16")
-    return ret
-
-
-_GROUP = None  # (group_b, upper half's operands) while _gemm_grouped issues its launch
-
-
-def _gemm_grouped(a, w, hi, kw):
-    """One launch over both halves of the batch (see gemm's `hi`), or one launch per half where a tile would straddle
-    them.  An [M, K] `a` is viewed as two images of M/2 rows."""
-    global _GROUP
-    assert a.shape[0] % 2 == 0
+    # a tile would straddle the halves: one plain launch per half, over the rows of the row-indexed operands and the
+    # images of the V^T-layout segments
     half = a.shape[0] // 2
-    a4 = a.view(2, 1, half, a.shape[1]) if a.dim() == 2 else a
-    out = kw.pop("out")
-    if out is None and kw["seg_outs"] is None:
-        out = torch.empty(a.shape[:-1] + (w.shape[0] // 2 if kw["geglu"] else w.shape[0],), device=a.device,
-                          dtype=torch.float32 if kw["out_f32"] else torch.float16)
-    out4 = out.view(a4.shape[:3] + (out.shape[-1],)) if out is not None and a.dim() == 2 else out
-    g = {k: v for k, v in hi.items() if v is not None}
-    if "rowbias" in g:  # the kernel reads both halves' row terms with the lower half's row stride
-        assert kw["rowbias"] is not None and g["rowbias"].stride(0) == kw["rowbias"].stride(0) and \
-            g["rowbias"].stride(-1) == 1, "the two halves' row terms need one row stride"
-    _GROUP = (a4.shape[0] // 2, g)
-    try:
-        ret = gemm(a4, w, out=out4, **kw)
-    finally:
-        _GROUP = None
-    if ret is not None:
-        return kw["seg_outs"] if kw["seg_outs"] is not None else out
-    # two plain launches: rows of the row-indexed operands, images of the V^T-layout segments
     rows = half if a.dim() == 2 else half * a.shape[1] * a.shape[2]
-    imgs = rows // (kw["rows_per_img"] or rows)
+    imgs = rows // (rows_per_img or rows)
 
     def cut(t, lo, by_image=False):
         if t is None:
@@ -274,14 +223,37 @@ def _gemm_grouped(a, w, hi, kw):
         return t[:n] if lo else t[n:]
 
     for lo in (True, False):
-        k = dict(kw)
-        k["residual"], k["a2"] = cut(kw["residual"], lo), cut(kw["a2"], lo)
-        if kw["seg_outs"] is not None:
-            k["seg_outs"] = [cut(o, lo, by_image=bool(t)) for o, t in zip(kw["seg_outs"], kw["transposed"])]
-        if not lo:
-            k["bias"], k["rowbias"], k["w2"] = hi.get("bias"), hi.get("rowbias"), hi.get("w2")
-        gemm(cut(a, lo), w if lo else hi["w"], out=cut(out, lo), **k)
-    return kw["seg_outs"] if kw["seg_outs"] is not None else out
+        segs = None if seg_outs is None else [cut(o, lo, by_image=bool(t)) for o, t in zip(seg_outs, transposed)]
+        gemm(cut(a, lo), w if lo else hi["w"], ksize=ksize, bias=bias if lo else hi.get("bias"),
+             rowbias=rowbias if lo else hi.get("rowbias"), rows_per_img=rows_per_img, rowbias_ld=rowbias_ld,
+             residual=cut(residual, lo), out_scale=out_scale, a2=cut(a2, lo), w2=w2 if lo else hi.get("w2"),
+             geglu=geglu, out=cut(out, lo), out_f32=out_f32, seg_outs=segs, seg_width=seg_width, transposed=transposed,
+             head_dim=head_dim, tok_pad=tok_pad, block_n=block_n, split_k=split_k)
+    return ret
+
+
+def _launch_gemm(fn, args, simt, shape, keep):
+    """One ctrlora_gemm_f16 / ctrlora_gemm_f16_simt launch with its bookkeeping: the launch count, and for the wgmma
+    kernel the replay_gemms record and the profile_gemm timing.  Returns False when a grouped launch is refused as
+    UNSUPPORTED (nothing was launched); raises on any other error."""
+    flops = 2.0 * shape["B"] * shape["H"] * shape["W"] * shape["N"] * (shape["ksize"] ** 2 * shape["C"] + shape["c2"])
+    timed = _GEMM_PROFILE is not None and not simt
+    if timed:
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+    rc = fn(C.addressof(args), _sp())
+    if rc == _lib.STATUS_UNSUPPORTED and args.group_b:
+        return False
+    check(rc, "ctrlora_gemm_f16")
+    _count()
+    if _GEMM_RECORD is not None and not simt:
+        _GEMM_RECORD.append((args, flops, keep))
+    if timed:
+        e1.record()
+        _GEMM_PROFILE.append((flops, e0, e1))
+        if _GEMM_SHAPES is not None:
+            _GEMM_SHAPES.append(shape)
+    return True
 
 
 def _dp(t):
@@ -366,16 +338,32 @@ def _gn_partial_buffers(device):
     return _GN_PARTIAL[key]
 
 
-def groupnorm(x1, gamma, beta, eps, silu, *, add1=None, add1_scale=1.0, x2=None, add2=None, add2_scale=1.0,
-              groups=32, want_raw=False, stats_ws=None, want_stats=False, out=None, gamma_hi=None, beta_hi=None):
-    """GroupNorm(+SiLU) over [x1 (+s1*add1) | x2 (+s2*add2)], pixel-major fp16 [B,H,W,C*]; returns y (and raw concat).
-    gamma_hi / beta_hi: the affine parameters of the upper half of the batch (two networks' layers in one launch)."""
-    _require_cuda(x1, x2, add1, add2)
+def _gn_args(x1, gamma, beta, eps, silu, add1, add1_scale, x2, add2, add2_scale, groups):
+    """GroupNormArgs of a groupnorm / groupnorm_bwd call: the source description and the partial-statistics scratch
+    (the forward's and the backward's are one buffer: bit-reproducible dx); the caller sets the statistics workspace"""
     b, h, w, c1, ld1 = _as_bhwc(x1)
     c2, ld2 = 0, 0
     if x2 is not None:
         b2, h2, w2, c2, ld2 = _as_bhwc(x2)
         assert (b2, h2, w2) == (b, h, w)
+    a = _lib.GroupNormArgs()
+    a.x1, a.add1, a.add1_scale, a.c1, a.ld1 = _dp(x1), _dp(add1), float(add1_scale), c1, ld1
+    a.x2, a.add2, a.add2_scale, a.c2, a.ld2 = _dp(x2), _dp(add2), float(add2_scale), c2, ld2
+    a.batch, a.hw, a.groups = b, h * w, groups
+    a.gamma, a.beta, a.eps, a.silu = _dp(gamma), _dp(beta), float(eps), int(silu)
+    if not torch.cuda.is_current_stream_capturing() or x1.device.index in _GN_PARTIAL or torch.cuda.current_device() in _GN_PARTIAL:
+        pws, pcnt = _gn_partial_buffers(x1.device)  # never first allocated inside a capture
+        a.partial_ws, a.partial_ws_floats = _dp(pws), GN_PARTIAL_FLOATS
+        a.partial_counters, a.partial_counters_len = _dp(pcnt), GN_PARTIAL_COUNTERS
+    return a, (b, h, w, c1, c2)
+
+
+def groupnorm(x1, gamma, beta, eps, silu, *, add1=None, add1_scale=1.0, x2=None, add2=None, add2_scale=1.0,
+              groups=32, want_raw=False, stats_ws=None, want_stats=False, out=None, gamma_hi=None, beta_hi=None):
+    """GroupNorm(+SiLU) over [x1 (+s1*add1) | x2 (+s2*add2)], pixel-major fp16 [B,H,W,C*]; returns y (and raw concat).
+    gamma_hi / beta_hi: the affine parameters of the upper half of the batch (two networks' layers in one launch)."""
+    _require_cuda(x1, x2, add1, add2)
+    a, (b, h, w, c1, c2) = _gn_args(x1, gamma, beta, eps, silu, add1, add1_scale, x2, add2, add2_scale, groups)
     for ad, ref in ((add1, x1), (add2, x2)):
         if ad is not None:
             assert ad.shape == ref.shape and ad.stride() == ref.stride() and ad.dtype == torch.float16
@@ -386,21 +374,12 @@ def groupnorm(x1, gamma, beta, eps, silu, *, add1=None, add1_scale=1.0, x2=None,
     prezeroed = 0
     if stats_ws is None:
         stats_ws, prezeroed = _stats_take(x1.device, b * groups * 2)
-    a = _lib.GroupNormArgs()
-    a.stats_prezeroed = prezeroed
-    a.x1, a.add1, a.add1_scale, a.c1, a.ld1 = _dp(x1), _dp(add1), float(add1_scale), c1, ld1
-    a.x2, a.add2, a.add2_scale, a.c2, a.ld2 = _dp(x2), _dp(add2), float(add2_scale), c2, ld2
-    a.batch, a.hw, a.groups = b, h * w, groups
+    a.stats_ws, a.stats_prezeroed = _dp(stats_ws), prezeroed
     assert gamma.dtype == torch.float32 and beta.dtype == torch.float32 and gamma.numel() == ctot
-    a.gamma, a.beta, a.eps, a.silu = _dp(gamma), _dp(beta), float(eps), int(silu)
     if gamma_hi is not None:
         assert b % 2 == 0 and gamma_hi.numel() == ctot and beta_hi.numel() == ctot
         a.gamma_hi, a.beta_hi, a.group_b = _dp(gamma_hi), _dp(beta_hi), b // 2
-    a.y, a.raw_out, a.stats_ws = _dp(y), _dp(raw), _dp(stats_ws)
-    if not torch.cuda.is_current_stream_capturing() or x1.device.index in _GN_PARTIAL or torch.cuda.current_device() in _GN_PARTIAL:
-        pws, pcnt = _gn_partial_buffers(x1.device)  # (never first allocated inside a capture)
-        a.partial_ws, a.partial_ws_floats = _dp(pws), GN_PARTIAL_FLOATS
-        a.partial_counters, a.partial_counters_len = _dp(pcnt), GN_PARTIAL_COUNTERS
+    a.y, a.raw_out = _dp(y), _dp(raw)
     _count(2)
     check(_lib.load().ctrlora_groupnorm_f16(C.addressof(a), _sp()), "ctrlora_groupnorm_f16")
     if want_stats:
@@ -703,20 +682,6 @@ def wgrad_tn(a, b, out=None, alpha=1.0, beta=0.0):
 
 
 # ------------------------------------------------------------------------------------------------ training kernels
-def _gn_args(x1, gamma, beta, eps, silu, add1, add1_scale, x2, add2, add2_scale, groups, stats_ws):
-    b, h, w, c1, ld1 = _as_bhwc(x1)
-    c2, ld2 = 0, 0
-    if x2 is not None:
-        _, _, _, c2, ld2 = _as_bhwc(x2)
-    a = _lib.GroupNormArgs()
-    a.x1, a.add1, a.add1_scale, a.c1, a.ld1 = _dp(x1), _dp(add1), float(add1_scale), c1, ld1
-    a.x2, a.add2, a.add2_scale, a.c2, a.ld2 = _dp(x2), _dp(add2), float(add2_scale), c2, ld2
-    a.batch, a.hw, a.groups = b, h * w, groups
-    a.gamma, a.beta, a.eps, a.silu = _dp(gamma), _dp(beta), float(eps), int(silu)
-    a.stats_ws = _dp(stats_ws)
-    return a, (b, h, w, c1, c2)
-
-
 def groupnorm_bwd(dy, fwd_stats, x1, gamma, beta, eps, silu, *, add1=None, add1_scale=1.0, x2=None, add2=None,
                   add2_scale=1.0, groups=32, want_dx2=False, dx2_scale=1.0, dgamma=None, dbeta=None, res=None, dx1_scale=1.0):
     """Backward of ops.groupnorm (same source description).  Returns dx1 (and dx2 scaled by dx2_scale if want_dx2);
@@ -724,12 +689,8 @@ def groupnorm_bwd(dy, fwd_stats, x1, gamma, beta, eps, silu, *, add1=None, add1_
     _require_cuda(dy, x1)
     assert dy.dtype == torch.float16 and dy.is_contiguous()
     ws, prezeroed = _stats_take(dy.device, fwd_stats.numel())
-    a, (b, h, w, c1, c2) = _gn_args(x1, gamma, beta, eps, silu, add1, add1_scale, x2, add2, add2_scale, groups, ws)
-    a.stats_prezeroed = prezeroed
-    if not torch.cuda.is_current_stream_capturing() or dy.device.index in _GN_PARTIAL or torch.cuda.current_device() in _GN_PARTIAL:
-        pws, pcnt = _gn_partial_buffers(dy.device)  # the forward's scratch: bit-reproducible dx (never first allocated in a capture)
-        a.partial_ws, a.partial_ws_floats = _dp(pws), GN_PARTIAL_FLOATS
-        a.partial_counters, a.partial_counters_len = _dp(pcnt), GN_PARTIAL_COUNTERS
+    a, (b, h, w, c1, c2) = _gn_args(x1, gamma, beta, eps, silu, add1, add1_scale, x2, add2, add2_scale, groups)
+    a.stats_ws, a.stats_prezeroed = _dp(ws), prezeroed
     dx1 = torch.empty((b, h, w, c1), device=dy.device, dtype=torch.float16)
     dx2 = torch.empty((b, h, w, c2), device=dy.device, dtype=torch.float16) if (want_dx2 and c2) else None
     _count(2)
