@@ -123,6 +123,10 @@ _ARGTYPES = {
     "ctrlora_clip_patch_gather": [_P, _I, _P, _I, _I, _I, _I, _I, _P],
     "ctrlora_clip_vision_embed": [_P, _L, _P, _P, _P, _I, _I, _I, _P],
     "ctrlora_gelu_f16": [_P, _L, _P],
+    "ctrlora_dpm_model_output": [_P, _P, _P, _P, _P, _L, _I, _I, _P, _P],
+    "ctrlora_dpm_solver_update": [_P, _P, _P, _P, _P, _L, _I, _P, _P],
+    "ctrlora_dpm_threshold": [_P, _P, _I, _L, _L, _L, _F, _F, _P],
+    "ctrlora_dpm_adaptive_error": [_P, _P, _P, _P, _I, _L, _F, _F, _P],
 }
 
 
@@ -199,4 +203,8 @@ EXPORTS = [
     "ctrlora_clip_patch_gather",
     "ctrlora_clip_vision_embed",
     "ctrlora_gelu_f16",
+    "ctrlora_dpm_model_output",
+    "ctrlora_dpm_solver_update",
+    "ctrlora_dpm_threshold",
+    "ctrlora_dpm_adaptive_error",
 ]

@@ -664,6 +664,71 @@ def plms_update(x, e_cond, e_uncond, e_out, cfg_scale, sqrt_a_t, sqrt_one_minus_
     return x_prev, pred_x0
 
 
+DPM_NCOEF = 9
+DPM_MODEL_TYPES = {"noise": 0, "x_start": 1, "v": 2}
+DPM_UPDATE_MODES = {"first": 0, "diff": 1, "multistep2": 2, "multistep3": 3, "singlestep3_taylor": 4}
+
+
+def _dpm_coef(coef):
+    vals = [float(v) for v in coef] + [0.0] * (DPM_NCOEF - len(coef))
+    assert len(vals) == DPM_NCOEF
+    return (C.c_float * DPM_NCOEF)(*vals)
+
+
+def _dpm_like(x, *ts):
+    _require_cuda(x, *ts)
+    for t in (x,) + ts:
+        assert t is None or (t.dtype == torch.float32 and t.is_contiguous() and t.shape == x.shape), \
+            "DPM-Solver kernels take fp32 contiguous tensors of x's shape"
+
+
+def dpm_model_output(x, out_cond, m_out, model_type="noise", out_uncond=None, grad=None, predict_x0=False,
+                     scale=1.0, alpha_w=1.0, sigma_w=1.0, grad_coef=0.0, sigma_t=1.0, alpha_t=1.0):
+    """One DPM_Solver model value into m_out (ldm/models/diffusion/dpm_solver/dpm_solver.py:257-312, :352-359): the
+    model output converted to noise, guided by out_uncond (classifier-free) or grad (classifier), and with predict_x0
+    the data prediction (x - sigma_t e) / alpha_t.  Scalars from ctrlora_b200.dpm_schedule."""
+    _dpm_like(x, out_cond, m_out, out_uncond, grad)
+    _count()
+    check(_lib.load().ctrlora_dpm_model_output(
+        _dp(x), _dp(out_cond), _dp(out_uncond), _dp(grad), _dp(m_out), x.numel(), DPM_MODEL_TYPES[model_type],
+        int(bool(predict_x0)), _dpm_coef((scale, alpha_w, sigma_w, grad_coef, sigma_t, alpha_t)), _sp()),
+        "dpm_model_output")
+    return m_out
+
+
+def dpm_solver_update(mode, x, m0, coef, m1=None, m2=None, out=None):
+    """One DPM_Solver update of the given mode (first / diff / multistep2 / multistep3 / singlestep3_taylor, see
+    include/ctrlora_b200.h) with coef = (a, b, c, d, k0, k1, k2, k3, rd) from ctrlora_b200.dpm_schedule; returns x_t."""
+    out = torch.empty_like(x) if out is None else out
+    _dpm_like(x, m0, m1, m2, out)
+    _count()
+    check(_lib.load().ctrlora_dpm_solver_update(_dp(x), _dp(m0), _dp(m1), _dp(m2), _dp(out), x.numel(),
+                                                DPM_UPDATE_MODES[mode], _dpm_coef(coef), _sp()), "dpm_solver_update")
+    return out
+
+
+def dpm_threshold_(x0, k_lo, k_hi, weight, max_val, s_out=None):
+    """Dynamic thresholding of x0 [B, ...] in place (dpm_solver.py:360-364); k_lo / k_hi / weight locate torch.quantile's
+    0.995 order statistics (ctrlora_b200.dpm_schedule.quantile_rank).  s_out [B] receives the per-image s."""
+    _require_cuda(x0, s_out)
+    assert x0.dtype == torch.float32 and x0.is_contiguous()
+    _count()
+    check(_lib.load().ctrlora_dpm_threshold(_dp(x0), _dp(s_out), x0.shape[0], x0[0].numel(), int(k_lo), int(k_hi),
+                                            float(weight), float(max_val), _sp()), "dpm_threshold")
+    return x0
+
+
+def dpm_adaptive_error(x_lower, x_prev, x_higher, atol, rtol, err=None):
+    """The adaptive solver's E (dpm_solver.py:926-928) as a one-element fp32 device tensor."""
+    _dpm_like(x_lower, x_prev, x_higher)
+    err = torch.empty(1, device=x_lower.device, dtype=torch.float32) if err is None else err
+    _count()
+    check(_lib.load().ctrlora_dpm_adaptive_error(_dp(x_lower), _dp(x_prev), _dp(x_higher), _dp(err), x_lower.shape[0],
+                                                 x_lower[0].numel(), float(atol), float(rtol), _sp()),
+          "dpm_adaptive_error")
+    return err
+
+
 def wgrad_tn(a, b, out=None, alpha=1.0, beta=0.0):
     """out[p, q] = alpha * sum_m a[m, p] * b[m, q] + beta * out  (fp16 a [M,P], b [M,Q] -> fp32 [P,Q])."""
     _require_cuda(a, b)

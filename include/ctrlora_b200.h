@@ -238,6 +238,52 @@ int ctrlora_plms_update(const float* x, const float* e_cond, const float* e_unco
                         float* x_prev, float* pred_x0, int order, int total, float cfg_scale, float sqrt_a_t,
                         float sqrt_one_minus_at, float sqrt_a_prev, float dir_coef, void* stream);
 
+/* DPM_Solver (ldm/models/diffusion/dpm_solver/dpm_solver.py), every method and order.  fp32 contiguous tensors, all
+ * arithmetic round-to-nearest in the reference's order; `coef` is a host array of CTRLORA_DPM_NCOEF floats formed by
+ * ctrlora_b200.dpm_schedule on the CPU (unused entries are ignored). */
+#define CTRLORA_DPM_NCOEF 9
+#define CTRLORA_DPM_MODEL_NOISE 0
+#define CTRLORA_DPM_MODEL_X_START 1
+#define CTRLORA_DPM_MODEL_V 2
+/* One model value, written to the caller's history slot m_out (model_wrapper :257-312, data_prediction_fn :352-359):
+ *   e = to_noise(out_cond), to_noise by model_type: out | (x - alpha_w out) / sigma_w | alpha_w out + sigma_w x
+ *   e = u + coef[0] * (e - u)                 u = to_noise(out_uncond), classifier-free guidance  (NULL: none)
+ *   e = e - coef[3] * grad                    classifier guidance, coef[3] = scale * sigma_t      (NULL: none)
+ *   m_out = (x - coef[4] * e) / coef[5]       predict_x0: sigma_t, alpha_t of the solver's schedule
+ * coef[1] = alpha_w, coef[2] = sigma_w (the wrapper's schedule at t). */
+int ctrlora_dpm_model_output(const float* x, const float* out_cond, const float* out_uncond, const float* grad,
+                             float* m_out, long long total, int model_type, int predict_x0, const float* coef,
+                             void* stream);
+#define CTRLORA_DPM_UPDATE_FIRST 0
+#define CTRLORA_DPM_UPDATE_DIFF 1
+#define CTRLORA_DPM_UPDATE_MULTISTEP2 2
+#define CTRLORA_DPM_UPDATE_MULTISTEP3 3
+#define CTRLORA_DPM_UPDATE_SINGLESTEP3_TAYLOR 4
+/* One update, out = a x - b m0 + ... with (a, b, c, d, k0, k1, k2, k3, rd) = coef[0..8]; c and d carry their sign:
+ *   FIRST                 a x - b m0                                          dpm_solver_first_update :469-513, and
+ *                                                                             every singlestep x_s1
+ *   DIFF                  a x - b m0 + c (m1 - m0)                            singlestep-2 :553-593, singlestep-3 x_s2
+ *                                                                             :655-698 and 'dpm_solver' x_t :661-705
+ *   MULTISTEP2            D = k0 (m0 - m1); a x - b m0 + c D                  :751-777 (m0 newest, m1 previous)
+ *   MULTISTEP3            D0 = k0 (m0 - m1), D1 = k1 (m1 - m2), G = D0 - D1;  :807-824
+ *                         a x - b m0 + c (D0 + k2 G) + d (k3 G)
+ *   SINGLESTEP3_TAYLOR    D0 = k0 (m1 - m0), D1 = k1 (m2 - m0);               'taylor' x_t :668-677, :707-716
+ *                         a x - b m0 + c ((k3 D0 - k2 D1) / rd) + d ((2 (D1 - D0)) / rd)
+ * m1 / m2 are NULL exactly when the mode does not read them. */
+int ctrlora_dpm_solver_update(const float* x, const float* m0, const float* m1, const float* m2, float* out,
+                              long long total, int mode, const float* coef, void* stream);
+/* Dynamic thresholding in place (data_prediction_fn :360-364), x0 [batch, per_image]: per image, the order statistics
+ * k_lo / k_hi of |x0| joined as torch.quantile's lerp with `weight` (the fractional part of fp32(0.995) * (n - 1)),
+ * s = max(that, max_val), x0 = clamp(x0, -s, s) / s.  s_out (optional, [batch]) receives s.  Radix select in shared
+ * memory when the image fits, in global memory otherwise. */
+int ctrlora_dpm_threshold(float* x0, float* s_out, int batch, long long per_image, long long k_lo, long long k_hi,
+                          float weight, float max_val, void* stream);
+/* Adaptive solver's error (dpm_solver_adaptive :926-928) into the device scalar err:
+ * max over images of sqrt(mean(((x_higher - x_lower) / max(atol, rtol * max(|x_lower|, |x_prev|)))^2)).
+ * The sum's order is a fixed tree, not torch's: E agrees with the reference to rounding, not to the bit. */
+int ctrlora_dpm_adaptive_error(const float* x_lower, const float* x_prev, const float* x_higher, float* err, int batch,
+                               long long per_image, float atol, float rtol, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * Training (backward of the trainable set; reference: autograd over cldm/lora.py:70-80,285-291 and cldm/cldm.py:281-282,
  * parameters selected by cldm/cldm_ctrlora_finetune.py:88-100).
