@@ -127,6 +127,9 @@ _ARGTYPES = {
     "ctrlora_dpm_solver_update": [_P, _P, _P, _P, _P, _L, _I, _P, _P],
     "ctrlora_dpm_threshold": [_P, _P, _I, _L, _L, _L, _F, _F, _P],
     "ctrlora_dpm_adaptive_error": [_P, _P, _P, _P, _I, _L, _F, _F, _P],
+    "ctrlora_tap_gather_f16": [_P, _I, _L, _P, _I, _I, _I, _I, _P, _I, _I, _I, _P],
+    "ctrlora_instance_norm_f16": [_P, _P, _P, _P, _L, _I, _I, _I, _I, _I, _I, _F, _P],
+    "ctrlora_lineart_out_f16": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
 }
 
 
@@ -207,4 +210,7 @@ EXPORTS = [
     "ctrlora_dpm_solver_update",
     "ctrlora_dpm_threshold",
     "ctrlora_dpm_adaptive_error",
+    "ctrlora_tap_gather_f16",
+    "ctrlora_instance_norm_f16",
+    "ctrlora_lineart_out_f16",
 ]

@@ -1035,6 +1035,76 @@ def gelu_(x):
     return x
 
 
+# ------------------------------------------------------------------------------------------------ line-art annotator
+def tap_gather(x, taps, *, reflect, k_pad, channels=None, out=None):
+    """Gather the (dy, dx) taps of every pixel into GEMM rows: fp16 [B, H, W, k_pad], column t * C + c = x at (y + dy_t,
+    x + dx_t), reflected at the border (nn.ReflectionPad2d) or zero outside, zero beyond len(taps) * C.
+    x: fp16 pixel-major [B, H, W, ld] (channels <= ld, default ld) or fp32 NCHW [B, C, H, W] contiguous."""
+    _require_cuda(x)
+    if x.dtype == torch.float32:
+        assert x.dim() == 4 and x.is_contiguous()
+        b, c, h, w = x.shape
+        ld, f32 = 0, 1
+    else:
+        assert x.dtype == torch.float16
+        b, h, w, c, ld = _as_bhwc(x)
+        c, f32 = channels or c, 0
+    n = len(taps)
+    flat = (C.c_int * (2 * n))(*[int(v) for t in taps for v in t])
+    if out is None:
+        out = torch.empty((b, h, w, k_pad), device=x.device, dtype=torch.float16)
+    assert out.shape == (b, h, w, k_pad) and out.is_contiguous() and out.dtype == torch.float16
+    _count()
+    check(_lib.load().ctrlora_tap_gather_f16(_dp(x), f32, ld, _dp(out), b, h, w, c, C.cast(flat, C.c_void_p), n,
+                                             int(bool(reflect)), k_pad, _sp()), "tap_gather")
+    return out
+
+
+INSTANCE_NORM_MAX_CHUNKS = 1024  # per-image statistics chunks (annotator_sm90.cu kNormMaxChunks)
+
+
+def instance_norm(x, *, relu, residual=None, phases=False, eps=1e-5, out=None):
+    """InstanceNorm2d (affine=False) + optional ReLU + optional residual add, fp16 pixel-major.
+    phases=False: x [B, H, W, C] -> [B, H, W, C].  phases=True: x [4, B, H, W, C], the four sub-pixel phase outputs
+    (2 py + px) of a stride-2 transposed conv -> [B, 2H, 2W, C] interleaved.  residual: y's shape, added last."""
+    _require_cuda(x, residual)
+    assert x.dtype == torch.float16 and x.is_contiguous()
+    if phases:
+        assert x.dim() == 5 and x.shape[0] == 4
+        _, b, h, w, c = x.shape
+        shape = (b, 2 * h, 2 * w, c)
+    else:
+        b, h, w, c = x.shape
+        shape = (b, h, w, c)
+    if out is None:
+        out = torch.empty(shape, device=x.device, dtype=torch.float16)
+    assert out.shape == shape and out.is_contiguous() and out.dtype == torch.float16
+    if residual is not None:
+        assert residual.shape == shape and residual.is_contiguous() and residual.dtype == torch.float16
+    ws_floats = 2 * b * c * (INSTANCE_NORM_MAX_CHUNKS + 1)
+    ws = torch.empty(ws_floats, device=x.device, dtype=torch.float32)
+    _count(3)
+    check(_lib.load().ctrlora_instance_norm_f16(_dp(x), _dp(residual), _dp(out), _dp(ws), ws_floats, b, h, w, c,
+                                                int(bool(phases)), int(bool(relu)), float(eps), _sp()), "instance_norm")
+    return out
+
+
+def lineart_out(x, weight, bias, want_u8=False):
+    """ReflectionPad2d(3) + Conv2d(C -> 1, 7) + Sigmoid: x fp16 [B, H, W, C], weight fp32 [49, C] (tap-major), bias fp32
+    [1] (device) -> fp32 [B, 1, H, W] (and with want_u8 the uint8 [B, H, W] map (uint8)clip(y * 255, 0, 255))."""
+    _require_cuda(x, weight, bias)
+    assert x.dtype == torch.float16 and x.is_contiguous() and x.dim() == 4
+    b, h, w, c = x.shape
+    assert weight.dtype == torch.float32 and weight.is_contiguous() and weight.shape == (49, c)
+    assert bias.dtype == torch.float32 and bias.numel() == 1
+    out = torch.empty((b, 1, h, w), device=x.device, dtype=torch.float32)
+    u8 = torch.empty((b, h, w), device=x.device, dtype=torch.uint8) if want_u8 else None
+    _count()
+    check(_lib.load().ctrlora_lineart_out_f16(_dp(x), _dp(weight), _dp(bias), _dp(out), _dp(u8), b, h, w, c, _sp()),
+          "lineart_out")
+    return (out, u8) if want_u8 else out
+
+
 def set_sm_limit(limit):
     """persistent GEMM grids use at most `limit` SMs (0 = all); baked into CUDA graphs at capture"""
     check(_lib.load().ctrlora_set_sm_limit(int(limit)), "set_sm_limit")

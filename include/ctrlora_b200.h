@@ -398,6 +398,35 @@ int ctrlora_clip_vision_embed(const float* patch_out, long long ldp, const float
  * towers), fp32 math, in place on fp16 [n] (n % 8 == 0) */
 int ctrlora_gelu_f16(void* x, long long n, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * Line-art annotator (annotator/lineart/__init__.py:36-91, informative-drawings' Generator, as
+ * LineartDetector.__call__ :111-122 runs it).  Its convs become ctrlora_gemm_f16 launches over gathered operands.
+ *
+ * Tap gather: dst[b, y, x, t * channels + c] = src[b, Y(y + dy_t), X(x + dx_t), c] for the n_taps (dy, dx) pairs of the
+ * host array `taps` (n_taps <= 64), fp16 [batch, h, w, k_pad]; columns >= n_taps * channels are zero.  reflect = 1: Y / X
+ * mirror without repeating the border (nn.ReflectionPad2d, :21,25,41,77; |dy| < h, |dx| < w); reflect = 0: outside taps
+ * read 0 (the sub-pixel phases of ConvTranspose2d(3, stride 2, padding 1, output_padding 1), :69).  src: fp16 pixel-major
+ * [batch, h, w, ld] (src_f32_nchw = 0), or fp32 NCHW [batch, channels, h, w] (src_f32_nchw = 1, ld unused: the network
+ * input of :116-119).  k_pad % 8 == 0.
+ */
+int ctrlora_tap_gather_f16(const void* src, int src_f32_nchw, long long ld, void* dst, int batch, int h, int w, int channels,
+                           const int* taps, int n_taps, int reflect, int k_pad, void* stream);
+/* InstanceNorm2d(affine = False, track_running_stats = False) (:14): per (image, channel) biased statistics over the
+ * image's rows, then y = relu?((x - mean) / sqrt(var + eps)) + residual?, fp16 in and out, fp32 math (the ReLU of :24,44,54,71
+ * and ResidualBlock's x + conv_block(x), :33).  phases = 0: x and y are [batch, h, w, channels].  phases = 1: x holds the
+ * four sub-pixel phase outputs of a stride-2 transposed conv, [4, batch, h, w, channels] with phase 2 py + px, and y is
+ * [batch, 2h, 2w, channels], y[b, 2m + py, 2n + px] = f(x[2 py + px, b, m, n]).  residual (or NULL) has y's layout.
+ * Statistics: fixed per-image row chunks and a fixed summation order, no atomics (bit-reproducible, and independent of
+ * the batch).  ws: fp32 scratch of at least 2 * batch * channels * 1025 floats.  channels in {64, 128, 256}. */
+int ctrlora_instance_norm_f16(const void* x, const void* residual, void* y, float* ws, long long ws_floats, int batch, int h,
+                              int w, int channels, int phases, int relu, float eps, void* stream);
+/* The output layer (:77-80): ReflectionPad2d(3) + Conv2d(channels -> 1, 7) + Sigmoid on fp16 [batch, h, w, channels]
+ * (channels % 16 == 0, h, w > 3), fp32 accumulation.  weight: fp32 [49, channels] (tap-major), bias: fp32 [1] (device).
+ * out: fp32 [batch, h, w]; out_u8 (or NULL): uint8 [batch, h, w] = (uint8)clip(out * 255, 0, 255) with an fp32 multiply
+ * and truncation, as LineartDetector's `(line * 255.0).clip(0, 255).astype(np.uint8)` (:122). */
+int ctrlora_lineart_out_f16(const void* x, const float* weight, const float* bias, float* out, unsigned char* out_u8,
+                            int batch, int h, int w, int channels, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
