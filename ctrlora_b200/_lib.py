@@ -27,6 +27,7 @@ class GemmArgs(C.Structure):
         ("splitk_counters", c_void_p), ("splitk_counters_len", c_int),
         ("dup_out", c_void_p), ("dup_ld", c_int), ("force_single_cta", c_int),
         ("group_b", c_int), ("w_hi", c_void_p), ("bias_hi", c_void_p), ("rowbias_hi", c_void_p), ("w2_hi", c_void_p),
+        ("relu", c_int),
     ]
 
 
@@ -130,6 +131,8 @@ _ARGTYPES = {
     "ctrlora_tap_gather_f16": [_P, _I, _L, _P, _I, _I, _I, _I, _P, _I, _I, _I, _P],
     "ctrlora_instance_norm_f16": [_P, _P, _P, _P, _L, _I, _I, _I, _I, _I, _I, _F, _P],
     "ctrlora_lineart_out_f16": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
+    "ctrlora_hed_side_pool_f16": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
+    "ctrlora_hed_fuse": [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
 }
 
 
@@ -213,4 +216,6 @@ EXPORTS = [
     "ctrlora_tap_gather_f16",
     "ctrlora_instance_norm_f16",
     "ctrlora_lineart_out_f16",
+    "ctrlora_hed_side_pool_f16",
+    "ctrlora_hed_fuse",
 ]

@@ -1,2 +1,3 @@
-"""Condition-image annotators on the sm_90a kernels.  Only line art (`ctrlora_b200.annotator.lineart`) is implemented;
-the reference's other detectors stay its own `annotator` package."""
+"""Condition-image annotators on the sm_90a kernels: line art (`ctrlora_b200.annotator.lineart`), HED
+(`ctrlora_b200.annotator.hed`) and HED-sketch (`ctrlora_b200.annotator.hedsketch`).  The reference's other detectors
+stay its own `annotator` package."""

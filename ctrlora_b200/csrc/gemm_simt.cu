@@ -44,6 +44,7 @@ __global__ void gemm_simt_kernel(ctrlora_gemm_args a, int M, int rows_per_img) {
     v *= a.out_scale;
     if (a.residual) v += a.residual_f32 ? reinterpret_cast<const float*>(a.residual)[m * a.ldr + n]
                                          : __half2float(reinterpret_cast<const __half*>(a.residual)[m * a.ldr + n]);
+    if (a.relu) v = fmaxf(v, 0.f);
     int seg = 0, nloc = n;
     if (a.seg_width > 0) { seg = n / a.seg_width; nloc = n % a.seg_width; }
     if (a.transposed[seg]) {

@@ -88,6 +88,10 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, float* v, i
                 if (c + j < bn_out && nbase + j < p.N) v[j] += __half2float(rp[j]);
         }
     }
+    if (p.relu) {
+#pragma unroll
+        for (int j = 0; j < CW; ++j) v[j] = fmaxf(v[j], 0.f);
+    }
     int seg = 0, nloc = nbase;
     if (p.seg_width > 0) { seg = nbase / p.seg_width; nloc = nbase - seg * p.seg_width; }
     if (p.transposed[seg]) {
@@ -334,6 +338,10 @@ __device__ __forceinline__ void gemm_pingpong_consumers(const GemmKParams& p, ui
                         const float2 r0 = h2_to_f2(lds32(a0)), r1 = h2_to_f2(lds32(a1));
                         v00 = __fadd_rn(v00, r0.x); v01 = __fadd_rn(v01, r0.y);
                         v10 = __fadd_rn(v10, r1.x); v11 = __fadd_rn(v11, r1.y);
+                    }
+                    if (p.relu) {
+                        v00 = fmaxf(v00, 0.f); v01 = fmaxf(v01, 0.f);
+                        v10 = fmaxf(v10, 0.f); v11 = fmaxf(v11, 0.f);
                     }
                     sts32(a0, pack_h2(v00, v01));
                     sts32(a1, pack_h2(v10, v11));
@@ -634,6 +642,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                         const float2 r0 = h2_to_f2(lds32(a0)), r1 = h2_to_f2(lds32(a1));
                         v00 = __fadd_rn(v00, r0.x); v01 = __fadd_rn(v01, r0.y);
                         v10 = __fadd_rn(v10, r1.x); v11 = __fadd_rn(v11, r1.y);
+                    }
+                    if (p.relu) {
+                        v00 = fmaxf(v00, 0.f); v01 = fmaxf(v01, 0.f);
+                        v10 = fmaxf(v10, 0.f); v11 = fmaxf(v11, 0.f);
                     }
                     sts32(a0, pack_h2(v00, v01));
                     sts32(a1, pack_h2(v10, v11));
@@ -952,6 +964,7 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
     p.out_scale = a->out_scale;
     p.head_dim = a->head_dim; p.tok_pad = a->tok_pad;
     p.dup_out = reinterpret_cast<__half*>(a->dup_out); p.dup_ld = a->dup_ld;
+    p.relu = a->relu;
 
     const int b_box = p.geglu || p.BN > 256 ? p.BN / 2 : p.BN;  // rows of a B box (the kernel's BOX)
     CUtensorMap tm[10];  // A, B, A2, B2, residual, out[0..2], B and B2 of the second group

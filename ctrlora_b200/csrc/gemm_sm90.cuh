@@ -71,6 +71,7 @@ struct GemmKParams {
     int rb_img_off;
     const float* bias_g[2];
     const float* rowbias_g[2];
+    int relu;                       // max(v, 0) just before the output rounding
 };
 
 }  // namespace ctrl

@@ -146,6 +146,21 @@ def gemm(a, w, *, ksize=1, bias=None, rowbias=None, rows_per_img=0, rowbias_ld=0
     an [M,K] one): a dict with the upper half's "w" and, as the call has them, "bias", "rowbias" (indexed from the
     half's first image) and "w2".  A batch whose halves cannot be tiled apart runs as two launches.
     """
+    return _gemm(a, w, ksize=ksize, bias=bias, rowbias=rowbias, rows_per_img=rows_per_img, rowbias_ld=rowbias_ld,
+                 residual=residual, out_scale=out_scale, a2=a2, w2=w2, geglu=geglu, out=out, out_f32=out_f32,
+                 seg_outs=seg_outs, seg_width=seg_width, transposed=transposed, head_dim=head_dim, tok_pad=tok_pad,
+                 block_n=block_n, split_k=split_k, dup_out=dup_out, single_cta=single_cta, simt=simt, hi=hi)
+
+
+def gemm_relu(a, w, **kwargs):
+    """ops.gemm (same arguments) with max(., 0) as the epilogue's last step, before the output rounding: a conv + ReLU
+    pair in one launch.  A function of its own, so that gemm's arguments stay those of its fp32 launch reference."""
+    return _gemm(a, w, relu=True, **kwargs)
+
+
+def _gemm(a, w, *, ksize=1, bias=None, rowbias=None, rows_per_img=0, rowbias_ld=0, residual=None, out_scale=1.0, a2=None,
+          w2=None, geglu=False, out=None, out_f32=False, seg_outs=None, seg_width=0, transposed=(0, 0, 0), head_dim=0,
+          tok_pad=0, block_n=0, split_k=0, dup_out=None, single_cta=False, simt=False, hi=None, relu=False):
     _require_cuda(a, w)
     assert a.dtype == torch.float16 and w.dtype == torch.float16 and w.is_contiguous()
     n_rows = w.shape[0]
@@ -198,6 +213,7 @@ def gemm(a, w, *, ksize=1, bias=None, rowbias=None, rows_per_img=0, rowbias_ld=0
     if dup_out is not None:
         args.dup_out, args.dup_ld = dup_out.data_ptr(), dup_out.stride(0)
     args.force_single_cta = int(single_cta)
+    args.relu = int(bool(relu))
     if hi is not None:
         if hi.get("rowbias") is not None:  # the kernel reads both halves' row terms with the lower half's row stride
             assert rowbias is not None and hi["rowbias"].stride(0) == rowbias.stride(0) and \
@@ -224,11 +240,11 @@ def gemm(a, w, *, ksize=1, bias=None, rowbias=None, rows_per_img=0, rowbias_ld=0
 
     for lo in (True, False):
         segs = None if seg_outs is None else [cut(o, lo, by_image=bool(t)) for o, t in zip(seg_outs, transposed)]
-        gemm(cut(a, lo), w if lo else hi["w"], ksize=ksize, bias=bias if lo else hi.get("bias"),
-             rowbias=rowbias if lo else hi.get("rowbias"), rows_per_img=rows_per_img, rowbias_ld=rowbias_ld,
-             residual=cut(residual, lo), out_scale=out_scale, a2=cut(a2, lo), w2=w2 if lo else hi.get("w2"),
-             geglu=geglu, out=cut(out, lo), out_f32=out_f32, seg_outs=segs, seg_width=seg_width, transposed=transposed,
-             head_dim=head_dim, tok_pad=tok_pad, block_n=block_n, split_k=split_k)
+        _gemm(cut(a, lo), w if lo else hi["w"], ksize=ksize, bias=bias if lo else hi.get("bias"),
+              rowbias=rowbias if lo else hi.get("rowbias"), rows_per_img=rows_per_img, rowbias_ld=rowbias_ld,
+              residual=cut(residual, lo), out_scale=out_scale, a2=cut(a2, lo), w2=w2 if lo else hi.get("w2"),
+              geglu=geglu, out=cut(out, lo), out_f32=out_f32, seg_outs=segs, seg_width=seg_width, transposed=transposed,
+              head_dim=head_dim, tok_pad=tok_pad, block_n=block_n, split_k=split_k, relu=relu)
     return ret
 
 
@@ -1103,6 +1119,49 @@ def lineart_out(x, weight, bias, want_u8=False):
     check(_lib.load().ctrlora_lineart_out_f16(_dp(x), _dp(weight), _dp(bias), _dp(out), _dp(u8), b, h, w, c, _sp()),
           "lineart_out")
     return (out, u8) if want_u8 else out
+
+
+# ------------------------------------------------------------------------------------------------ HED annotator
+def hed_side_pool(x, weight, bias, pool):
+    """A HED block's 1x1 side projection (C -> 1) and, with pool, the 2x2 max-pool (floor) that feeds the next block, in
+    one read of x fp16 [B, h, w, C].  weight fp32 [C], bias fp32 [1] (device).  Returns (fp32 [B, 1, h, w] side map,
+    fp16 [B, h // 2, w // 2, C] pooled or None)."""
+    _require_cuda(x, weight, bias)
+    assert x.dtype == torch.float16 and x.is_contiguous() and x.dim() == 4
+    b, h, w, c = x.shape
+    assert weight.dtype == torch.float32 and weight.is_contiguous() and weight.numel() == c
+    assert bias.dtype == torch.float32 and bias.numel() == 1
+    side = torch.empty((b, 1, h, w), device=x.device, dtype=torch.float32)
+    pooled = torch.empty((b, h // 2, w // 2, c), device=x.device, dtype=torch.float16) if pool else None
+    _count()
+    check(_lib.load().ctrlora_hed_side_pool_f16(_dp(x), _dp(weight), _dp(bias), _dp(side), _dp(pooled), b, h, w, c, _sp()),
+          "hed_side_pool")
+    return side, pooled
+
+
+def hed_fuse(sides, tables, safe):
+    """HEDdetector's post-process on the device.  sides: the five fp32 [B, 1, h_l, w_l] side maps, the first at the
+    output size H x W; tables: for levels 1..4, (int32 [H + W] source index, fp32 [H + W] fraction) device pairs (rows
+    then columns, annotator.hed.resize_tables).  Returns (fp32 [B, H, W] mean map, uint8 [B, H, W] edge map)."""
+    _require_cuda(*sides)
+    assert len(sides) == 5 and len(tables) == 4
+    b, _, h, w = sides[0].shape
+    for s in sides:
+        assert s.dtype == torch.float32 and s.is_contiguous() and s.shape[:2] == (b, 1)
+    for idx, frac in tables:
+        _require_cuda(idx, frac)
+        assert idx.dtype == torch.int32 and frac.dtype == torch.float32 and idx.numel() == frac.numel() == h + w
+    mean = torch.empty((b, h, w), device=sides[0].device, dtype=torch.float32)
+    u8 = torch.empty((b, h, w), device=sides[0].device, dtype=torch.uint8)
+    ptrs = (C.c_void_p * 5)(*[s.data_ptr() for s in sides])
+    hw = (C.c_int * 10)(*[v for s in sides for v in s.shape[2:]])
+    idx_p = (C.c_void_p * 5)(None, *[t[0].data_ptr() for t in tables])
+    frac_p = (C.c_void_p * 5)(None, *[t[1].data_ptr() for t in tables])
+    _count()
+    check(_lib.load().ctrlora_hed_fuse(C.cast(ptrs, C.c_void_p), C.cast(hw, C.c_void_p), C.cast(idx_p, C.c_void_p),
+                                       C.cast(frac_p, C.c_void_p), _dp(mean), _dp(u8), b, h, w, int(bool(safe)), _sp()),
+          "hed_fuse")
+    return mean, u8
 
 
 def set_sm_limit(limit):

@@ -88,6 +88,9 @@ typedef struct ctrlora_gemm_args {
     const float* bias_hi;
     const float* rowbias_hi;
     const void* w2_hi;
+    /* relu = 1: max(v, 0) as the last step before the output rounding, after bias, row term, scale and residual (split
+     * tiles: after the split-K sum).  The ReLU of HED's conv + ReLU pairs (annotator/hed/__init__.py:30-31). */
+    int relu;
 } ctrlora_gemm_args;
 
 int ctrlora_gemm_f16(const ctrlora_gemm_args* args, void* stream);
@@ -426,6 +429,28 @@ int ctrlora_instance_norm_f16(const void* x, const void* residual, void* y, floa
  * and truncation, as LineartDetector's `(line * 255.0).clip(0, 255).astype(np.uint8)` (:122). */
 int ctrlora_lineart_out_f16(const void* x, const float* weight, const float* bias, float* out, unsigned char* out_u8,
                             int batch, int h, int w, int channels, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
+ * HED annotator (annotator/hed/__init__.py, ControlNetHED_Apache2 :36-52 as HEDdetector.__call__ :65-79 runs it).  Its
+ * 3x3 conv + ReLU pairs (:28-31) are ctrlora_gemm_f16 launches with relu = 1.
+ *
+ * Side projection and pool: x is a block's output, fp16 [batch, h, w, channels] (channels in {64, 128, 256, 512}, 16-byte
+ * aligned), read once.  side: fp32 [batch, h, w] = bias[0] + sum_c weight[c] * x[.., c], fp32 accumulation in a fixed
+ * order (DoubleConvBlock.projection, :32).  pooled (or NULL): fp16 [batch, h / 2, w / 2, channels], the 2x2 max of x,
+ * floor sizes (the next block's max_pool2d(2, 2), :28); a max is exact, so it equals max_pool2d on x bit for bit.
+ * weight: fp32 [channels], bias: fp32 [1] (device).
+ */
+int ctrlora_hed_side_pool_f16(const void* x, const float* weight, const float* bias, float* side, void* pooled, int batch,
+                              int h, int w, int channels, void* stream);
+/* The detector's post-process (:70-78) for the five side maps at once.  sides[l]: fp32 [batch, side_hw[2l], side_hw[2l+1]];
+ * level 0 is h x w and is taken as is (cv2.resize to its own size is a copy).  Levels 1..4 are resized bilinearly to
+ * h x w through host-built tables (cv2's INTER_LINEAR coordinate rule): idx[l] int32 [h + w], the source row of each
+ * output row then the source column of each output column, and frac[l] fp32 [h + w], their fractional weights (the
+ * neighbour index is clamped to the map).  mean: fp32 [batch, h, w] = ((((e1 + e2) + e3) + e4) + e5) / 5 in fp32;
+ * then edge = 1 / (1 + exp(-mean)) in float64, with safe = 1 safe_step's (float)(int)((float)edge * 3) / 2
+ * (annotator/util.py:78-81), and out_u8 = (uint8)clip(edge * 255, 0, 255).  idx and frac of level 0 are unused. */
+int ctrlora_hed_fuse(const float* const* sides, const int* side_hw, const int* const* idx, const float* const* frac,
+                     float* mean, unsigned char* out_u8, int batch, int h, int w, int safe, void* stream);
 
 #ifdef __cplusplus
 }
