@@ -70,6 +70,7 @@ def load():
 
 
 _P, _I, _L, _F = c_void_p, c_int, c_ll, c_float
+_D = C.c_double
 _ARGTYPES = {
     "ctrlora_gemm_f16": [_P, _P],
     "ctrlora_gemm_f16_simt": [_P, _P],
@@ -133,6 +134,10 @@ _ARGTYPES = {
     "ctrlora_lineart_out_f16": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
     "ctrlora_hed_side_pool_f16": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
     "ctrlora_hed_fuse": [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
+    "ctrlora_openpose_resample": [_P, _I, _I, _I, _I, _P, _P, _I, _P, _P, _I, _P, _I, _I, _P],
+    "ctrlora_openpose_smooth": [_P, _P, _P, _I, _I, _I, _P, _I, _P],
+    "ctrlora_openpose_peaks": [_P, _P, _I, _I, _I, _D, _P, _L, _P, _P, _P, _P, _I, _P],
+    "ctrlora_openpose_limbs": [_P, _I, _I, _I, _P, _P, _I, _P, _P, _I, _P, _P, _P, _I, _L, _I, _D, _P, _P, _P],
 }
 
 
@@ -218,4 +223,8 @@ EXPORTS = [
     "ctrlora_lineart_out_f16",
     "ctrlora_hed_side_pool_f16",
     "ctrlora_hed_fuse",
+    "ctrlora_openpose_resample",
+    "ctrlora_openpose_smooth",
+    "ctrlora_openpose_peaks",
+    "ctrlora_openpose_limbs",
 ]

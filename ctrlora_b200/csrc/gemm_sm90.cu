@@ -808,7 +808,9 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     if (!a || !a->a || !a->w || !a->out[0]) return CTRLORA_ERR_ARG;
     if (a->a_c % 8 != 0 || a->a_ld % 8 != 0) return CTRLORA_ERR_ARG;
-    if (a->kh != a->kw || (a->kh != 1 && a->kh != 3)) return CTRLORA_ERR_UNSUPPORTED;
+    // square 1x1, 3x3 and 7x7 taps (7x7: OpenPose's CPM stages); the box origin goes down to -pad, which the tensor
+    // map's out-of-bounds fill reads as zero padding
+    if (a->kh != a->kw || (a->kh != 1 && a->kh != 3 && a->kh != 7)) return CTRLORA_ERR_UNSUPPORTED;
     if (a->bf16) return CTRLORA_ERR_UNSUPPORTED;
     GemmKParams p;
     memset(&p, 0, sizeof(p));

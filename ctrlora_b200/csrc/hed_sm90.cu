@@ -12,7 +12,8 @@ namespace ctrl {
 // 8-channel vectors l, l + G, ... (NV of them) of every pixel of its quad and reads each with one 16-byte load.  Side:
 // the lane's products summed in channel order, then a fixed xor tree across the group, then the bias.  Pool: the max
 // of the quad's four vectors, stored only for the quads that lie wholly inside the image (max_pool2d floors odd sizes).
-template <int NV>
+// SIDE = false: the pool alone (OpenPose's VGG trunk), no projection weights and no side map.
+template <int NV, bool SIDE>
 __global__ void __launch_bounds__(256)
 hed_side_pool_kernel(const __half* __restrict__ x, const float* __restrict__ wt, const float* __restrict__ bias,
                      float* __restrict__ side, __half* __restrict__ pooled, int h, int w, int channels, long long quads,
@@ -25,8 +26,8 @@ hed_side_pool_kernel(const __half* __restrict__ x, const float* __restrict__ wt,
 #pragma unroll
     for (int k = 0; k < NV; ++k)
 #pragma unroll
-        for (int e = 0; e < 8; ++e) wr[k][e] = __ldg(wt + (gl + k * G) * 8 + e);
-    const float b0 = __ldg(bias);
+        for (int e = 0; e < 8; ++e) wr[k][e] = SIDE ? __ldg(wt + (gl + k * G) * 8 + e) : 0.f;
+    const float b0 = SIDE ? __ldg(bias) : 0.f;
     const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
     const int ph = h >> 1, pw = w >> 1;
     for (long long base = ((long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * per_warp; base < quads;
@@ -59,14 +60,16 @@ hed_side_pool_kernel(const __half* __restrict__ x, const float* __restrict__ wt,
             }
             acc[p] = s;
         }
+        if constexpr (SIDE) {
 #pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            if (o >= G) break;
+            for (int o = 1; o < 32; o <<= 1) {
+                if (o >= G) break;
 #pragma unroll
-            for (int p = 0; p < 4; ++p) acc[p] += __shfl_xor_sync(0xffffffffu, acc[p], o);
+                for (int p = 0; p < 4; ++p) acc[p] += __shfl_xor_sync(0xffffffffu, acc[p], o);
+            }
         }
         if (!valid) continue;
-        if (gl == 0) {
+        if (SIDE && gl == 0) {
 #pragma unroll
             for (int p = 0; p < 4; ++p) {
                 const int y = 2 * qy + (p >> 1), xx = 2 * qx + (p & 1);
@@ -147,7 +150,9 @@ using namespace ctrl;
 extern "C" int ctrlora_hed_side_pool_f16(const void* x, const float* weight, const float* bias, float* side, void* pooled,
                                          int batch, int h, int w, int channels, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    if (!x || !weight || !bias || !side || batch < 0 || h < 1 || w < 1 ||
+    // weight = bias = side = NULL: the pool alone, which then needs `pooled`
+    const bool with_side = weight || side;
+    if (!x || (with_side && (!weight || !bias || !side)) || (!with_side && !pooled) || batch < 0 || h < 1 || w < 1 ||
         (channels != 64 && channels != 128 && channels != 256 && channels != 512) ||
         (reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(pooled) & 15))
         return CTRLORA_ERR_ARG;
@@ -159,11 +164,18 @@ extern "C" int ctrlora_hed_side_pool_f16(const void* x, const float* weight, con
     const __half* xh = static_cast<const __half*>(x);
     __half* ph = static_cast<__half*>(pooled);
     const dim3 grid(grid_hed(quads, per_block));
+    if (!with_side) {
+        if (nv == 2)
+            return launched_hed(launch_pdl(hed_side_pool_kernel<2, false>, grid, dim3(256), (size_t)0, stream, xh, weight,
+                                           bias, side, ph, h, w, channels, quads, qh, qw));
+        return launched_hed(launch_pdl(hed_side_pool_kernel<1, false>, grid, dim3(256), (size_t)0, stream, xh, weight, bias,
+                                       side, ph, h, w, channels, quads, qh, qw));
+    }
     if (nv == 2)
-        return launched_hed(launch_pdl(hed_side_pool_kernel<2>, grid, dim3(256), (size_t)0, stream, xh, weight, bias, side,
-                                       ph, h, w, channels, quads, qh, qw));
-    return launched_hed(launch_pdl(hed_side_pool_kernel<1>, grid, dim3(256), (size_t)0, stream, xh, weight, bias, side, ph,
-                                   h, w, channels, quads, qh, qw));
+        return launched_hed(launch_pdl(hed_side_pool_kernel<2, true>, grid, dim3(256), (size_t)0, stream, xh, weight, bias,
+                                       side, ph, h, w, channels, quads, qh, qw));
+    return launched_hed(launch_pdl(hed_side_pool_kernel<1, true>, grid, dim3(256), (size_t)0, stream, xh, weight, bias,
+                                   side, ph, h, w, channels, quads, qh, qw));
 }
 
 extern "C" int ctrlora_hed_fuse(const float* const* sides, const int* side_hw, const int* const* idx,

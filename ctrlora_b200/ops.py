@@ -1164,6 +1164,111 @@ def hed_fuse(sides, tables, safe):
     return mean, u8
 
 
+def max_pool2x2(x):
+    """nn.MaxPool2d(2, 2) (floor) on fp16 [B, h, w, C] (C in {64, 128, 256, 512}) -> fp16 [B, h // 2, w // 2, C]:
+    ctrlora_hed_side_pool_f16 without its projection"""
+    _require_cuda(x)
+    assert x.dtype == torch.float16 and x.is_contiguous() and x.dim() == 4
+    b, h, w, c = x.shape
+    pooled = torch.empty((b, h // 2, w // 2, c), device=x.device, dtype=torch.float16)
+    _count()
+    check(_lib.load().ctrlora_hed_side_pool_f16(_dp(x), None, None, None, _dp(pooled), b, h, w, c, _sp()), "max_pool2x2")
+    return pooled
+
+
+# ------------------------------------------------------------------------------------------------ OpenPose annotator
+def _openpose_tabs(tables):
+    ys, yw, xs, xw = tables
+    _require_cuda(ys, yw, xs, xw)
+    assert ys.dtype == xs.dtype == torch.int32 and yw.dtype == xw.dtype == torch.float64
+    assert yw.dim() == xw.dim() == 2 and yw.shape[0] == ys.numel() and xw.shape[0] == xs.numel()
+    return [_dp(ys), _dp(yw), yw.shape[1], _dp(xs), _dp(xw), xw.shape[1]]
+
+
+def _pixel_maps(maps):
+    """fp32 pixel-major [h8, w8, ld] (one image) -> (h8, w8, ld)"""
+    assert maps.dtype == torch.float32 and maps.dim() == 3 and maps.stride(2) == 1
+    h8, w8, ld = maps.shape[0], maps.shape[1], maps.stride(1)
+    assert maps.stride(0) == w8 * ld
+    return h8, w8, ld
+
+
+def openpose_resample(maps, tables, channels):
+    """Channels 0 .. channels - 1 of one image's stride-8 maps (fp32 pixel-major [h8, w8, ld]) resampled to the image
+    through `tables` = (int32 [H] row starts, float64 [H, ty] row weights, int32 [W], float64 [W, tx]) -> fp32
+    [channels, H, W]"""
+    _require_cuda(maps)
+    h8, w8, ld = _pixel_maps(maps)
+    tab = _openpose_tabs(tables)
+    h, w = tables[0].numel(), tables[2].numel()
+    out = torch.empty((channels, h, w), device=maps.device, dtype=torch.float32)
+    _count()
+    check(_lib.load().ctrlora_openpose_resample(_dp(maps), ld, h8, w8, channels, *tab, _dp(out), h, w, _sp()),
+          "openpose_resample")
+    return out
+
+
+def openpose_smooth(heat, weights):
+    """scipy.ndimage.gaussian_filter(mode='reflect') of each fp32 [H, W] map of heat [maps, H, W], in float64, with the
+    symmetric kernel `weights` (host sequence, centre tap first) -> float64 [maps, H, W]"""
+    _require_cuda(heat)
+    assert heat.dtype == torch.float32 and heat.is_contiguous() and heat.dim() == 3
+    tmp = torch.empty(heat.shape, device=heat.device, dtype=torch.float64)
+    out = torch.empty(heat.shape, device=heat.device, dtype=torch.float64)
+    wts = (C.c_double * len(weights))(*[float(v) for v in weights])
+    _count(2)
+    check(_lib.load().ctrlora_openpose_smooth(_dp(heat), _dp(tmp), _dp(out), heat.shape[0], heat.shape[1],
+                                              heat.shape[2], C.cast(wts, C.c_void_p), len(weights) - 1, _sp()),
+          "openpose_smooth")
+    return out
+
+
+OPENPOSE_PEAK_CHUNK = 2048  # map elements per block of the peak passes (openpose_sm90.cu kPeakChunk)
+
+
+def openpose_peaks(smoothed, heat, thre, capacity=1024):
+    """The peaks of smoothed float64 [maps, H, W] (>= the four neighbours, > thre) in (map, y, x) order -> device (int32
+    x, int32 y, int32 part, fp32 score = heat at the peak), each [number of peaks].  Reads the count on the host."""
+    _require_cuda(smoothed, heat)
+    assert smoothed.dtype == torch.float64 and smoothed.is_contiguous() and smoothed.dim() == 3
+    assert heat.dtype == torch.float32 and heat.is_contiguous() and heat.shape == smoothed.shape
+    m, h, w = smoothed.shape
+    blocks = (m * h * w + OPENPOSE_PEAK_CHUNK - 1) // OPENPOSE_PEAK_CHUNK
+    ws = torch.empty(blocks + 1, device=smoothed.device, dtype=torch.int32)
+    while True:
+        pk = torch.empty((3, capacity), device=smoothed.device, dtype=torch.int32)
+        score = torch.empty(capacity, device=smoothed.device, dtype=torch.float32)
+        _count(3)
+        check(_lib.load().ctrlora_openpose_peaks(_dp(smoothed), _dp(heat), m, h, w, float(thre), _dp(ws), ws.numel(),
+                                                 _dp(pk[0]), _dp(pk[1]), _dp(pk[2]), _dp(score), capacity, _sp()),
+              "openpose_peaks")
+        n = int(ws[blocks].item())
+        if n <= capacity:
+            return pk[0, :n], pk[1, :n], pk[2, :n], score[:n]
+        capacity = n
+
+
+def openpose_limbs(paf, tables, px, py, limbs, img_h, thre):
+    """Score every candidate pair of every limb.  paf: fp32 pixel-major [h8, w8, ld] stride-8 PAF maps; tables: as for
+    openpose_resample; px, py: int32 peak coordinates (device); limbs: host rows (first pair, first A peak, nA, first B
+    peak, nB, x channel, y channel).  Returns device (float64 score, uint8 ok) per pair."""
+    _require_cuda(paf, px, py)
+    h8, w8, ld = _pixel_maps(paf)
+    tab = _openpose_tabs(tables)
+    pairs = sum(r[2] * r[4] for r in limbs)
+    score = torch.empty(pairs, device=paf.device, dtype=torch.float64)
+    ok = torch.empty(pairs, device=paf.device, dtype=torch.uint8)
+    if pairs == 0:
+        return score, ok
+    assert px.dtype == py.dtype == torch.int32
+    flat = (C.c_int * (7 * len(limbs)))(*[int(v) for r in limbs for v in r])
+    _count()
+    check(_lib.load().ctrlora_openpose_limbs(_dp(paf), ld, h8, w8, *tab, _dp(px), _dp(py), C.cast(flat, C.c_void_p),
+                                             len(limbs), pairs, int(img_h), float(thre), _dp(score), _dp(ok), _sp()),
+          "openpose_limbs")
+    return score, ok
+
+
 def set_sm_limit(limit):
     """persistent GEMM grids use at most `limit` SMs (0 = all); baked into CUDA graphs at capture"""
     check(_lib.load().ctrlora_set_sm_limit(int(limit)), "set_sm_limit")

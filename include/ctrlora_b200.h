@@ -48,7 +48,7 @@ typedef struct ctrlora_gemm_args {
     int a_b, a_h, a_w, a_c;
     long long a_ld;
     const void* w;          /* fp16 weights [n (2n for GEGLU), kh*kw, a_c], dense */
-    int kh, kw, pad;        /* 1x1 (pad 0) or 3x3 (pad 1), stride 1 */
+    int kh, kw, pad;        /* 1x1 (pad 0), 3x3 (pad 1) or 7x7 (pad 3), stride 1 */
     const void* a2;         /* optional second activation operand with the same B,H,W (1x1), or NULL */
     int a2_c;
     long long a2_ld;
@@ -438,7 +438,8 @@ int ctrlora_lineart_out_f16(const void* x, const float* weight, const float* bia
  * aligned), read once.  side: fp32 [batch, h, w] = bias[0] + sum_c weight[c] * x[.., c], fp32 accumulation in a fixed
  * order (DoubleConvBlock.projection, :32).  pooled (or NULL): fp16 [batch, h / 2, w / 2, channels], the 2x2 max of x,
  * floor sizes (the next block's max_pool2d(2, 2), :28); a max is exact, so it equals max_pool2d on x bit for bit.
- * weight: fp32 [channels], bias: fp32 [1] (device).
+ * weight: fp32 [channels], bias: fp32 [1] (device).  weight = bias = side = NULL runs the pool alone (pooled is then
+ * required): OpenPose's max pools (annotator/openpose/model.py:10-13).
  */
 int ctrlora_hed_side_pool_f16(const void* x, const float* weight, const float* bias, float* side, void* pooled, int batch,
                               int h, int w, int channels, void* stream);
@@ -451,6 +452,47 @@ int ctrlora_hed_side_pool_f16(const void* x, const float* weight, const float* b
  * (annotator/util.py:78-81), and out_u8 = (uint8)clip(edge * 255, 0, 255).  idx and frac of level 0 are unused. */
 int ctrlora_hed_fuse(const float* const* sides, const int* side_hw, const int* const* idx, const float* const* frac,
                      float* mean, unsigned char* out_u8, int batch, int h, int w, int safe, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
+ * OpenPose body estimator (annotator/openpose/body.py, Body.__call__ :24-138 with the single scale 0.5).  bodypose_model's
+ * 3x3 and 7x7 conv + ReLU pairs are ctrlora_gemm_f16 launches with relu = 1; its max pools are
+ * ctrlora_hed_side_pool_f16 with weight = side = NULL.  The host keeps the input resize, the greedy matching and the
+ * assembly of people; these run the rest.
+ *
+ * Resampling tables: the reference resizes each stride-8 map by 8 (cv2 LANCZOS4), crops the padding and resizes to the
+ * image (LANCZOS4 or INTER_AREA, annotator/openpose/util.py:10-35).  Both are linear and separable, so each axis is one
+ * banded float64 matrix built on the host: output row y reads source rows y_start[y] ... y_start[y] + ty - 1 with
+ * weights y_w[y * ty + i] (source rows < h8), and the same for columns (x_start, x_w, tx).  A resampled value is
+ * sum_i y_w_i * (sum_j x_w_j * map) in float64, rounded once to fp32.
+ *
+ * Resample: maps fp32 pixel-major [h8, w8, map_ld] (one image); out: fp32 [channels, h, w], channels 0 .. channels - 1.
+ */
+int ctrlora_openpose_resample(const float* maps, int map_ld, int h8, int w8, int channels, const int* y_start,
+                              const double* y_w, int ty, const int* x_start, const double* x_w, int tx, float* out, int h,
+                              int w, void* stream);
+/* scipy.ndimage.gaussian_filter with mode 'reflect' (body.py:84) on `maps` fp32 [h, w] maps, in float64: first along the
+ * rows (axis 0) into tmp, then along the columns into out (both float64 [maps, h, w]), each as scipy's correlate1d
+ * computes a symmetric kernel: in[0] * w[0], then + (in[-j] + in[+j]) * w[j] for j = radius ... 1.  weights: host array
+ * of radius + 1 doubles (centre first), radius <= 16. */
+int ctrlora_openpose_smooth(const float* in, double* tmp, double* out, int maps, int h, int w, const double* weights,
+                            int radius, void* stream);
+/* Peaks (body.py:86-100): element (m, y, x) of smoothed float64 [maps, h, w] is a peak when it is >= its four neighbours
+ * (0 outside the map) and > thre.  Peaks are numbered in (m, y, x) order by a prefix sum: peak id gets px, py, part
+ * (= m) and score = heat[m, y, x] (heat: the unsmoothed fp32 [maps, h, w]) when id < capacity.  ws: int32 scratch of at
+ * least ceil(maps * h * w / 2048) + 1 ints; its last used entry, ws[ceil(maps * h * w / 2048)], receives the number of
+ * peaks (which may exceed capacity: the caller then calls again with more room). */
+int ctrlora_openpose_peaks(const double* smoothed, const float* heat, int maps, int h, int w, double thre, int* ws,
+                           long long ws_ints, int* px, int* py, int* part, float* score, int capacity, void* stream);
+/* Limb scores (body.py:107-131): for each of n_limbs (<= 32) limbs, limbs[7 k ...] = {first pair index, first peak of
+ * part A, peaks of A (>= 1), first peak of part B, peaks of B (>= 1), PAF channel of x, PAF channel of y}, the pair
+ * ranges consecutive and summing to `pairs`.  Pair (i, j) of a limb (index first + i * nB + j) samples the resampled
+ * PAF (paf: fp32 pixel-major [h8, w8, paf_ld], the same tables as above) at the 10 points of np.linspace from peak A to
+ * peak B rounded half to even, and gets, in float64 as numpy computes it: score = sum(dot(PAF, unit vector)) / 10 +
+ * min(0.5 * img_h / max(0.001, norm) - 1, 0), and ok = (more than 8 of the 10 dots > thre) and score > 0. */
+int ctrlora_openpose_limbs(const float* paf, int paf_ld, int h8, int w8, const int* y_start, const double* y_w, int ty,
+                           const int* x_start, const double* x_w, int tx, const int* px, const int* py, const int* limbs,
+                           int n_limbs, long long pairs, int img_h, double thre, double* score, unsigned char* ok,
+                           void* stream);
 
 #ifdef __cplusplus
 }

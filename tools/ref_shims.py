@@ -111,3 +111,25 @@ def reference_module(name):
     install()
     import importlib
     return importlib.import_module(name)
+
+
+def install_openpose_shims():
+    """Import-only stand-ins for matplotlib and skimage, which the reference's annotator.openpose imports but whose body
+    path (Body, OpenposeDetector without hands and faces) never calls; touching them raises"""
+    def stub(name):
+        m = types.ModuleType(name)
+        m.__path__ = []
+
+        def missing(attr):
+            if attr.startswith("__"):
+                raise AttributeError(attr)
+            raise RuntimeError(f"{name}.{attr} is an import-only stand-in: the body path must not use it")
+        m.__getattr__ = missing
+        return m
+    for name in ("matplotlib", "matplotlib.pyplot", "skimage", "skimage.measure"):
+        sys.modules.setdefault(name, stub(name))
+    sys.modules["matplotlib"].__dict__["pyplot"] = sys.modules["matplotlib.pyplot"]
+    sys.modules["skimage"].__dict__["measure"] = sys.modules["skimage.measure"]
+    sys.modules["skimage.measure"].__dict__["label"] = None
+    if REFERENCE_ROOT not in sys.path:
+        sys.path.insert(0, REFERENCE_ROOT)
