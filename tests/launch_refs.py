@@ -5,8 +5,10 @@ written, computed in fp32 (fp64 when the operands are fp64) without tiling or an
 buffers among the arguments are read only for their shapes and for values the call accumulates onto (`wgrad_tn`'s
 `out` when beta != 0, `groupnorm_bwd` / `layernorm_bwd`'s dgamma / dbeta); a caller checking a call that overwrites an
 input passes that input's pre-call copy.  The semantics are those of include/ctrlora_b200.h.  Device-agnostic:
-tests/test_launch_refs_cpu.py pins them at tiny shapes on the host, tests/test_step_launches_gpu.py checks every launch of
-the benchmarked steps against them.
+tests/test_launch_refs_cpu.py pins them at tiny shapes on the host; tests/test_step_launches_gpu.py and
+tests/test_path_launches_gpu.py check every launch of the benchmarked steps, the sampling variants, the VAE encoder and
+the annotators against them (through tests/launch_shadow.py).  Gathers, pools and copies return the kernel's dtype and
+are compared bit for bit.
 """
 import contextlib
 
@@ -119,6 +121,12 @@ def gemm(a, w, *, ksize=1, bias=None, rowbias=None, rows_per_img=0, rowbias_ld=0
     if dup_out is not None:
         res.append(dup.reshape(dup_out.shape))
     return res
+
+
+def gemm_relu(a, w, **kwargs):
+    """ops.gemm_relu: gemm's result, then max(., 0) after the residual, on every segment and dup_out"""
+    y = gemm(a, w, **kwargs)
+    return [t.clamp_min(0) for t in y] if isinstance(y, list) else y.clamp_min(0)
 
 
 # ------------------------------------------------------------------------------------------------------- GroupNorm
@@ -274,3 +282,129 @@ def layernorm_bwd(x, dy, gamma, eps=1e-5, dgamma=None, dbeta=None, res=None):
     dx = xf.grad if res is None else xf.grad + _f(res).reshape(-1, c)
     return (dx.view(x.shape), None if dgamma is None else _f(dgamma) + g.grad,
             None if dbeta is None else _f(dbeta) + b.grad)
+
+
+# ------------------------------------------------------------------------------------------- gathers and small kernels
+def im2col_s2(x, pad_lo=1):
+    """ops.im2col_s2: the 3x3 stride-2 patches of x [B, H, W, C] zero-padded by pad_lo on the top / left and 1 on the
+    bottom / right, tap-major and channel-minor -> x.dtype [B, H // 2, W // 2, 9 C]"""
+    b, h, w, c = x.shape
+    xp = F.pad(_f(x).permute(0, 3, 1, 2), (pad_lo, 1, pad_lo, 1))
+    cols = F.unfold(xp, 3, stride=2)                                     # [B, C * 9, L], channel-major
+    oh, ow = (h + pad_lo - 2) // 2 + 1, (w + pad_lo - 2) // 2 + 1
+    cols = cols.view(b, c, 9, oh, ow)[:, :, :, :h // 2, :w // 2]
+    return cols.permute(0, 3, 4, 2, 1).reshape(b, h // 2, w // 2, 9 * c).to(x.dtype)
+
+
+def upsample2x(x):
+    """ops.upsample2x: nearest-neighbour x2 of x [B, H, W, C] -> [B, 2H, 2W, C]"""
+    return x.repeat_interleave(2, 1).repeat_interleave(2, 2)
+
+
+def softmax_rows(logits, scale=1.0):
+    """ops.softmax_rows: softmax(scale * logits) over the last dim, fp32"""
+    return (_f(logits) * scale).softmax(-1)
+
+
+def weighted_sum(tensors, weights, out=None):
+    """ops.weighted_sum: sum_i weights[i] tensors[i] in fp32"""
+    y = torch.zeros(tensors[0].shape, dtype=_dtype(tensors[0]), device=tensors[0].device)
+    for t, wt in zip(tensors, weights):
+        y = y + float(wt) * _f(t)
+    return y
+
+
+def gaussian_sample(moments, noise=None, scale=1.0):
+    """ops.gaussian_sample: scale (mean + exp(0.5 clamp(logvar, -30, 20)) noise), or scale mean without noise; moments
+    [B, 2Z, H, W] = mean | logvar"""
+    mean, logvar = _f(moments).chunk(2, dim=1)
+    if noise is None:
+        return scale * mean
+    return scale * (mean + torch.exp(0.5 * logvar.clamp(-30.0, 20.0)) * _f(noise))
+
+
+# ------------------------------------------------------------------------------------------------------ annotators
+TAPS7 = [(ky - 3, kx - 3) for ky in range(7) for kx in range(7)]
+
+
+def _tap_index(n, d, reflect, device):
+    """(source index, inside mask | None) of positions 0 .. n-1 shifted by d along an axis of length n: mirrored
+    without repeating the border (nn.ReflectionPad2d, |d| < n), or clamped with the mask of those inside"""
+    i = torch.arange(n, device=device) + d
+    if reflect:
+        i = i.abs()
+        return torch.where(i >= n, 2 * (n - 1) - i, i), None
+    return i.clamp(0, n - 1), (i >= 0) & (i < n)
+
+
+def _shifted(src, dy, dx, reflect):
+    """src [B, H, W, C] read at (y + dy, x + dx), reflected at the border or zero outside"""
+    _, h, w, _ = src.shape
+    iy, my = _tap_index(h, dy, reflect, src.device)
+    ix, mx = _tap_index(w, dx, reflect, src.device)
+    g = src[:, iy][:, :, ix]
+    if reflect:
+        return g
+    inside = (my[:, None] & mx[None, :])[None, :, :, None]
+    return torch.where(inside, g, torch.zeros((), dtype=g.dtype, device=g.device))
+
+
+def tap_gather(x, taps, *, reflect, k_pad, channels=None, out=None):
+    """ops.tap_gather: column t * C + c of pixel (y, x) = source channel c at (y + dy_t, x + dx_t), reflected or zero
+    outside; columns >= len(taps) * C zero.  x fp16 pixel-major [B, H, W, ld] (the first `channels`), or fp32 NCHW
+    [B, C, H, W], which the gather rounds to fp16.  -> fp16 [B, H, W, k_pad] (fp64 for an fp64 source)"""
+    src = x[..., :channels or x.shape[-1]] if x.dtype == torch.float16 else x.permute(0, 2, 3, 1)
+    b, h, w, c = src.shape
+    y = torch.zeros((b, h, w, k_pad), dtype=torch.float64 if x.dtype == torch.float64 else torch.float16,
+                    device=x.device)
+    for t, (dy, dx) in enumerate(taps):
+        y[..., t * c:(t + 1) * c] = _shifted(src, dy, dx, reflect)   # fp32 -> fp16: round to nearest even
+    return y
+
+
+def instance_norm(x, *, relu, residual=None, phases=False, eps=1e-5, out=None):
+    """ops.instance_norm: per (image, channel) biased statistics over the image's pixels, y = relu?((x - mean) /
+    sqrt(var + eps)) + residual?.  phases: x [4, B, H, W, C] holds sub-pixel phase 2 py + px, and y[b, 2m + py, 2n + px]
+    = f(x[2 py + px, b, m, n]) -> [B, 2H, 2W, C]"""
+    xf = _f(x)
+    if phases:
+        _, b, h, w, c = x.shape
+        xf = xf.view(2, 2, b, h, w, c).permute(2, 3, 0, 4, 1, 5).reshape(b, 2 * h, 2 * w, c)
+    mean = xf.mean((1, 2), keepdim=True)
+    var = ((xf - mean) ** 2).mean((1, 2), keepdim=True)
+    y = (xf - mean) / torch.sqrt(var + eps)
+    if relu:
+        y = y.clamp_min(0)
+    return y if residual is None else y + _f(residual)
+
+
+def _quantise(y):
+    """LineartDetector's uint8 map of an fp32 map (lineart_golden.quantise, on the host)"""
+    import lineart_golden
+    return torch.from_numpy(lineart_golden.quantise(y.cpu().numpy())).to(y.device)
+
+
+def lineart_out(x, weight, bias, want_u8=False):
+    """ops.lineart_out: sigmoid(bias + the 7x7 taps of x [B, H, W, C] reflected by 3, weighted by weight [49, C]
+    tap-major) -> [B, 1, H, W] (and with want_u8 the uint8 map of that reference)"""
+    xf = _f(x)
+    wf = _f(weight).to(xf.dtype)
+    y = torch.zeros(x.shape[:3], dtype=xf.dtype, device=x.device)
+    with exact_fp32():
+        for t, (dy, dx) in enumerate(TAPS7):
+            y += _shifted(xf, dy, dx, True) @ wf[t]
+    y = torch.sigmoid(y + _f(bias).to(xf.dtype)).unsqueeze(1)
+    return (y, _quantise(y[:, 0])) if want_u8 else y
+
+
+def max_pool2x2(x):
+    """ops.max_pool2x2: the 2x2 max of x [B, h, w, C], floor sizes -> x.dtype [B, h // 2, w // 2, C]"""
+    b, h, w, c = x.shape
+    return x[:, :h // 2 * 2, :w // 2 * 2].reshape(b, h // 2, 2, w // 2, 2, c).amax((2, 4))
+
+
+def hed_side_pool(x, weight, bias, pool):
+    """ops.hed_side_pool: (bias + x @ weight [B, 1, h, w], max_pool2x2(x) or None).  The projection sums in fp64, as its
+    per-kernel test does: the bound is 1e-6, a few times fp32's rounding of a sum over C products"""
+    side = (x.double() @ weight.double() + bias.double()).unsqueeze(1).to(_dtype(x))
+    return side, (max_pool2x2(x) if pool else None)

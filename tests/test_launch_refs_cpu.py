@@ -254,3 +254,150 @@ def test_exact_fp32_restores_the_tf32_flags():
     with R.exact_fp32():
         assert not torch.backends.cuda.matmul.allow_tf32 and not torch.backends.cudnn.allow_tf32
     assert (torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32) == old
+
+
+# ---------------------------------------------------------------------- the sampling variants, VAE encoder, annotators
+def test_gemm_relu_clamps_after_the_residual_and_on_every_segment():
+    M, K, N = 9, 6, 8
+    a, w, bias = _r(M, K, seed=1).half(), _r(2 * N, K, seed=2).half(), _r(2 * N, seed=3)
+    res = _r(M, 2 * N, seed=4).half()
+    plain = R.gemm(a, w, bias=bias, residual=res)
+    assert (plain < 0).any()
+    torch.testing.assert_close(R.gemm_relu(a, w, bias=bias, residual=res), plain.clamp_min(0), rtol=0, atol=0)
+    segs = R.gemm_relu(a, w, seg_outs=[torch.empty(M, N), torch.empty(M, N)], seg_width=N, transposed=(0, 0))
+    torch.testing.assert_close(torch.cat(segs, 1), R.gemm(a, w).clamp_min(0), rtol=0, atol=0)
+
+
+def _mirror(i, n):
+    return -i if i < 0 else (2 * (n - 1) - i if i >= n else i)
+
+
+@pytest.mark.parametrize("reflect", [True, False])
+@pytest.mark.parametrize("src", ["f16", "f16_ld", "f32_nchw"])
+def test_tap_gather_is_a_loop_over_pixels_and_taps(reflect, src):
+    """column t * C + c of pixel (y, x) = channel c at (y + dy_t, x + dx_t): mirrored without repeating the border, or
+    zero outside; the columns past the taps zero; an fp32 NCHW source rounded to fp16"""
+    B, H, W, C = 2, 5, 6, 3
+    taps = [(ky - 3, kx - 3) for ky in range(7) for kx in range(7)] if src == "f32_nchw" else \
+        [(0, 0), (0, 1), (1, 0), (1, 1), (-1, 2)]
+    k_pad = (len(taps) * C + 15) // 16 * 16
+    if src == "f32_nchw":
+        x = _r(B, C, H, W, seed=1) * 3
+        at = lambda b, y, xx, c: x[b, c, y, xx].half()
+        got = R.tap_gather(x, taps, reflect=reflect, k_pad=k_pad)
+    else:
+        ld = C + 5 if src == "f16_ld" else C
+        x = _r(B, H, W, ld, seed=2).half()
+        at = lambda b, y, xx, c: x[b, y, xx, c]
+        got = R.tap_gather(x, taps, reflect=reflect, k_pad=k_pad, channels=C)
+    assert got.dtype == torch.float16 and got.shape == (B, H, W, k_pad)
+    ref = torch.zeros(B, H, W, k_pad, dtype=torch.float16)
+    for b in range(B):
+        for y in range(H):
+            for xx in range(W):
+                for t, (dy, dx) in enumerate(taps):
+                    sy, sx = y + dy, xx + dx
+                    if reflect:
+                        sy, sx = _mirror(sy, H), _mirror(sx, W)
+                    elif not (0 <= sy < H and 0 <= sx < W):
+                        continue
+                    for c in range(C):
+                        ref[b, y, xx, t * C + c] = at(b, sy, sx, c)
+    assert torch.equal(got, ref)
+
+
+@pytest.mark.parametrize("mode", ["relu", "residual", "phases"])
+def test_instance_norm_against_fp64_statistics(mode):
+    """biased per (image, channel) statistics; with phases the output pixel (2m + py, 2n + px) of image b is phase
+    2 py + px's pixel (m, n)"""
+    B, H, W, C = 2, 3, 4, 5
+    phases = mode == "phases"
+    x = (_r(4, B, H, W, C, seed=1) if phases else _r(B, H, W, C, seed=1)) * 2 + 3
+    res = _r(B, H, W, C, seed=2) if mode == "residual" else None
+    got = R.instance_norm(x.half(), relu=mode != "residual", residual=None if res is None else res.half(),
+                          phases=phases)
+    xd = x.half().double()
+    if phases:
+        full = torch.zeros(B, 2 * H, 2 * W, C, dtype=D)
+        for p in range(4):
+            py, px = divmod(p, 2)
+            for b in range(B):
+                for m in range(H):
+                    for n in range(W):
+                        full[b, 2 * m + py, 2 * n + px] = xd[p, b, m, n]
+        xd = full
+    ref = torch.empty_like(xd)
+    for b in range(B):
+        for c in range(C):
+            v = xd[b, :, :, c]
+            mean = v.sum() / v.numel()
+            var = ((v - mean) ** 2).sum() / v.numel()
+            ref[b, :, :, c] = (v - mean) / torch.sqrt(var + 1e-5)
+    ref = ref + res.half().double() if res is not None else ref.clamp_min(0)
+    torch.testing.assert_close(got.double(), ref, rtol=1e-5, atol=1e-5)
+
+
+def test_lineart_out_is_a_reflect_padded_conv_and_sigmoid():
+    B, H, W, C = 2, 5, 7, 4
+    x = _r(B, H, W, C, seed=1).half()
+    conv_w, bias = _r(1, C, 7, 7, seed=2) * 0.3, _r(1, seed=3)
+    weight = conv_w[0].permute(1, 2, 0).reshape(49, C).contiguous()  # tap-major, as the Generator prepares it
+    y, u8 = R.lineart_out(x, weight, bias, want_u8=True)
+    ref = torch.sigmoid(F.conv2d(F.pad(x.float().permute(0, 3, 1, 2), (3, 3, 3, 3), mode="reflect"), conv_w, bias))
+    torch.testing.assert_close(y, ref, rtol=1e-5, atol=1e-6)
+    assert torch.equal(u8, (ref[:, 0] * 255.0).clamp(0, 255).to(torch.uint8))
+    assert torch.equal(R.lineart_out(x, weight, bias), y)
+
+
+@pytest.mark.parametrize("h,w", [(6, 8), (7, 9)])
+def test_hed_side_pool_and_max_pool(h, w):
+    B, C = 2, 16
+    x = _r(B, h, w, C, seed=1).half()
+    weight, bias = _r(C, seed=2), _r(1, seed=3)
+    side, pooled = R.hed_side_pool(x, weight, bias, pool=True)
+    ref = F.conv2d(x.double().permute(0, 3, 1, 2), weight.double().view(1, C, 1, 1), bias.double())
+    torch.testing.assert_close(side, ref.float(), rtol=1e-6, atol=1e-6)
+    want = F.max_pool2d(x.float().permute(0, 3, 1, 2), 2, 2).permute(0, 2, 3, 1).half()
+    assert torch.equal(pooled, want) and torch.equal(R.max_pool2x2(x), want)
+    assert R.hed_side_pool(x, weight, bias, pool=False)[1] is None
+
+
+@pytest.mark.parametrize("pad_lo", [0, 1])
+@pytest.mark.parametrize("h,w", [(6, 8), (7, 9)])
+def test_im2col_s2_is_a_loop_over_patches(pad_lo, h, w):
+    """out[b, r, s, t C + c] = x[b, 2r + ky - pad_lo, 2s + kx - pad_lo, c] for tap t = 3 ky + kx, zero outside"""
+    B, C = 2, 3
+    x = _r(B, h, w, C, seed=1).half()
+    got = R.im2col_s2(x, pad_lo=pad_lo)
+    ref = torch.zeros(B, h // 2, w // 2, 9 * C, dtype=torch.float16)
+    for r in range(h // 2):
+        for s in range(w // 2):
+            for t in range(9):
+                ky, kx = divmod(t, 3)
+                y, xx = 2 * r + ky - pad_lo, 2 * s + kx - pad_lo
+                if 0 <= y < h and 0 <= xx < w:
+                    ref[:, r, s, t * C:(t + 1) * C] = x[:, y, xx]
+    assert got.dtype == torch.float16 and torch.equal(got, ref)
+
+
+def test_upsample2x_is_nearest():
+    x = _r(2, 3, 5, 4, seed=1).half()
+    ref = F.interpolate(x.float().permute(0, 3, 1, 2), scale_factor=2, mode="nearest").permute(0, 2, 3, 1).half()
+    assert torch.equal(R.upsample2x(x), ref)
+
+
+def test_softmax_weighted_sum_and_gaussian_sample_formulas():
+    logits = _r(3, 7, seed=1) * 4
+    e = torch.exp(logits.double() * 0.3 - (logits.double() * 0.3).max(-1, keepdim=True).values)
+    torch.testing.assert_close(R.softmax_rows(logits, 0.3).double(), e / e.sum(-1, keepdim=True), rtol=1e-6, atol=1e-7)
+    ts, wts = [_r(2, 4, 8, seed=i).half() for i in range(3)], (0.7, 0.45, -1.25)
+    ref = 0.7 * ts[0].double() + 0.45 * ts[1].double() - 1.25 * ts[2].double()
+    torch.testing.assert_close(R.weighted_sum(ts, wts).double(), ref, rtol=1e-6, atol=1e-6)
+    mom = _r(2, 8, 3, 3, seed=5) * 3
+    mom[0, 4] = 40.0                    # log-variances beyond clamp(-30, 20) on both sides
+    mom[1, 5] = -50.0
+    noise = _r(2, 4, 3, 3, seed=6)
+    logvar = mom[:, 4:].double().clamp(-30, 20)
+    ref = 0.18215 * (mom[:, :4].double() + torch.exp(0.5 * logvar) * noise.double())
+    torch.testing.assert_close(R.gaussian_sample(mom, noise, 0.18215).double(), ref, rtol=1e-6, atol=1e-7)
+    torch.testing.assert_close(R.gaussian_sample(mom, None, 0.18215).double(), 0.18215 * mom[:, :4].double())
