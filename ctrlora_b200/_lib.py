@@ -38,7 +38,7 @@ class GroupNormArgs(C.Structure):
         ("x2", c_void_p), ("add2", c_void_p), ("add2_scale", c_float), ("c2", c_int), ("ld2", c_ll),
         ("batch", c_int), ("hw", c_int), ("groups", c_int),
         ("gamma", c_void_p), ("beta", c_void_p), ("eps", c_float), ("silu", c_int),
-        ("y", c_void_p), ("raw_out", c_void_p), ("stats_ws", c_void_p), ("stats_prezeroed", c_int),
+        ("y", c_void_p), ("raw_out", c_void_p), ("stats_ws", c_void_p),
         ("partial_ws", c_void_p), ("partial_ws_floats", c_ll), ("partial_counters", c_void_p), ("partial_counters_len", c_int),
         ("gamma_hi", c_void_p), ("beta_hi", c_void_p), ("group_b", c_int),
     ]

@@ -33,60 +33,9 @@ __device__ __forceinline__ void load8(const GnSrc& s, long long pix, int c, floa
     }
 }
 
-// stats[b][g] = {sum, sumsq} accumulated with atomics (buffer zeroed by the launcher)
-__global__ void __launch_bounds__(512)
-gn_stats_kernel(GnSrc s, int C, int HW, int groups, int pix_per_block, float* __restrict__ stats) {
-    pdl_launch_dependents();
-    pdl_wait();
-    extern __shared__ float sm[];  // [2][C]
-    float* csum = sm;
-    float* csq = sm + C;
-    const int b = blockIdx.y;
-    const int vecs = C >> 3;
-    const int lanes = blockDim.x / vecs;  // pixel lanes
-    const int vec = threadIdx.x % vecs, pl = threadIdx.x / vecs;
-    for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) sm[i] = 0.f;
-    __syncthreads();
-    const int p0 = blockIdx.x * pix_per_block;
-    const int p1 = min(HW, p0 + pix_per_block);
-    if (pl < lanes) {
-        float a[8], q[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) { a[e] = 0.f; q[e] = 0.f; }
-        // four independent 16 B loads in flight per thread: this kernel is pure latency/bandwidth
-        int p = p0 + pl;
-        for (; p + 3 * lanes < p1; p += 4 * lanes) {
-            float v[4][8];
-#pragma unroll
-            for (int u = 0; u < 4; ++u) load8(s, static_cast<long long>(b) * HW + p + u * lanes, vec * 8, v[u]);
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-#pragma unroll
-                for (int e = 0; e < 8; ++e) { a[e] += v[u][e]; q[e] += v[u][e] * v[u][e]; }
-            }
-        }
-        for (; p < p1; p += lanes) {
-            float v[8];
-            load8(s, static_cast<long long>(b) * HW + p, vec * 8, v);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) { a[e] += v[e]; q[e] += v[e] * v[e]; }
-        }
-#pragma unroll
-        for (int e = 0; e < 8; ++e) { atomicAdd(&csum[vec * 8 + e], a[e]); atomicAdd(&csq[vec * 8 + e], q[e]); }
-    }
-    __syncthreads();
-    const int cpg = C / groups;
-    for (int g = threadIdx.x; g < groups; g += blockDim.x) {
-        float su = 0.f, sq = 0.f;
-        for (int c = g * cpg; c < (g + 1) * cpg; ++c) { su += csum[c]; sq += csq[c]; }
-        atomicAdd(&stats[(b * groups + g) * 2], su);
-        atomicAdd(&stats[(b * groups + g) * 2 + 1], sq);
-    }
-}
-
-// Deterministic statistics (used whenever the caller provides a partial workspace): per-thread partials are reduced through
-// shared memory in a fixed order, every block stores its per-group partial {sum, sumsq} (no atomics), and the LAST block of
-// an image to arrive (one self-cleaning counter per image) adds the partials up in block order and writes the totals.
+// Statistics of the two-pass pair (gn_stats_det_kernel + gn_apply_kernel), deterministic: per-thread partials are reduced
+// through shared memory in a fixed order, every block stores its per-group partial {sum, sumsq} (no atomics), and the LAST
+// block of an image to arrive (one self-cleaning counter per image) adds the partials up in block order and writes the totals.
 __global__ void __launch_bounds__(512)
 gn_stats_det_kernel(GnSrc s, int C, int HW, int groups, int pix_per_block, float* __restrict__ stats, float* __restrict__ partial,
                     unsigned int* __restrict__ counters) {
@@ -227,8 +176,8 @@ gn_apply_kernel(GnSrc s, int C, int HW, int groups, int pix_per_block, const flo
 // ---- single-pass GroupNorm on a thread-block CLUSTER: the image's activations are read from HBM/L2 ONCE, parked in the
 // shared memory of the `cs` CTAs of a cluster (one cluster per image, each CTA holds HW/cs pixels x C channels, <= 200 KB),
 // the per-group {sum, sumsq} partials are exchanged through distributed shared memory, and every CTA normalises its own
-// slice out of shared memory.  Replaces the two-pass pair (gn_stats_kernel + gn_apply_kernel: two launches, the tensor read
-// twice) wherever the slice fits -- every GroupNorm of the 512x512 path except the decoder's widest concat inputs.
+// slice out of shared memory.  Replaces the two-pass pair (gn_stats_det_kernel + gn_apply_kernel: two launches, the tensor
+// read twice) wherever the slice fits -- every GroupNorm of the 512x512 path except the decoder's widest concat inputs.
 __device__ __forceinline__ float ld_dsmem_f32(const float* local_ptr, uint32_t cta_rank) {
     uint32_t remote;
     float v;
@@ -246,25 +195,22 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src, uint32
 // BULK: the slice of this CTA is one contiguous block of global memory (single source, no addend, dense rows): it is
 // brought in by the TMA engine (cp.async.bulk, 32 KiB pieces on one mbarrier) with no registers in the way; otherwise (the
 // UNet decoder's `cat([h, hs.pop() + control.pop()])` inputs) the threads gather it with 16-byte loads, four in flight each.
-// MODE 2 (no tile): slices too large for shared memory (the decoder's widest concat inputs) keep the cluster-wide statistics
-// exchange but re-read their input (from L2) for the normalisation pass -- still one launch, still deterministic.
 // Determinism: no atomics anywhere -- per-thread partials go through a shared scratch array and are summed in a fixed order,
 // CTA partials are summed in rank order -- so a forward pass is bit-reproducible.  (With fp16 storage this matters more than
 // it sounds: a 1e-7 perturbation of one statistic flips a few fp16 roundings, and every following rounding stage amplifies
-// the difference towards the rounding-noise level itself; the two-pass kernels' fp32 atomics made two identical SD1.5
+// the difference towards the rounding-noise level itself; fp32 atomics in the statistics made two identical SD1.5
 // passes differ by 1.6e-3, tools/debug_determinism.py.)
-template <int MODE>  // 0: register-gathered tile, 1: TMA bulk-staged tile, 2: no tile
+template <int MODE>  // 0: register-gathered tile, 1: TMA bulk-staged tile
 __global__ void __launch_bounds__(512, 1)
 gn_cluster_kernel(GnSrc s, int C, int HW, int groups, int ppc, int cs, const float* __restrict__ gamma_lo,
                   const float* __restrict__ beta_lo, const float* __restrict__ gamma_hi, const float* __restrict__ beta_hi,
                   int group_b, float eps, int silu, __half* __restrict__ y, __half* __restrict__ raw,
                   float* __restrict__ stats_out) {
     constexpr bool BULK = MODE == 1;
-    constexpr bool TILE = MODE != 2;
     pdl_launch_dependents();
     extern __shared__ __align__(128) uint8_t gsm[];
-    __half* tile = reinterpret_cast<__half*>(gsm);                                    // [ppc][C] (absent in MODE 2)
-    float* scratch = reinterpret_cast<float*>(gsm + (TILE ? static_cast<size_t>(ppc) * C * 2 : 0));  // [lanes][2][C]
+    __half* tile = reinterpret_cast<__half*>(gsm);                                    // [ppc][C]
+    float* scratch = reinterpret_cast<float*>(gsm + static_cast<size_t>(ppc) * C * 2);  // [lanes][2][C]
     float* csum = scratch + static_cast<size_t>(blockDim.x / (C >> 3)) * 2 * C;      // [2][C]: per-channel sum, sumsq
     float* part = csum + 2 * C;                                                       // [groups][2]: this CTA's group partials
     float* mr = part + 2 * groups;                                                    // [groups][2]: mean, rstd
@@ -318,7 +264,7 @@ gn_cluster_kernel(GnSrc s, int C, int HW, int groups, int ppc, int cs, const flo
                 __half2* h = reinterpret_cast<__half2*>(&w);
 #pragma unroll
                 for (int e = 0; e < 4; ++e) h[e] = __floats2half2_rn(v[u][2 * e], v[u][2 * e + 1]);
-                if (TILE) *reinterpret_cast<uint4*>(tile + static_cast<size_t>(p + u * lanes) * C + vec * 8) = w;
+                *reinterpret_cast<uint4*>(tile + static_cast<size_t>(p + u * lanes) * C + vec * 8) = w;
 #pragma unroll
                 for (int e = 0; e < 8; ++e) { a[e] += v[u][e]; q[e] += v[u][e] * v[u][e]; }
             }
@@ -330,7 +276,7 @@ gn_cluster_kernel(GnSrc s, int C, int HW, int groups, int ppc, int cs, const flo
             __half2* h = reinterpret_cast<__half2*>(&w);
 #pragma unroll
             for (int e = 0; e < 4; ++e) h[e] = __floats2half2_rn(v[2 * e], v[2 * e + 1]);
-            if (TILE) *reinterpret_cast<uint4*>(tile + static_cast<size_t>(p) * C + vec * 8) = w;
+            *reinterpret_cast<uint4*>(tile + static_cast<size_t>(p) * C + vec * 8) = w;
 #pragma unroll
             for (int e = 0; e < 8; ++e) { a[e] += v[e]; q[e] += v[e] * v[e]; }
         }
@@ -393,16 +339,7 @@ gn_cluster_kernel(GnSrc s, int C, int HW, int groups, int ppc, int cs, const flo
     }
     for (int p = pl; p < npix; p += lanes) {
         const long long pix = static_cast<long long>(b) * HW + p0 + p;
-        uint4 w;
-        if (TILE) {
-            w = *reinterpret_cast<const uint4*>(tile + static_cast<size_t>(p) * C + vec * 8);
-        } else {  // second read of the input (L2-resident: this CTA just streamed it); same fp16 rounding of the sum as the tile
-            float v[8];
-            load8(s, pix, vec * 8, v);
-            __half2* hw = reinterpret_cast<__half2*>(&w);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) hw[e] = __floats2half2_rn(v[2 * e], v[2 * e + 1]);
-        }
+        const uint4 w = *reinterpret_cast<const uint4*>(tile + static_cast<size_t>(p) * C + vec * 8);
         if (raw) *reinterpret_cast<uint4*>(raw + pix * C + vec * 8) = w;
         const __half2* h = reinterpret_cast<const __half2*>(&w);
         uint4 o;
@@ -498,32 +435,31 @@ extern "C" int ctrlora_groupnorm_f16(const ctrlora_groupnorm_args* a, void* stre
     s.x2 = reinterpret_cast<const __half*>(a->x2); s.add2 = reinterpret_cast<const __half*>(a->add2); s.s2 = a->add2_scale;
     s.c2 = a->x2 ? a->c2 : 0; s.ld2 = a->ld2;
     const int HW = a->hw, B = a->batch;
-    // ---- single-pass cluster kernel where one image's slice per CTA fits in shared memory (CTRLORA_GN_CLUSTER=0 disables)
+    // two-pass geometry: ~4 blocks per SM in total, at least 8 pixels per block; a grouped launch splits each image as a
+    // call over the larger group would, so that its statistics are summed in the same order
+    const int B_split = a->group_b > 0 ? (a->group_b > B - a->group_b ? a->group_b : B - a->group_b) : B;
+    int chunks = (592 + B_split - 1) / B_split;
+    int ppb = (HW + chunks - 1) / chunks;
+    if (ppb < 8) ppb = 8;
+    chunks = (HW + ppb - 1) / ppb;
+    if (!a->partial_ws || !a->partial_counters || B > a->partial_counters_len ||
+        static_cast<long long>(B) * chunks * a->groups * 2 > a->partial_ws_floats)
+        return CTRLORA_ERR_ARG;
+    // ---- single-pass cluster kernel where one image's slice fits the shared memory of 1, 2, 4 or 8 CTAs
     {
-        static int cl_env = -1;
-        if (cl_env < 0) {
-            const char* e = getenv("CTRLORA_GN_CLUSTER");
-            cl_env = (e && e[0] == '0') ? 0 : (e && e[0] == '2') ? 2 : 1;
-        }
         const int vecs = C / 8;
         const int lanes_max = vecs <= 512 ? 512 / vecs : 0;
         auto fixed_for = [&](int lanes) {  // scratch [lanes][2C] + csum [2C] + part/mr [4 groups] + the staging mbarrier
             return static_cast<size_t>((lanes + 1) * 2 * C + 4 * a->groups) * sizeof(float) + 16;
         };
         const size_t budget = 216 * 1024;
-        int cs = 0, mode = 0;
-        static int cl_max = -1;  // largest cluster used: 16-CTA clusters measured slower than the two-pass pair (profiles/README.md)
-        if (cl_max < 0) {
-            const char* e = getenv("CTRLORA_GN_CLUSTER_MAX");
-            cl_max = e ? atoi(e) : 8;
-        }
-        for (int c = 1; c <= cl_max && c <= 16 && cl_env && lanes_max > 0; c *= 2) {
+        int cs = 0;
+        for (int c = 1; c <= 8 && lanes_max > 0; c *= 2) {  // 16-CTA clusters measured slower than the two-pass pair
             const int ppc = (HW + c - 1) / c;
             if (c > HW) break;
             const int lanes = lanes_max < ppc ? lanes_max : ppc;
             if (static_cast<size_t>(ppc) * C * 2 + fixed_for(lanes) <= budget) { cs = c; break; }
         }
-        if (cs == 0 && cl_env == 2 && lanes_max > 0 && HW >= 16) { cs = 16; mode = 2; }  // CTRLORA_GN_CLUSTER=2: statistics-only cluster
         if (cs > 0) {
             const int ppc = (HW + cs - 1) / cs;
             int lanes = lanes_max;
@@ -532,38 +468,18 @@ extern "C" int ctrlora_groupnorm_f16(const ctrlora_groupnorm_args* a, void* stre
             const size_t fixed = fixed_for(lanes);
             const int threads = vecs * lanes;  // exact: the scratch layout is indexed by blockDim.x / vecs
             // contiguous slice -> TMA bulk staging (needs 16-byte aligned base, dense rows)
-            if (mode != 2 && !a->x2 && !a->add1 && a->ld1 == C && (reinterpret_cast<uintptr_t>(a->x1) & 15) == 0) mode = 1;
-            const size_t smem = (mode == 2 ? 0 : static_cast<size_t>(ppc) * C * 2) + fixed;
+            const bool bulk = !a->x2 && !a->add1 && a->ld1 == C && (reinterpret_cast<uintptr_t>(a->x1) & 15) == 0;
+            const size_t smem = static_cast<size_t>(ppc) * C * 2 + fixed;
             static bool attr = false;
-            static int ok16 = -1;  // can a 16-CTA cluster of this kernel be co-scheduled on this part at all?
             if (!attr) {
                 if (cudaFuncSetAttribute(gn_cluster_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess ||
                     cudaFuncSetAttribute(gn_cluster_kernel<0>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess ||
                     cudaFuncSetAttribute(gn_cluster_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess ||
-                    cudaFuncSetAttribute(gn_cluster_kernel<1>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess ||
-                    cudaFuncSetAttribute(gn_cluster_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess ||
-                    cudaFuncSetAttribute(gn_cluster_kernel<2>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess)
+                    cudaFuncSetAttribute(gn_cluster_kernel<1>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess)
                     return CTRLORA_ERR_CUDA;
                 attr = true;
             }
-            if (cs == 16 && ok16 < 0) {
-                cudaLaunchConfig_t qc;
-                memset(&qc, 0, sizeof(qc));
-                qc.gridDim = dim3(16, 1);
-                qc.blockDim = dim3(512);
-                qc.dynamicSmemBytes = 216 * 1024;
-                cudaLaunchAttribute qa[1];
-                qa[0].id = cudaLaunchAttributeClusterDimension;
-                qa[0].val.clusterDim.x = 16; qa[0].val.clusterDim.y = 1; qa[0].val.clusterDim.z = 1;
-                qc.attrs = qa;
-                qc.numAttrs = 1;
-                int nclusters = 0;
-                ok16 = (cudaOccupancyMaxActiveClusters(&nclusters, gn_cluster_kernel<0>, &qc) == cudaSuccess && nclusters >= 1) ? 1 : 0;
-                (void)cudaGetLastError();
-            }
-            if (cs == 16 && ok16 == 0) goto two_pass;
-            const cudaError_t rc = launch_cluster_pdl(mode == 1 ? gn_cluster_kernel<1> : mode == 2 ? gn_cluster_kernel<2> : gn_cluster_kernel<0>,
-                                                      dim3(cs, B),
+            const cudaError_t rc = launch_cluster_pdl(bulk ? gn_cluster_kernel<1> : gn_cluster_kernel<0>, dim3(cs, B),
                                                       dim3(threads), smem, stream, (unsigned)cs, s, C, HW, (int)a->groups, ppc, cs,
                                                       a->gamma, a->beta, gamma_hi, beta_hi, (int)a->group_b, a->eps,
                                                       (int)a->silu, reinterpret_cast<__half*>(a->y),
@@ -572,33 +488,18 @@ extern "C" int ctrlora_groupnorm_f16(const ctrlora_groupnorm_args* a, void* stre
             (void)cudaGetLastError();  // fall through to the two-pass pair
         }
     }
-two_pass:
-    // ~4 blocks per SM in total, at least 8 pixels per block; a grouped launch splits each image as a call over the
-    // larger group would, so that its statistics are summed in the same order
-    const int B_split = a->group_b > 0 ? (a->group_b > B - a->group_b ? a->group_b : B - a->group_b) : B;
-    int chunks = (592 + B_split - 1) / B_split;
-    int ppb = (HW + chunks - 1) / chunks;
-    if (ppb < 8) ppb = 8;
-    chunks = (HW + ppb - 1) / ppb;
     dim3 grid(chunks, B);
     const int vecs = C / 8;
     const int lanes = vecs >= 256 ? 1 : 256 / vecs;
     const int threads = vecs * lanes;  // every thread owns one 8-channel vector of one pixel lane
-    const bool det = a->partial_ws && a->partial_counters && B <= a->partial_counters_len &&
-                     static_cast<long long>(B) * chunks * a->groups * 2 <= a->partial_ws_floats;
-    if (!det && !a->stats_prezeroed &&
-        cudaMemsetAsync(a->stats_ws, 0, sizeof(float) * 2 * B * a->groups, stream) != cudaSuccess)
-        return CTRLORA_ERR_CUDA;
-    // after a memset node the stats kernel is a plain launch; with a pre-zeroed workspace it chains programmatically
-    if (det)
-        launch_pdl(gn_stats_det_kernel, grid, dim3(threads), (size_t)((lanes + 1) * 2 * C * sizeof(float)), stream, s, C, HW,
-                   (int)a->groups, ppb, reinterpret_cast<float*>(a->stats_ws), a->partial_ws, a->partial_counters);
-    else if (a->stats_prezeroed)
-        launch_pdl(gn_stats_kernel, grid, dim3(threads), (size_t)(2 * C * sizeof(float)), stream, s, C, HW, (int)a->groups, ppb,
-                   reinterpret_cast<float*>(a->stats_ws));
-    else
-        gn_stats_kernel<<<grid, threads, 2 * C * sizeof(float), stream>>>(s, C, HW, a->groups, ppb,
-                                                                     reinterpret_cast<float*>(a->stats_ws));
+    static bool det_attr = false;  // (lanes + 1) * 2 * C floats: up to 64 KB (C = 4096, one lane), over the default 48 KB
+    if (!det_attr) {
+        if (cudaFuncSetAttribute(gn_stats_det_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024) != cudaSuccess)
+            return CTRLORA_ERR_CUDA;
+        det_attr = true;
+    }
+    launch_pdl(gn_stats_det_kernel, grid, dim3(threads), (size_t)((lanes + 1) * 2 * C * sizeof(float)), stream, s, C, HW,
+               (int)a->groups, ppb, reinterpret_cast<float*>(a->stats_ws), a->partial_ws, a->partial_counters);
     launch_pdl(gn_apply_kernel, grid, dim3(threads), (size_t)0, stream, s, C, HW, (int)a->groups, ppb,
                reinterpret_cast<const float*>(a->stats_ws), a->gamma, a->beta, gamma_hi, beta_hi, (int)a->group_b, a->eps,
                (int)a->silu, reinterpret_cast<__half*>(a->y), reinterpret_cast<__half*>(a->raw_out));
@@ -647,76 +548,7 @@ __device__ __forceinline__ void load8h(const __half* p, float* v) {
     for (int e = 0; e < 4; ++e) { float2 f = __half22float2(h[e]); v[2 * e] = f.x; v[2 * e + 1] = f.y; }
 }
 
-// bstats[b][g] = {sum dz*gamma, sum dz*gamma*xhat}; optional dgamma/dbeta accumulation (fp32 atomics, one per channel per block)
-__global__ void __launch_bounds__(512)
-gn_bwd_stats_kernel(GnSrc s, const __half* __restrict__ dy, int C, int HW, int groups, int pix_per_block,
-                    const float* __restrict__ fstats, const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
-                    int silu, float* __restrict__ bstats, float* __restrict__ dgamma, float* __restrict__ dbeta) {
-    pdl_launch_dependents();
-    pdl_wait();
-    extern __shared__ float sm[];  // [2][C]: sum dz, sum dz*xhat per channel
-    float* c_dz = sm;
-    float* c_dzx = sm + C;
-    const int b = blockIdx.y;
-    const int vecs = C >> 3, lanes = blockDim.x / vecs;
-    const int vec = threadIdx.x % vecs, pl = threadIdx.x / vecs;
-    for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) sm[i] = 0.f;
-    __syncthreads();
-    const int cpg = C / groups;
-    const float inv_n = 1.0f / (static_cast<float>(cpg) * HW);
-    if (pl < lanes) {
-        float mu[8], rs[8], ga[8], be[8], a[8], q[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-            const int c = vec * 8 + e, g = c / cpg;
-            const float mean = fstats[(b * groups + g) * 2] * inv_n;
-            const float var = fmaxf(fstats[(b * groups + g) * 2 + 1] * inv_n - mean * mean, 0.f);
-            mu[e] = mean; rs[e] = rsqrtf(var + eps); ga[e] = gamma[c]; be[e] = beta[c]; a[e] = 0.f; q[e] = 0.f;
-        }
-        const int p0 = blockIdx.x * pix_per_block, p1 = min(HW, p0 + pix_per_block);
-        auto accum = [&](const float* x, const float* d) {
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-                const float xh = (x[e] - mu[e]) * rs[e];
-                const float dz = silu ? d[e] * dsilu_f(xh * ga[e] + be[e]) : d[e];
-                a[e] += dz; q[e] += dz * xh;
-            }
-        };
-        int p = p0 + pl;
-        for (; p + lanes < p1; p += 2 * lanes) {  // two pixels (four 16-byte loads) in flight per thread
-            const long long pix = static_cast<long long>(b) * HW + p;
-            float x0[8], d0[8], x1[8], d1[8];
-            load8(s, pix, vec * 8, x0);
-            load8h(dy + pix * C + vec * 8, d0);
-            load8(s, pix + lanes, vec * 8, x1);
-            load8h(dy + (pix + lanes) * C + vec * 8, d1);
-            accum(x0, d0);
-            accum(x1, d1);
-        }
-        for (; p < p1; p += lanes) {
-            const long long pix = static_cast<long long>(b) * HW + p;
-            float x[8], d[8];
-            load8(s, pix, vec * 8, x);
-            load8h(dy + pix * C + vec * 8, d);
-            accum(x, d);
-        }
-#pragma unroll
-        for (int e = 0; e < 8; ++e) { atomicAdd(&c_dz[vec * 8 + e], a[e]); atomicAdd(&c_dzx[vec * 8 + e], q[e]); }
-    }
-    __syncthreads();
-    for (int g = threadIdx.x; g < groups; g += blockDim.x) {
-        float g1 = 0.f, g2 = 0.f;
-        for (int c = g * cpg; c < (g + 1) * cpg; ++c) { g1 += gamma[c] * c_dz[c]; g2 += gamma[c] * c_dzx[c]; }
-        atomicAdd(&bstats[(b * groups + g) * 2], g1);
-        atomicAdd(&bstats[(b * groups + g) * 2 + 1], g2);
-    }
-    if (dgamma) {
-        for (int c = threadIdx.x; c < C; c += blockDim.x) { atomicAdd(&dgamma[c], c_dzx[c]); atomicAdd(&dbeta[c], c_dz[c]); }
-    }
-}
-
-// Deterministic form of gn_bwd_stats_kernel (used whenever the caller provides a partial workspace), the backward twin of
-// gn_stats_det_kernel: per-lane channel sums reduced through shared memory in lane order, one per-group partial per block
+// bstats[b][g] = {sum dz*gamma, sum dz*gamma*xhat}, the backward twin of gn_stats_det_kernel: per-lane channel sums reduced through shared memory in lane order, one per-group partial per block
 // (no atomics), and the last block of an image to arrive adds the partials up in block order.  bstats -- and with them every
 // dx the apply kernel writes -- are then bit-reproducible; dgamma/dbeta still accumulate with fp32 atomics (one per
 // channel per block): they feed only the fp32 gradient buffer, never an fp16 activation.
@@ -1015,25 +847,19 @@ extern "C" int ctrlora_groupnorm_bwd_f16(const ctrlora_groupnorm_args* a, const 
     const int vecs = C / 8;
     const int lanes = vecs >= 256 ? 1 : 256 / vecs;
     const int threads = vecs * lanes;
-    const bool det = a->partial_ws && a->partial_counters && B <= a->partial_counters_len &&
-                     static_cast<long long>(B) * chunks * a->groups * 2 <= a->partial_ws_floats &&
-                     (lanes + 1) * 2 * C * sizeof(float) <= 48 * 1024;
-    if (!det && !a->stats_prezeroed &&
-        cudaMemsetAsync(a->stats_ws, 0, sizeof(float) * 2 * B * a->groups, stream) != cudaSuccess)
-        return CTRLORA_ERR_CUDA;
-    if (det)
-        launch_pdl(gn_bwd_stats_det_kernel, grid, dim3(threads), (size_t)((lanes + 1) * 2 * C * sizeof(float)), stream, s,
-                   reinterpret_cast<const __half*>(dy), C, HW, (int)a->groups, ppb, reinterpret_cast<const float*>(fwd_stats),
-                   a->gamma, a->beta, a->eps, (int)a->silu, reinterpret_cast<float*>(a->stats_ws), dgamma, dbeta,
-                   a->partial_ws, a->partial_counters);
-    else if (a->stats_prezeroed)
-        launch_pdl(gn_bwd_stats_kernel, grid, dim3(threads), (size_t)(2 * C * sizeof(float)), stream, s,
-                   reinterpret_cast<const __half*>(dy), C, HW, (int)a->groups, ppb, reinterpret_cast<const float*>(fwd_stats),
-                   a->gamma, a->beta, a->eps, (int)a->silu, reinterpret_cast<float*>(a->stats_ws), dgamma, dbeta);
-    else
-        gn_bwd_stats_kernel<<<grid, threads, 2 * C * sizeof(float), stream>>>(
-            s, reinterpret_cast<const __half*>(dy), C, HW, a->groups, ppb, reinterpret_cast<const float*>(fwd_stats), a->gamma,
-            a->beta, a->eps, a->silu, reinterpret_cast<float*>(a->stats_ws), dgamma, dbeta);
+    if (!a->partial_ws || !a->partial_counters || B > a->partial_counters_len ||
+        static_cast<long long>(B) * chunks * a->groups * 2 > a->partial_ws_floats)
+        return CTRLORA_ERR_ARG;
+    static bool attr = false;  // (lanes + 1) * 2 * C floats: up to 64 KB (C = 4096, one lane), over the default 48 KB
+    if (!attr) {
+        if (cudaFuncSetAttribute(gn_bwd_stats_det_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024) != cudaSuccess)
+            return CTRLORA_ERR_CUDA;
+        attr = true;
+    }
+    launch_pdl(gn_bwd_stats_det_kernel, grid, dim3(threads), (size_t)((lanes + 1) * 2 * C * sizeof(float)), stream, s,
+               reinterpret_cast<const __half*>(dy), C, HW, (int)a->groups, ppb, reinterpret_cast<const float*>(fwd_stats),
+               a->gamma, a->beta, a->eps, (int)a->silu, reinterpret_cast<float*>(a->stats_ws), dgamma, dbeta,
+               a->partial_ws, a->partial_counters);
     launch_pdl(gn_bwd_apply_kernel, grid, dim3(threads), (size_t)0, stream, s, reinterpret_cast<const __half*>(dy), C, HW,
                (int)a->groups, ppb, reinterpret_cast<const float*>(fwd_stats), reinterpret_cast<const float*>(a->stats_ws),
                a->gamma, a->beta, a->eps, (int)a->silu, reinterpret_cast<__half*>(dx1), ldd1, dx1_scale,

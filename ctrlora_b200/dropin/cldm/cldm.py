@@ -373,7 +373,6 @@ class ControlLDM(LatentDiffusion):
     def scaled_control(self, control):
         return [Scaled(c, s) for c, s in zip(control, self.control_scales)]
 
-    @ops.with_stats_arena
     def apply_model(self, x_noisy, t, cond, *args, **kwargs):
         assert isinstance(cond, dict)
         diffusion_model = self.model.diffusion_model

@@ -5,8 +5,6 @@ import os
 
 import torch
 
-from ctrlora_b200 import ops
-
 from cldm.cldm import ControlLDM, ControlNet
 from cldm.ddim_hacked import DDIMSampler
 from cldm.lora import LoRALinearLayer
@@ -60,7 +58,6 @@ class ControlFinetuneLDM(ControlLDM):
         shape = (self.channels, h // 8, w // 8) if c != self.channels else (self.channels, h, w)
         return sampler.sample(ddim_steps, batch_size, shape, cond, verbose=False, **kwargs)
 
-    @ops.with_stats_arena
     def apply_model(self, x_noisy, t, cond, *args, **kwargs):
         assert isinstance(cond, dict)
         diffusion_model = self.model.diffusion_model

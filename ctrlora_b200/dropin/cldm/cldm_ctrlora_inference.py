@@ -177,7 +177,6 @@ class ControlInferenceLDM(ControlLDM):
         shape = (self.channels, h // 8, w // 8) if c != self.channels else (self.channels, h, w)
         return sampler.sample(ddim_steps, batch_size, shape, cond, verbose=False, **kwargs)
 
-    @ops.with_stats_arena
     def apply_model(self, x_noisy, t, conds, *args, **kwargs):
         if isinstance(conds, dict):
             conds = [conds]

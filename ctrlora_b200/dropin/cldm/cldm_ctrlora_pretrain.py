@@ -3,8 +3,6 @@ task in `loras_dict`, re-pointed per mini-batch by `switch_lora(task)`."""
 import torch
 import torch.nn as nn
 
-from ctrlora_b200 import ops
-
 from cldm.cldm import ControlLDM, ControlNet
 from cldm.ddim_hacked import DDIMSampler
 from cldm.lora import LoRACompatibleLinear, LoRALinearLayer
@@ -49,7 +47,6 @@ class ControlPretrainLDM(ControlLDM):
         shape = (self.channels, h // 8, w // 8) if c != self.channels else (self.channels, h, w)
         return sampler.sample(ddim_steps, batch_size, shape, cond, verbose=False, **kwargs)
 
-    @ops.with_stats_arena
     def apply_model(self, x_noisy, t, cond, *args, **kwargs):
         assert isinstance(cond, dict)
         diffusion_model = self.model.diffusion_model

@@ -11,7 +11,6 @@ from ctrlora_b200.runtime import Scaled
 
 
 class ControlInferenceLDM(_ControlInferenceLDM):
-    @ops.with_stats_arena
     def apply_model(self, x_noisy, t, conds, *args, **kwargs):
         if isinstance(conds, dict):
             conds = [conds]

@@ -281,66 +281,6 @@ def _sp():
     return torch.cuda.current_stream().cuda_stream
 
 
-# ---- GroupNorm statistics arena: ONE memset per step instead of one per GroupNorm ---------------------------------------
-# `stats_arena_begin()` (called by the sampler / trainer at the top of a step, also inside graph capture) zeroes a flat
-# fp32 buffer; every groupnorm / groupnorm_bwd call of the step then takes its {sum, sumsq} workspace from it and tells the
-# library the workspace is already zero, which removes the memset node in front of each statistics kernel and lets that
-# kernel chain programmatically (PDL) onto its predecessor.  Outside a step (tests, ad-hoc calls) nothing changes.
-_ARENA = {}  # device index -> [tensor, offset, active]
-ARENA_FLOATS = 1 << 20
-
-
-def stats_arena_begin(device=None):
-    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-    key = dev.index if dev.index is not None else torch.cuda.current_device()
-    ent = _ARENA.get(key)
-    if ent is None:
-        if torch.cuda.is_current_stream_capturing():
-            return  # never allocate the arena inside a capture (it would live in that graph's pool); plain path instead
-        ent = _ARENA[key] = [torch.zeros(ARENA_FLOATS, device=dev, dtype=torch.float32), 0, True]
-    ent[0].zero_()
-    ent[1], ent[2] = 0, True
-    _count()
-
-
-def stats_arena_end(device=None):
-    key = torch.cuda.current_device() if device is None else (torch.device(device).index or 0)
-    if key in _ARENA:
-        _ARENA[key][2] = False
-
-
-def with_stats_arena(fn):
-    """Decorator for a step-level entry point (apply_model): GroupNorm statistics come from the per-step arena."""
-    import functools
-
-    @functools.wraps(fn)
-    def wrapped(self, x, *args, **kwargs):
-        nested = False
-        if torch.is_tensor(x) and x.is_cuda:
-            key = x.device.index if x.device.index is not None else torch.cuda.current_device()
-            nested = key in _ARENA and _ARENA[key][2]
-            if not nested:
-                stats_arena_begin(x.device)
-        try:
-            return fn(self, x, *args, **kwargs)
-        finally:
-            if torch.is_tensor(x) and x.is_cuda and not nested:
-                stats_arena_end(x.device)
-    return wrapped
-
-
-def _stats_take(device, n):
-    """(workspace, prezeroed) for n floats"""
-    key = device.index if device.index is not None else torch.cuda.current_device()
-    ent = _ARENA.get(key)
-    n_al = (n + 31) // 32 * 32
-    if ent is not None and ent[2] and ent[1] + n_al <= ARENA_FLOATS:
-        ws = ent[0][ent[1]:ent[1] + n]
-        ent[1] += n_al
-        return ws, 1
-    return torch.empty(n, device=device, dtype=torch.float32), 0
-
-
 _GN_PARTIAL = {}  # device index -> (fp32 scratch for per-block partial statistics, uint32 self-cleaning arrival counters)
 GN_PARTIAL_FLOATS = 1 << 19
 GN_PARTIAL_COUNTERS = 256
@@ -349,6 +289,9 @@ GN_PARTIAL_COUNTERS = 256
 def _gn_partial_buffers(device):
     key = device.index if device.index is not None else torch.cuda.current_device()
     if key not in _GN_PARTIAL:
+        if torch.cuda.is_current_stream_capturing():  # it would live in that graph's private pool
+            raise _lib.CtrloraError("the GroupNorm partial-statistics scratch is allocated on the first call on a device; "
+                                    "make one un-captured GroupNorm call before capturing a graph")
         _GN_PARTIAL[key] = (torch.empty(GN_PARTIAL_FLOATS, device=device, dtype=torch.float32),
                             torch.zeros(GN_PARTIAL_COUNTERS, device=device, dtype=torch.int32))
     return _GN_PARTIAL[key]
@@ -367,15 +310,14 @@ def _gn_args(x1, gamma, beta, eps, silu, add1, add1_scale, x2, add2, add2_scale,
     a.x2, a.add2, a.add2_scale, a.c2, a.ld2 = _dp(x2), _dp(add2), float(add2_scale), c2, ld2
     a.batch, a.hw, a.groups = b, h * w, groups
     a.gamma, a.beta, a.eps, a.silu = _dp(gamma), _dp(beta), float(eps), int(silu)
-    if not torch.cuda.is_current_stream_capturing() or x1.device.index in _GN_PARTIAL or torch.cuda.current_device() in _GN_PARTIAL:
-        pws, pcnt = _gn_partial_buffers(x1.device)  # never first allocated inside a capture
-        a.partial_ws, a.partial_ws_floats = _dp(pws), GN_PARTIAL_FLOATS
-        a.partial_counters, a.partial_counters_len = _dp(pcnt), GN_PARTIAL_COUNTERS
+    pws, pcnt = _gn_partial_buffers(x1.device)
+    a.partial_ws, a.partial_ws_floats = _dp(pws), GN_PARTIAL_FLOATS
+    a.partial_counters, a.partial_counters_len = _dp(pcnt), GN_PARTIAL_COUNTERS
     return a, (b, h, w, c1, c2)
 
 
 def groupnorm(x1, gamma, beta, eps, silu, *, add1=None, add1_scale=1.0, x2=None, add2=None, add2_scale=1.0,
-              groups=32, want_raw=False, stats_ws=None, want_stats=False, out=None, gamma_hi=None, beta_hi=None):
+              groups=32, want_raw=False, want_stats=False, out=None, gamma_hi=None, beta_hi=None):
     """GroupNorm(+SiLU) over [x1 (+s1*add1) | x2 (+s2*add2)], pixel-major fp16 [B,H,W,C*]; returns y (and raw concat).
     gamma_hi / beta_hi: the affine parameters of the upper half of the batch (two networks' layers in one launch)."""
     _require_cuda(x1, x2, add1, add2)
@@ -387,10 +329,8 @@ def groupnorm(x1, gamma, beta, eps, silu, *, add1=None, add1_scale=1.0, x2=None,
     y = torch.empty((b, h, w, ctot), device=x1.device, dtype=torch.float16) if out is None else out
     assert y.shape == (b, h, w, ctot) and y.is_contiguous() and y.dtype == torch.float16
     raw = torch.empty_like(y) if want_raw else None
-    prezeroed = 0
-    if stats_ws is None:
-        stats_ws, prezeroed = _stats_take(x1.device, b * groups * 2)
-    a.stats_ws, a.stats_prezeroed = _dp(stats_ws), prezeroed
+    stats_ws = torch.empty(b * groups * 2, device=x1.device, dtype=torch.float32)
+    a.stats_ws = _dp(stats_ws)
     assert gamma.dtype == torch.float32 and beta.dtype == torch.float32 and gamma.numel() == ctot
     if gamma_hi is not None:
         assert b % 2 == 0 and gamma_hi.numel() == ctot and beta_hi.numel() == ctot
@@ -769,9 +709,9 @@ def groupnorm_bwd(dy, fwd_stats, x1, gamma, beta, eps, silu, *, add1=None, add1_
     dgamma/dbeta (fp32 [C]) are accumulated into when given."""
     _require_cuda(dy, x1)
     assert dy.dtype == torch.float16 and dy.is_contiguous()
-    ws, prezeroed = _stats_take(dy.device, fwd_stats.numel())
+    ws = torch.empty(fwd_stats.numel(), device=dy.device, dtype=torch.float32)
     a, (b, h, w, c1, c2) = _gn_args(x1, gamma, beta, eps, silu, add1, add1_scale, x2, add2, add2_scale, groups)
-    a.stats_ws, a.stats_prezeroed = _dp(ws), prezeroed
+    a.stats_ws = _dp(ws)
     dx1 = torch.empty((b, h, w, c1), device=dy.device, dtype=torch.float16)
     dx2 = torch.empty((b, h, w, c2), device=dy.device, dtype=torch.float16) if (want_dx2 and c2) else None
     _count(2)

@@ -778,18 +778,14 @@ class FinetuneTrainer:
             self.G.zero()
             self.overflow_flag.zero_()
             self._scale_used = self._scale_for(x0.numel())
-        ops.stats_arena_begin(x0.device)  # one memset for all GroupNorm forward / backward statistics of the step
-        try:
-            x_noisy = m.q_sample(x_start=x0, t=t, noise=noise)
-            control, cn_saved = controlnet_fwd(self.cn, hint_latent, t, context)
-            eps, un_saved = unet_fwd(self.unet, x_noisy, t, context, control, m.control_scales, m.only_mid_control)
-            loss, d_eps = ops.mse_loss_grad(eps, noise, c_pad=un_saved["n_pad"], grad_scale=self._scale_used)
-            d_ctrl = unet_bwd(self.unet, un_saved, d_eps)
-            if m.only_mid_control:
-                d_ctrl = [d if d is not None else torch.zeros_like(c) for d, c in zip(d_ctrl, control)]
-            controlnet_bwd(self.cn, cn_saved, d_ctrl, self.G, on_stage=self._on_stage)
-        finally:
-            ops.stats_arena_end(x0.device)
+        x_noisy = m.q_sample(x_start=x0, t=t, noise=noise)
+        control, cn_saved = controlnet_fwd(self.cn, hint_latent, t, context)
+        eps, un_saved = unet_fwd(self.unet, x_noisy, t, context, control, m.control_scales, m.only_mid_control)
+        loss, d_eps = ops.mse_loss_grad(eps, noise, c_pad=un_saved["n_pad"], grad_scale=self._scale_used)
+        d_ctrl = unet_bwd(self.unet, un_saved, d_eps)
+        if m.only_mid_control:
+            d_ctrl = [d if d is not None else torch.zeros_like(c) for d, c in zip(d_ctrl, control)]
+        controlnet_bwd(self.cn, cn_saved, d_ctrl, self.G, on_stage=self._on_stage)
         self.last_eps = eps
         return loss
 

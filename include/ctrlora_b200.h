@@ -16,7 +16,7 @@
 extern "C" {
 #endif
 
-#define CTRLORA_ABI_VERSION 2
+#define CTRLORA_ABI_VERSION 3
 
 /* status codes */
 #define CTRLORA_STATUS_OK 0
@@ -114,12 +114,12 @@ typedef struct ctrlora_groupnorm_args {
     void* y;          /* fp16 [batch*hw, c1+c2] */
     void* raw_out;    /* optional fp16 [batch*hw, c1+c2]: the concatenated (and summed) input itself, or NULL */
     void* stats_ws;   /* fp32 workspace [batch * groups * 2] */
-    int stats_prezeroed; /* 1: the caller guarantees stats_ws is zero on entry (e.g. one memset per step over an arena of
-                            workspaces): no memset node in front of the statistics kernel, which is then PDL-chained */
-    float* partial_ws;   /* optional: scratch for per-block partial statistics (any contents).  With it the forward and the
+    float* partial_ws;   /* required: scratch for per-block partial statistics (any contents), so that the forward and the
                             backward's dx are bit-reproducible: no fp32 atomics in the statistics, the last block of an image
                             sums the partials in a fixed order (the backward's dgamma/dbeta still accumulate atomically).
-                            NULL: round-1 behaviour (atomic accumulation into stats_ws). */
+                            The call returns CTRLORA_STATUS_BAD_ARGUMENT and launches nothing when partial_ws or
+                            partial_counters is NULL, when batch > partial_counters_len, or when the two-pass launch's
+                            partials (batch * blocks per image * groups * 2 floats) exceed partial_ws_floats. */
     long long partial_ws_floats;
     unsigned int* partial_counters;   /* [>= batch] arrival counters: all zero on entry, left all zero on exit */
     int partial_counters_len;

@@ -155,9 +155,9 @@ def _gn_forward(cat, gamma, beta, eps, silu, groups, gamma_hi=None, beta_hi=None
 
 
 def groupnorm(x1, gamma, beta, eps, silu, *, add1=None, add1_scale=1.0, x2=None, add2=None, add2_scale=1.0, groups=32,
-              want_raw=False, stats_ws=None, want_stats=False, out=None, gamma_hi=None, beta_hi=None):
-    """ops.groupnorm: y (and the raw concatenation, and the fp64 {sum, sumsq} per (image, group) in stats_ws's
-    [batch * groups * 2] layout), in the order ops.groupnorm returns them"""
+              want_raw=False, want_stats=False, out=None, gamma_hi=None, beta_hi=None):
+    """ops.groupnorm: y (and the raw concatenation, and the fp64 {sum, sumsq} per (image, group) in the
+    [batch * groups * 2] layout of its statistics), in the order ops.groupnorm returns them"""
     cat = _concat(x1, add1, add1_scale, x2, add2, add2_scale)
     y = _gn_forward(cat, gamma, beta, eps, silu, groups, gamma_hi, beta_hi)
     ret = [y]

@@ -62,9 +62,6 @@ LSE_ABS = 2e-3                        # |lse - ref| <= 2e-3 * max(1, max|ref|) (
 # ops functions the scenarios call that the shadow does not check, and why
 UNCHECKED = {
     "zeros": "cudaMemsetAsync of a new buffer, no kernel (test_round2_kernels_gpu.py)",
-    "stats_arena_begin": "one memset of the step's GroupNorm statistics arena; the statistics it pre-zeroes are checked "
-                         "at every groupnorm call",
-    "stats_arena_end": "host bookkeeping only",
     "small_linear": "time-embedding MLP and emb_layers GEMV, fp32 against torch in test_kernels_gpu.py / "
                     "test_round2_kernels_gpu.py at the steps' row counts",
     "timestep_embedding": "bit-exact against the reference formula in test_kernels_gpu.py",
@@ -124,7 +121,7 @@ def _tensors(v):
 # op -> (argument names the call reads, argument names it writes)
 IO = {
     "gemm": (("a", "w", "a2", "w2", "bias", "rowbias", "residual", "hi"), ("out", "seg_outs", "dup_out")),
-    "groupnorm": (("x1", "add1", "x2", "add2", "gamma", "beta", "gamma_hi", "beta_hi"), ("out", "stats_ws")),
+    "groupnorm": (("x1", "add1", "x2", "add2", "gamma", "beta", "gamma_hi", "beta_hi"), ("out",)),
     "layernorm": (("x", "gamma", "beta", "gamma_hi", "beta_hi"), ()),
     "attention": (("q", "k", "vt"), ("out", "lse")),
     "wgrad_tn": (("a", "b", "out"), ("out",)),
@@ -270,7 +267,7 @@ class Shadow:
         replace = replace or {}
         members = inspect.getmembers(ops, inspect.isfunction)
         for name, fn in members:
-            if fn.__module__ != ops.__name__ or name.startswith("_") or name == "with_stats_arena":
+            if fn.__module__ != ops.__name__ or name.startswith("_"):
                 continue
             real = replace.get(name, fn)
             monkeypatch.setattr(ops, name, self._wrap(name, real, _signature(dict(members), name)))

@@ -35,7 +35,12 @@ def test_abi_exports_every_declared_symbol():
     lib = _lib.load()
     for name in declared:
         assert getattr(lib, name) is not None
-    assert lib.ctrlora_abi_version() == 2
+
+
+def test_abi_version_is_3():
+    """version 3: ctrlora_groupnorm_args has no stats_prezeroed field, so the struct layout differs from version 2"""
+    from ctrlora_b200 import _lib
+    assert _lib.load().ctrlora_abi_version() == 3
 
 
 def test_gemm_args_struct_layout_matches_header():
