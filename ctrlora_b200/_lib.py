@@ -130,8 +130,10 @@ _ARGTYPES = {
     "ctrlora_dpm_threshold": [_P, _P, _I, _L, _L, _L, _F, _F, _P],
     "ctrlora_dpm_adaptive_error": [_P, _P, _P, _P, _I, _L, _F, _F, _P],
     "ctrlora_tap_gather_f16": [_P, _I, _L, _P, _I, _I, _I, _I, _P, _I, _I, _I, _P],
+    "ctrlora_tap_gather_act_f16": [_P, _I, _L, _P, _I, _I, _I, _I, _P, _I, _I, _I, _I, _I, _P],
     "ctrlora_instance_norm_f16": [_P, _P, _P, _P, _L, _I, _I, _I, _I, _I, _I, _F, _P],
     "ctrlora_lineart_out_f16": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
+    "ctrlora_lineart_anime_out_f16": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _F, _P],
     "ctrlora_hed_side_pool_f16": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
     "ctrlora_hed_fuse": [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
     "ctrlora_openpose_resample": [_P, _I, _I, _I, _I, _P, _P, _I, _P, _P, _I, _P, _I, _I, _P],
@@ -219,8 +221,10 @@ EXPORTS = [
     "ctrlora_dpm_threshold",
     "ctrlora_dpm_adaptive_error",
     "ctrlora_tap_gather_f16",
+    "ctrlora_tap_gather_act_f16",
     "ctrlora_instance_norm_f16",
     "ctrlora_lineart_out_f16",
+    "ctrlora_lineart_anime_out_f16",
     "ctrlora_hed_side_pool_f16",
     "ctrlora_hed_fuse",
     "ctrlora_openpose_resample",

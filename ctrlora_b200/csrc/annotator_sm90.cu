@@ -17,23 +17,31 @@ struct TapList {
 __device__ __forceinline__ int reflect_idx(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }
 
 // ------------------------------------------------------------------------------------------ tap gather
-// dst[b, y, x, t * C + c] = src[b, Y(y + dy_t), X(x + dx_t), c], Y / X reflecting or (zero) masking outside the image;
-// columns >= taps * C are zero.  Each thread writes 8 columns.  VEC: fp16 pixel-major source with C % 8 == 0, one
-// 16-byte load per thread; otherwise element by element from fp16 pixel-major (F32 = false) or fp32 NCHW (F32 = true).
+// dst[b, y, x, t * C + c] = act(src[b, Y(s y + dy_t), X(s x + dx_t), c]) for output pixels (y, x) of [b, h / s, w / s]
+// (h, w: the source's size, s: stride 1 or 2), Y / X reflecting or (zero) masking outside the image; columns
+// >= taps * C are zero.  act: 0 none, 1 ReLU, 2 LeakyReLU(0.2), in fp32 before the fp16 rounding.  Each thread writes
+// 8 columns.  VEC: fp16 pixel-major source with C % 8 == 0, one 16-byte load per thread; otherwise element by element
+// from fp16 pixel-major (F32 = false) or fp32 NCHW (F32 = true).
+__device__ __forceinline__ float gather_act(float v, int act) {
+    return act == 1 ? fmaxf(v, 0.f) : (act == 2 && v < 0.f ? v * 0.2f : v);
+}
+
 template <bool VEC, bool F32>
 __global__ void __launch_bounds__(256)
 tap_gather_kernel(const void* __restrict__ src_, long long ld, __half* __restrict__ dst, int vecs, int h, int w,
-                  int channels, const __grid_constant__ TapList taps, int n_taps, int reflect, int k_pad) {
+                  int channels, const __grid_constant__ TapList taps, int n_taps, int reflect, int k_pad, int stride,
+                  int act) {
     // taps is read in place from the parameter bank (__grid_constant__): a by-value copy indexed at run time would be
     // spilled to local memory by every thread; indices are 32-bit (the launch checks vecs < 2^31)
     pdl_launch_dependents();
     pdl_wait();
     const int vecs_per_row = k_pad >> 3, k = n_taps * channels;
+    const int ho = h / stride, wo = w / stride;
     for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < vecs; v += gridDim.x * blockDim.x) {
         const int row = v / vecs_per_row;
         const int col0 = (v - row * vecs_per_row) * 8;
-        const int by = row / w, x = row - by * w;
-        const int b = by / h, y = by - b * h;
+        const int by = row / wo, x = (row - by * wo) * stride;
+        const int b = by / ho, y = (by - b * ho) * stride;
         if (VEC) {
             uint4 val = make_uint4(0, 0, 0, 0);
             if (col0 < k) {
@@ -45,6 +53,14 @@ tap_gather_kernel(const void* __restrict__ src_, long long ld, __half* __restric
                 if (in) {
                     const __half* s = static_cast<const __half*>(src_) + (((long long)b * h + yy) * w + xx) * ld + c;
                     val = *reinterpret_cast<const uint4*>(s);
+                    if (act) {
+                        __half2* hv = reinterpret_cast<__half2*>(&val);
+#pragma unroll
+                        for (int e = 0; e < 4; ++e) {
+                            const float2 f = __half22float2(hv[e]);
+                            hv[e] = __floats2half2_rn(gather_act(f.x, act), gather_act(f.y, act));
+                        }
+                    }
                 }
             }
             reinterpret_cast<uint4*>(dst)[v] = val;
@@ -64,6 +80,7 @@ tap_gather_kernel(const void* __restrict__ src_, long long ld, __half* __restric
                             val = static_cast<const float*>(src_)[(((long long)b * channels + c) * h + yy) * w + xx];
                         else
                             val = __half2float(static_cast<const __half*>(src_)[(((long long)b * h + yy) * w + xx) * ld + c]);
+                        val = gather_act(val, act);
                     }
                 }
                 o[e] = __float2half_rn(val);
@@ -92,7 +109,7 @@ __device__ __forceinline__ long long norm_dst_row(int b, long long r, long long 
 
 // Per (image, chunk of rows, channel) partial sums of (x - x[row 0]) and its square, stored [image, channel, chunk]:
 // thread t owns the 8 channels of vector t % (C / 8) and rows t / (C / 8), + lanes, ... of the chunk; the lanes are then
-// summed in lane order.  The shift by the image's first row keeps the one-pass variance accurate when |mean| >> std.
+// summed in lane order (at 512 channels, lanes = 4 and each thread sums two channels).  The shift by the image's first row keeps the one-pass variance accurate when |mean| >> std.
 // Fixed partition, fixed order, no atomics.
 __global__ void __launch_bounds__(256)
 inorm_partial_kernel(const __half* __restrict__ x, float2* __restrict__ part, int batch, long long hw, int channels,
@@ -131,8 +148,8 @@ inorm_partial_kernel(const __half* __restrict__ x, float2* __restrict__ part, in
 #pragma unroll
     for (int e = 0; e < 8; ++e) red[threadIdx.x][e] = make_float2(s[e], q[e]);
     __syncthreads();
-    if (threadIdx.x < channels) {
-        const int c = threadIdx.x, v = c >> 3, e = c & 7;
+    for (int c = threadIdx.x; c < channels; c += 256) {
+        const int v = c >> 3, e = c & 7;
         float2 acc = red[v][e];
         for (int l = 1; l < lanes; ++l) {
             const float2 p = red[l * cv + v][e];
@@ -262,6 +279,65 @@ lineart_out_kernel(const __half* __restrict__ x, const float* __restrict__ wt, c
     }
 }
 
+// ------------------------------------------------------------------------------------------ anime output conv
+// Anime2Sketch's outermost up path: ReLU over the two halves [skip | up] (each fp16 [B, h, w, half], half = C / 2),
+// ConvTranspose2d(C -> 1, 4, stride 2, padding 1) + bias, tanh, then * scale + shift as two fp32 roundings (the
+// detector's `* 127.5 + 127.5`).  Output pixel (2m + py, 2n + px) reads input rows m + dy through kernel rows ky for the
+// (dy, ky) of kAnimeRows[py] (oy = 2 iy - 1 + ky), the same for columns: 4 taps x C channels.  A CTA computes 16 x 16
+// outputs, one per thread, from a 10 x 10 input window staged channel-pair-planar in shared memory (ReLU applied, zero
+// outside the image); the weights sit channel-major [C][16] so the four phases of a warp read four banks.
+constexpr int kAT = 16, kAW = kAT / 2 + 2, kAMaxC = 128;
+__global__ void __launch_bounds__(256)
+lineart_anime_out_kernel(const __half* __restrict__ skip, const __half* __restrict__ up, const float* __restrict__ wt,
+                         const float* __restrict__ bias, float* __restrict__ out, int h, int w, int channels, float scale,
+                         float shift) {
+    pdl_launch_dependents();
+    pdl_wait();
+    __shared__ __half2 tile[kAMaxC / 2][kAW][kAW];
+    __shared__ float wsm[kAMaxC * 16];
+    const int b = blockIdx.z, ty = threadIdx.x / kAT, tx = threadIdx.x % kAT;
+    const int pairs = channels / 2, half = channels / 2, hp = half / 2;  // channel pairs in all, channels and pairs per half
+    const int m0 = blockIdx.y * (kAT / 2) - 1, n0 = blockIdx.x * (kAT / 2) - 1;  // input origin of the window
+    for (int i = threadIdx.x; i < kAW * kAW * pairs; i += 256) {
+        const int cp = i % pairs, px = (i / pairs) % kAW, py = i / (pairs * kAW);
+        const int yy = m0 + py, xx = n0 + px;
+        __half2 v = __floats2half2_rn(0.f, 0.f);
+        if (yy >= 0 && yy < h && xx >= 0 && xx < w) {
+            const __half* src = cp < hp ? skip : up;
+            v = reinterpret_cast<const __half2*>(src + (((long long)b * h + yy) * w + xx) * half)[cp < hp ? cp : cp - hp];
+            v = __hmax2(v, __floats2half2_rn(0.f, 0.f));
+        }
+        tile[cp][py][px] = v;
+    }
+    for (int i = threadIdx.x; i < channels * 16; i += 256) wsm[i] = wt[i];
+    __syncthreads();
+    const int py = ty & 1, px = tx & 1;
+    // window coordinates of input row m (= ty / 2 + 1) and column n; tap a of phase py: (dy, ky)
+    const int wy = (ty >> 1) + 1, wx = (tx >> 1) + 1;
+    const int dy0 = py ? 1 : 0, ky0 = py ? 0 : 1, dy1 = py ? 0 : -1, ky1 = py ? 2 : 3;
+    const int dx0 = px ? 1 : 0, kx0 = px ? 0 : 1, dx1 = px ? 0 : -1, kx1 = px ? 2 : 3;
+    float acc = 0.f;
+#pragma unroll
+    for (int a = 0; a < 2; ++a) {
+        const int dy = a ? dy1 : dy0, ky = a ? ky1 : ky0;
+#pragma unroll
+        for (int bb = 0; bb < 2; ++bb) {
+            const int dx = bb ? dx1 : dx0, kx = bb ? kx1 : kx0;
+            const float* wk = wsm + ky * 4 + kx;
+#pragma unroll 8
+            for (int cp = 0; cp < pairs; ++cp) {
+                const float2 v = __half22float2(tile[cp][wy + dy][wx + dx]);
+                acc = fmaf(v.x, wk[(2 * cp) * 16], acc);
+                acc = fmaf(v.y, wk[(2 * cp + 1) * 16], acc);
+            }
+        }
+    }
+    const int oy = blockIdx.y * kAT + ty, ox = blockIdx.x * kAT + tx;
+    if (oy >= 2 * h || ox >= 2 * w) return;
+    const float t = tanhf(acc + bias[0]);
+    out[((long long)b * 2 * h + oy) * (2LL * w) + ox] = __fadd_rn(__fmul_rn(t, scale), shift);
+}
+
 static int launched_annot(cudaError_t e) {
     if (e != cudaSuccess) return CTRLORA_ERR_CUDA;
     return cudaGetLastError() == cudaSuccess ? CTRLORA_OK : CTRLORA_ERR_CUDA;
@@ -284,11 +360,13 @@ static long long inorm_chunk_rows(long long rows) {
 
 using namespace ctrl;
 
-extern "C" int ctrlora_tap_gather_f16(const void* src, int src_f32_nchw, long long ld, void* dst, int batch, int h, int w,
-                                      int channels, const int* taps, int n_taps, int reflect, int k_pad, void* stream_) {
+static int tap_gather_launch(const void* src, int src_f32_nchw, long long ld, void* dst, int batch, int h, int w,
+                             int channels, const int* taps, int n_taps, int reflect, int k_pad, int stride, int act,
+                             void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     if (!src || !dst || !taps || batch < 0 || h < 1 || w < 1 || channels < 1 || n_taps < 1 || n_taps > kMaxTaps ||
-        k_pad % 8 || k_pad < n_taps * channels || (!src_f32_nchw && ld < channels))
+        k_pad % 8 || k_pad < n_taps * channels || (!src_f32_nchw && ld < channels) || (stride != 1 && stride != 2) ||
+        h % stride || w % stride || act < 0 || act > 2)
         return CTRLORA_ERR_ARG;
     TapList tl;
     memset(&tl, 0, sizeof(tl));
@@ -300,26 +378,38 @@ extern "C" int ctrlora_tap_gather_f16(const void* src, int src_f32_nchw, long lo
         tl.dy[t] = static_cast<signed char>(dy);
         tl.dx[t] = static_cast<signed char>(dx);
     }
-    const long long vecs = (long long)batch * h * w * (k_pad / 8);
+    const long long vecs = (long long)batch * (h / stride) * (w / stride) * (k_pad / 8);
     if (vecs == 0) return CTRLORA_OK;
     if (vecs >= (1LL << 31)) return CTRLORA_ERR_UNSUPPORTED;
     __half* d = static_cast<__half*>(dst);
     const bool vec = !src_f32_nchw && channels % 8 == 0 && ld % 8 == 0 && !(reinterpret_cast<uintptr_t>(src) & 15);
     if (vec)
         return launched_annot(launch_pdl(tap_gather_kernel<true, false>, dim3(grid_annot(vecs)), dim3(256), (size_t)0, stream,
-                                         src, ld, d, (int)vecs, h, w, channels, tl, n_taps, reflect, k_pad));
+                                         src, ld, d, (int)vecs, h, w, channels, tl, n_taps, reflect, k_pad, stride, act));
     if (src_f32_nchw)
         return launched_annot(launch_pdl(tap_gather_kernel<false, true>, dim3(grid_annot(vecs)), dim3(256), (size_t)0, stream,
-                                         src, ld, d, (int)vecs, h, w, channels, tl, n_taps, reflect, k_pad));
+                                         src, ld, d, (int)vecs, h, w, channels, tl, n_taps, reflect, k_pad, stride, act));
     return launched_annot(launch_pdl(tap_gather_kernel<false, false>, dim3(grid_annot(vecs)), dim3(256), (size_t)0, stream,
-                                     src, ld, d, (int)vecs, h, w, channels, tl, n_taps, reflect, k_pad));
+                                     src, ld, d, (int)vecs, h, w, channels, tl, n_taps, reflect, k_pad, stride, act));
+}
+
+extern "C" int ctrlora_tap_gather_f16(const void* src, int src_f32_nchw, long long ld, void* dst, int batch, int h, int w,
+                                      int channels, const int* taps, int n_taps, int reflect, int k_pad, void* stream_) {
+    return tap_gather_launch(src, src_f32_nchw, ld, dst, batch, h, w, channels, taps, n_taps, reflect, k_pad, 1, 0, stream_);
+}
+
+extern "C" int ctrlora_tap_gather_act_f16(const void* src, int src_f32_nchw, long long ld, void* dst, int batch, int h,
+                                          int w, int channels, const int* taps, int n_taps, int reflect, int k_pad,
+                                          int stride, int act, void* stream_) {
+    return tap_gather_launch(src, src_f32_nchw, ld, dst, batch, h, w, channels, taps, n_taps, reflect, k_pad, stride, act,
+                             stream_);
 }
 
 extern "C" int ctrlora_instance_norm_f16(const void* x, const void* residual, void* y, float* ws, long long ws_floats,
                                          int batch, int h, int w, int channels, int phases, int relu, float eps,
                                          void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    if (!x || !y || !ws || batch < 0 || h < 1 || w < 1 || channels < 64 || channels % 64 || 256 % channels ||
+    if (!x || !y || !ws || batch < 0 || h < 1 || w < 1 || channels < 64 || channels % 64 || 512 % channels ||
         (phases != 0 && phases != 1) || ws_floats < 2LL * batch * channels * (kNormMaxChunks + 1) ||
         (reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(y) & 15) ||
         (reinterpret_cast<uintptr_t>(residual) & 15) || (reinterpret_cast<uintptr_t>(ws) & 7))
@@ -354,4 +444,19 @@ extern "C" int ctrlora_lineart_out_f16(const void* x, const float* weight, const
     const dim3 grid((w + kOT - 1) / kOT, (h + kOT - 1) / kOT, batch);
     return launched_annot(launch_pdl(lineart_out_kernel, grid, dim3(256), (size_t)0, stream, static_cast<const __half*>(x),
                                      weight, bias, out, out_u8, h, w, channels));
+}
+
+extern "C" int ctrlora_lineart_anime_out_f16(const void* skip, const void* up, const float* weight, const float* bias,
+                                             float* out, int batch, int h, int w, int channels, float scale, float shift,
+                                             void* stream_) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    if (!skip || !up || !weight || !bias || !out || batch < 0 || h < 1 || w < 1 || channels < 4 || channels % 4 ||
+        channels > kAMaxC || (reinterpret_cast<uintptr_t>(skip) & 3) || (reinterpret_cast<uintptr_t>(up) & 3))
+        return CTRLORA_ERR_ARG;
+    if (batch == 0) return CTRLORA_OK;
+    if (batch > 65535) return CTRLORA_ERR_UNSUPPORTED;
+    const dim3 grid((2 * w + kAT - 1) / kAT, (2 * h + kAT - 1) / kAT, batch);
+    return launched_annot(launch_pdl(lineart_anime_out_kernel, grid, dim3(256), (size_t)0, stream,
+                                     static_cast<const __half*>(skip), static_cast<const __half*>(up), weight, bias, out, h,
+                                     w, channels, scale, shift));
 }

@@ -992,10 +992,8 @@ def gelu_(x):
 
 
 # ------------------------------------------------------------------------------------------------ line-art annotator
-def tap_gather(x, taps, *, reflect, k_pad, channels=None, out=None):
-    """Gather the (dy, dx) taps of every pixel into GEMM rows: fp16 [B, H, W, k_pad], column t * C + c = x at (y + dy_t,
-    x + dx_t), reflected at the border (nn.ReflectionPad2d) or zero outside, zero beyond len(taps) * C.
-    x: fp16 pixel-major [B, H, W, ld] (channels <= ld, default ld) or fp32 NCHW [B, C, H, W] contiguous."""
+def _gather_source(x, taps, channels):
+    """(batch, h, w, channels, ld, src_f32_nchw, host tap array) of a tap gather's source"""
     _require_cuda(x)
     if x.dtype == torch.float32:
         assert x.dim() == 4 and x.is_contiguous()
@@ -1005,14 +1003,42 @@ def tap_gather(x, taps, *, reflect, k_pad, channels=None, out=None):
         assert x.dtype == torch.float16
         b, h, w, c, ld = _as_bhwc(x)
         c, f32 = channels or c, 0
-    n = len(taps)
-    flat = (C.c_int * (2 * n))(*[int(v) for t in taps for v in t])
+    flat = (C.c_int * (2 * len(taps)))(*[int(v) for t in taps for v in t])
+    return b, h, w, c, ld, f32, flat
+
+
+def _gather_out(out, shape, device):
     if out is None:
-        out = torch.empty((b, h, w, k_pad), device=x.device, dtype=torch.float16)
-    assert out.shape == (b, h, w, k_pad) and out.is_contiguous() and out.dtype == torch.float16
+        out = torch.empty(shape, device=device, dtype=torch.float16)
+    assert out.shape == shape and out.is_contiguous() and out.dtype == torch.float16
+    return out
+
+
+def tap_gather(x, taps, *, reflect, k_pad, channels=None, out=None):
+    """Gather the (dy, dx) taps of every pixel into GEMM rows: fp16 [B, H, W, k_pad], column t * C + c = x at (y + dy_t,
+    x + dx_t), reflected at the border (nn.ReflectionPad2d) or zero outside, zero beyond len(taps) * C.
+    x: fp16 pixel-major [B, H, W, ld] (channels <= ld, default ld) or fp32 NCHW [B, C, H, W] contiguous."""
+    b, h, w, c, ld, f32, flat = _gather_source(x, taps, channels)
+    out = _gather_out(out, (b, h, w, k_pad), x.device)
     _count()
-    check(_lib.load().ctrlora_tap_gather_f16(_dp(x), f32, ld, _dp(out), b, h, w, c, C.cast(flat, C.c_void_p), n,
+    check(_lib.load().ctrlora_tap_gather_f16(_dp(x), f32, ld, _dp(out), b, h, w, c, C.cast(flat, C.c_void_p), len(taps),
                                              int(bool(reflect)), k_pad, _sp()), "tap_gather")
+    return out
+
+
+GATHER_ACTS = {None: 0, "relu": 1, "leaky": 2}  # ctrlora_tap_gather_act_f16's act codes; "leaky" is LeakyReLU(0.2)
+
+
+def tap_gather_act(x, taps, *, reflect, k_pad, stride=1, act=None, channels=None, out=None):
+    """tap_gather with an output stride and an activation on load: fp16 [B, H / stride, W / stride, k_pad], column
+    t * C + c of output pixel (y, x) = act(x at (stride y + dy_t, stride x + dx_t)), reflected or zero outside.
+    stride 1 or 2; act None, "relu" or "leaky" (LeakyReLU(0.2)), applied in fp32 before the fp16 rounding."""
+    b, h, w, c, ld, f32, flat = _gather_source(x, taps, channels)
+    out = _gather_out(out, (b, h // stride, w // stride, k_pad), x.device)
+    _count()
+    check(_lib.load().ctrlora_tap_gather_act_f16(_dp(x), f32, ld, _dp(out), b, h, w, c, C.cast(flat, C.c_void_p),
+                                                 len(taps), int(bool(reflect)), k_pad, stride, GATHER_ACTS[act], _sp()),
+          "tap_gather_act")
     return out
 
 
@@ -1059,6 +1085,23 @@ def lineart_out(x, weight, bias, want_u8=False):
     check(_lib.load().ctrlora_lineart_out_f16(_dp(x), _dp(weight), _dp(bias), _dp(out), _dp(u8), b, h, w, c, _sp()),
           "lineart_out")
     return (out, u8) if want_u8 else out
+
+
+def lineart_anime_out(skip, up, weight, bias, scale=1.0, shift=0.0):
+    """Anime2Sketch's outermost up path: tanh(bias + ConvTranspose2d(C -> 1, 4, stride 2, padding 1)(ReLU([skip | up]))
+    ) * scale + shift.  skip, up: fp16 [B, h, w, C / 2] each; weight fp32 [C, 16] (the transposed kernel [C, 1, 4, 4]);
+    bias fp32 [1] (device) -> fp32 [B, 1, 2h, 2w]"""
+    _require_cuda(skip, up, weight, bias)
+    assert skip.dtype == up.dtype == torch.float16 and skip.is_contiguous() and up.is_contiguous()
+    assert skip.dim() == 4 and up.shape == skip.shape
+    b, h, w, half = skip.shape
+    assert weight.dtype == torch.float32 and weight.is_contiguous() and weight.shape == (2 * half, 16)
+    assert bias.dtype == torch.float32 and bias.numel() == 1
+    out = torch.empty((b, 1, 2 * h, 2 * w), device=skip.device, dtype=torch.float32)
+    _count()
+    check(_lib.load().ctrlora_lineart_anime_out_f16(_dp(skip), _dp(up), _dp(weight), _dp(bias), _dp(out), b, h, w,
+                                                    2 * half, float(scale), float(shift), _sp()), "lineart_anime_out")
+    return out
 
 
 # ------------------------------------------------------------------------------------------------ HED annotator

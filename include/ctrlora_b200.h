@@ -414,13 +414,21 @@ int ctrlora_gelu_f16(void* x, long long n, void* stream);
  */
 int ctrlora_tap_gather_f16(const void* src, int src_f32_nchw, long long ld, void* dst, int batch, int h, int w, int channels,
                            const int* taps, int n_taps, int reflect, int k_pad, void* stream);
+/* ctrlora_tap_gather_f16 with an output stride and an activation on load (Anime2Sketch's UnetGenerator,
+ * annotator/lineart_anime/__init__.py:73-99): dst is [batch, h / stride, w / stride, k_pad] and output pixel (y, x)
+ * reads (stride y + dy, stride x + dx); stride 1 or 2, h and w multiples of it.  act: 0 none, 1 ReLU (uprelu), 2
+ * LeakyReLU(0.2) (downrelu), applied in fp32 to each gathered value before the fp16 rounding (zero-masked taps stay
+ * 0).  stride = 1, act = 0 is ctrlora_tap_gather_f16, bit for bit. */
+int ctrlora_tap_gather_act_f16(const void* src, int src_f32_nchw, long long ld, void* dst, int batch, int h, int w,
+                               int channels, const int* taps, int n_taps, int reflect, int k_pad, int stride, int act,
+                               void* stream);
 /* InstanceNorm2d(affine = False, track_running_stats = False) (:14): per (image, channel) biased statistics over the
  * image's rows, then y = relu?((x - mean) / sqrt(var + eps)) + residual?, fp16 in and out, fp32 math (the ReLU of :24,44,54,71
  * and ResidualBlock's x + conv_block(x), :33).  phases = 0: x and y are [batch, h, w, channels].  phases = 1: x holds the
  * four sub-pixel phase outputs of a stride-2 transposed conv, [4, batch, h, w, channels] with phase 2 py + px, and y is
  * [batch, 2h, 2w, channels], y[b, 2m + py, 2n + px] = f(x[2 py + px, b, m, n]).  residual (or NULL) has y's layout.
  * Statistics: fixed per-image row chunks and a fixed summation order, no atomics (bit-reproducible, and independent of
- * the batch).  ws: fp32 scratch of at least 2 * batch * channels * 1025 floats.  channels in {64, 128, 256}. */
+ * the batch).  ws: fp32 scratch of at least 2 * batch * channels * 1025 floats.  channels in {64, 128, 256, 512}. */
 int ctrlora_instance_norm_f16(const void* x, const void* residual, void* y, float* ws, long long ws_floats, int batch, int h,
                               int w, int channels, int phases, int relu, float eps, void* stream);
 /* The output layer (:77-80): ReflectionPad2d(3) + Conv2d(channels -> 1, 7) + Sigmoid on fp16 [batch, h, w, channels]
@@ -429,6 +437,13 @@ int ctrlora_instance_norm_f16(const void* x, const void* residual, void* y, floa
  * and truncation, as LineartDetector's `(line * 255.0).clip(0, 255).astype(np.uint8)` (:122). */
 int ctrlora_lineart_out_f16(const void* x, const float* weight, const float* bias, float* out, unsigned char* out_u8,
                             int batch, int h, int w, int channels, void* stream);
+/* Anime2Sketch's outermost up path (annotator/lineart_anime/__init__.py:85,112, as LineartAnimeDetector.__call__
+ * :144 scales it): out = tanh(bias + ConvTranspose2d(channels -> 1, 4, stride 2, padding 1)(ReLU([skip | up]))) *
+ * scale + shift, a multiply then an add in fp32.  skip and up: fp16 [batch, h, w, channels / 2] each (4-byte aligned),
+ * the concatenation's two halves, never materialised; channels % 4 == 0, <= 128.  weight: fp32 [channels, 16], the
+ * transposed kernel's [channels, 1, 4, 4]; bias: fp32 [1] (device).  out: fp32 [batch, 2h, 2w], fp32 accumulation. */
+int ctrlora_lineart_anime_out_f16(const void* skip, const void* up, const float* weight, const float* bias, float* out,
+                                  int batch, int h, int w, int channels, float scale, float shift, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * HED annotator (annotator/hed/__init__.py, ControlNetHED_Apache2 :36-52 as HEDdetector.__call__ :65-79 runs it).  Its
