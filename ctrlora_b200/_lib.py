@@ -124,6 +124,7 @@ _ARGTYPES = {
     "ctrlora_layernorm_rows": [_P, _I, _L, _P, _I, _L, _I, _I, _P, _P, _F, _P],
     "ctrlora_clip_patch_gather": [_P, _I, _P, _I, _I, _I, _I, _I, _P],
     "ctrlora_clip_vision_embed": [_P, _L, _P, _P, _P, _I, _I, _I, _P],
+    "ctrlora_patch_gather_hw": [_P, _I, _P, _I, _I, _I, _I, _I, _I, _P],
     "ctrlora_gelu_f16": [_P, _L, _P],
     "ctrlora_dpm_model_output": [_P, _P, _P, _P, _P, _L, _I, _I, _P, _P],
     "ctrlora_dpm_solver_update": [_P, _P, _P, _P, _P, _L, _I, _P, _P],
@@ -140,6 +141,11 @@ _ARGTYPES = {
     "ctrlora_openpose_smooth": [_P, _P, _P, _I, _I, _I, _P, _I, _P],
     "ctrlora_openpose_peaks": [_P, _P, _I, _I, _I, _D, _P, _L, _P, _P, _P, _P, _I, _P],
     "ctrlora_openpose_limbs": [_P, _I, _I, _I, _P, _P, _I, _P, _P, _I, _P, _P, _P, _I, _L, _I, _D, _P, _P, _P],
+    "ctrlora_depth_to_space_bias": [_P, _P, _P, _I, _I, _I, _I, _I, _P],
+    "ctrlora_add_relu_f16": [_P, _P, _P, _P, _L, _P],
+    "ctrlora_upsample_bilinear2x_f16": [_P, _P, _I, _I, _I, _I, _P],
+    "ctrlora_midas_head_out_f16": [_P, _P, _P, _P, _L, _I, _P],
+    "ctrlora_midas_maps": [_P, _P, _P, _P, _I, _I, _I, _F, _F, _P],
 }
 
 
@@ -215,6 +221,7 @@ EXPORTS = [
     "ctrlora_layernorm_rows",
     "ctrlora_clip_patch_gather",
     "ctrlora_clip_vision_embed",
+    "ctrlora_patch_gather_hw",
     "ctrlora_gelu_f16",
     "ctrlora_dpm_model_output",
     "ctrlora_dpm_solver_update",
@@ -231,4 +238,9 @@ EXPORTS = [
     "ctrlora_openpose_smooth",
     "ctrlora_openpose_peaks",
     "ctrlora_openpose_limbs",
+    "ctrlora_depth_to_space_bias",
+    "ctrlora_add_relu_f16",
+    "ctrlora_upsample_bilinear2x_f16",
+    "ctrlora_midas_head_out_f16",
+    "ctrlora_midas_maps",
 ]

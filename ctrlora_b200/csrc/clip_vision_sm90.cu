@@ -10,15 +10,16 @@
 namespace ctrl {
 
 // ------------------------------------------------------------------------------------------ patch gather
-// out[b * P + py * G + px, c * p * p + kh * p + kw] = pixels[b, c, py * p + kh, px * p + kw]   (G = image / p, P = G * G),
-// the Conv2d weight's (c, kh, kw) order; columns in [channels * p * p, k_pad) are zero.  Each thread writes 8 columns.
+// out[b * P + py * gw + px, c * p * p + kh * p + kw] = pixels[b, c, py * p + kh, px * p + kw]   (pixels [B, C, img_h, img_w],
+// grid gh x gw, P = gh * gw; rows and columns beyond p * gh, p * gw are never read), the Conv2d weight's (c, kh, kw)
+// order; columns in [channels * p * p, k_pad) are zero.  Each thread writes 8 columns.
 template <typename T>
 __global__ void __launch_bounds__(256)
-patch_gather_kernel(const T* __restrict__ pix, __half* __restrict__ out, long long vecs, int channels, int image, int patch,
-                    int k_pad) {
+patch_gather_kernel(const T* __restrict__ pix, __half* __restrict__ out, long long vecs, int channels, int img_h, int img_w,
+                    int grid_h, int grid_w, int patch, int k_pad) {
     pdl_launch_dependents();
     pdl_wait();
-    const int grid_w = image / patch, per_img = grid_w * grid_w, pp = patch * patch, k = channels * pp;
+    const int per_img = grid_h * grid_w, pp = patch * patch, k = channels * pp;
     const int vecs_per_row = k_pad >> 3;
     for (long long v = blockIdx.x * (long long)blockDim.x + threadIdx.x; v < vecs; v += (long long)gridDim.x * blockDim.x) {
         const long long row = v / vecs_per_row;
@@ -32,7 +33,7 @@ patch_gather_kernel(const T* __restrict__ pix, __half* __restrict__ out, long lo
             float val = 0.f;
             if (col < k) {
                 const int c = col / pp, r = col % pp;
-                const long long idx = ((static_cast<long long>(b) * channels + c) * image + y0 + r / patch) * image + x0 + r % patch;
+                const long long idx = ((static_cast<long long>(b) * channels + c) * img_h + y0 + r / patch) * img_w + x0 + r % patch;
                 val = static_cast<float>(pix[idx]);
             }
             h[e] = __float2half_rn(val);
@@ -92,20 +93,35 @@ static unsigned grid_for(long long vecs) {
 
 using namespace ctrl;
 
-extern "C" int ctrlora_clip_patch_gather(const void* pixels, int pixels_f32, void* out, int batch, int channels, int image,
-                                         int patch, int k_pad, void* stream_) {
-    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    if (!pixels || !out || batch < 0 || channels < 1 || patch < 1 || image < patch || image % patch ||
+static int patch_gather_launch(const void* pixels, int pixels_f32, void* out, int batch, int channels, int img_h, int img_w,
+                               int patch, int k_pad, cudaStream_t stream) {
+    if (!pixels || !out || batch < 0 || channels < 1 || patch < 1 || img_h < patch || img_w < patch ||
         k_pad < channels * patch * patch || k_pad % 8)
         return CTRLORA_ERR_ARG;
-    const long long rows = static_cast<long long>(batch) * (image / patch) * (image / patch), vecs = rows * (k_pad / 8);
+    const int grid_h = img_h / patch, grid_w = img_w / patch;
+    const long long rows = static_cast<long long>(batch) * grid_h * grid_w, vecs = rows * (k_pad / 8);
     if (vecs == 0) return CTRLORA_OK;
     __half* o = static_cast<__half*>(out);
     if (pixels_f32)
         return launched_vision(launch_pdl(patch_gather_kernel<float>, dim3(grid_for(vecs)), dim3(256), (size_t)0, stream,
-                                          static_cast<const float*>(pixels), o, vecs, channels, image, patch, k_pad));
+                                          static_cast<const float*>(pixels), o, vecs, channels, img_h, img_w, grid_h, grid_w,
+                                          patch, k_pad));
     return launched_vision(launch_pdl(patch_gather_kernel<__half>, dim3(grid_for(vecs)), dim3(256), (size_t)0, stream,
-                                      static_cast<const __half*>(pixels), o, vecs, channels, image, patch, k_pad));
+                                      static_cast<const __half*>(pixels), o, vecs, channels, img_h, img_w, grid_h, grid_w,
+                                      patch, k_pad));
+}
+
+extern "C" int ctrlora_clip_patch_gather(const void* pixels, int pixels_f32, void* out, int batch, int channels, int image,
+                                         int patch, int k_pad, void* stream_) {
+    if (patch < 1 || image % patch) return CTRLORA_ERR_ARG;
+    return patch_gather_launch(pixels, pixels_f32, out, batch, channels, image, image, patch, k_pad,
+                               reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int ctrlora_patch_gather_hw(const void* pixels, int pixels_f32, void* out, int batch, int channels, int h, int w,
+                                       int patch, int k_pad, void* stream_) {
+    return patch_gather_launch(pixels, pixels_f32, out, batch, channels, h, w, patch, k_pad,
+                               reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int ctrlora_clip_vision_embed(const float* patch_out, long long ldp, const float* class_embedding,

@@ -963,6 +963,22 @@ def clip_patch_gather(pixels, patch, k_pad, out=None):
     return out
 
 
+def patch_gather_hw(pixels, patch, k_pad, out=None):
+    """pixels fp32 or fp16 [B, C, H, W] (contiguous) -> fp16 patch rows [B * gh * gw, k_pad], gh = H // patch, gw =
+    W // patch (rows and columns beyond the last whole patch are not read), in clip_patch_gather's column order"""
+    _require_cuda(pixels)
+    assert pixels.dim() == 4 and pixels.is_contiguous() and pixels.dtype in (torch.float32, torch.float16)
+    b, c, h, w = pixels.shape
+    rows = b * (h // patch) * (w // patch)
+    if out is None:
+        out = torch.empty((rows, k_pad), device=pixels.device, dtype=torch.float16)
+    assert out.shape == (rows, k_pad) and out.is_contiguous() and out.dtype == torch.float16
+    _count()
+    check(_lib.load().ctrlora_patch_gather_hw(_dp(pixels), int(pixels.dtype == torch.float32), _dp(out), b, c, h, w, patch,
+                                              k_pad, _sp()), "patch_gather_hw")
+    return out
+
+
 def clip_vision_embed(patch_out, class_embedding, position_embedding, batch, out=None):
     """patch_out fp32 [batch * P, C] (row stride free) -> fp32 [batch * (P + 1), C]: per image the class embedding, then
     its P patch rows, each plus its position embedding"""
@@ -1250,6 +1266,75 @@ def openpose_limbs(paf, tables, px, py, limbs, img_h, thre):
                                              len(limbs), pairs, int(img_h), float(thre), _dp(score), _dp(ok), _sp()),
           "openpose_limbs")
     return score, ok
+
+
+# ------------------------------------------------------------------------------------------------ MiDaS annotator
+def depth_to_space_bias(src, bias, s):
+    """src fp32 [B, h, w, s * s * C] (a kernel = stride ConvTranspose2d as one GEMM, column (ky * s + kx) * C + c), bias
+    fp32 [C] -> fp16 [B, h * s, w * s, C], the bias added before the one rounding"""
+    _require_cuda(src, bias)
+    assert src.dtype == torch.float32 and src.is_contiguous() and src.dim() == 4
+    assert bias.dtype == torch.float32 and bias.is_contiguous()
+    b, h, w, n = src.shape
+    c = n // (s * s)
+    assert c * s * s == n and bias.numel() == c
+    out = torch.empty((b, h * s, w * s, c), device=src.device, dtype=torch.float16)
+    _count()
+    check(_lib.load().ctrlora_depth_to_space_bias(_dp(src), _dp(bias), _dp(out), b, h, w, c, s, _sp()),
+          "depth_to_space_bias")
+    return out
+
+
+def add_relu(a, b=None):
+    """fp16 tensors of one shape (contiguous) -> (s, relu(s)) with s = a + b rounded to fp16 once; b None: relu(a) only"""
+    _require_cuda(a, b)
+    assert a.dtype == torch.float16 and a.is_contiguous()
+    if b is not None:
+        assert b.dtype == torch.float16 and b.is_contiguous() and b.shape == a.shape
+    s = torch.empty_like(a) if b is not None else None
+    r = torch.empty_like(a)
+    _count()
+    check(_lib.load().ctrlora_add_relu_f16(_dp(a), _dp(b), _dp(s), _dp(r), a.numel(), _sp()), "add_relu")
+    return r if b is None else (s, r)
+
+
+def upsample_bilinear2x(x):
+    """F.interpolate(scale_factor=2, mode="bilinear", align_corners=True) on fp16 [B, h, w, C] -> [B, 2h, 2w, C]"""
+    _require_cuda(x)
+    assert x.is_contiguous() and x.dtype == torch.float16 and x.dim() == 4
+    b, h, w, c = x.shape
+    y = torch.empty((b, 2 * h, 2 * w, c), device=x.device, dtype=torch.float16)
+    _count()
+    check(_lib.load().ctrlora_upsample_bilinear2x_f16(_dp(x), _dp(y), b, h, w, c, _sp()), "upsample_bilinear2x")
+    return y
+
+
+def midas_head_out(x, weight, bias):
+    """the DPT head's Conv2d(C -> 1, 1) + ReLU: x fp16 [B, H, W, C], weight fp32 [C], bias fp32 [1] -> fp32 [B, H, W]"""
+    _require_cuda(x, weight, bias)
+    assert x.dtype == torch.float16 and x.is_contiguous() and x.dim() == 4
+    b, h, w, c = x.shape
+    assert weight.dtype == torch.float32 and weight.is_contiguous() and weight.numel() == c
+    assert bias.dtype == torch.float32 and bias.numel() == 1
+    out = torch.empty((b, h, w), device=x.device, dtype=torch.float32)
+    _count()
+    check(_lib.load().ctrlora_midas_head_out_f16(_dp(x), _dp(weight), _dp(bias), _dp(out), b * h * w, c, _sp()),
+          "midas_head_out")
+    return out
+
+
+def midas_maps(depth, a, bg_th):
+    """MidasDetector's post-process: depth fp32 [B, H, W] -> (uint8 [B, H, W] depth map, uint8 [B, H, W, 3] normal map)"""
+    _require_cuda(depth)
+    assert depth.dtype == torch.float32 and depth.is_contiguous() and depth.dim() == 3
+    b, h, w = depth.shape
+    minmax = torch.empty((b, 2), device=depth.device, dtype=torch.float32)
+    d8 = torch.empty((b, h, w), device=depth.device, dtype=torch.uint8)
+    n8 = torch.empty((b, h, w, 3), device=depth.device, dtype=torch.uint8)
+    _count(2)
+    check(_lib.load().ctrlora_midas_maps(_dp(depth), _dp(minmax), _dp(d8), _dp(n8), b, h, w, float(a), float(bg_th), _sp()),
+          "midas_maps")
+    return d8, n8
 
 
 def set_sm_limit(limit):

@@ -149,31 +149,37 @@ def layer_weights(prep, layer, i):
             get(("ln2", i), [layer.layer_norm2.weight, layer.layer_norm2.bias], ln(layer.layer_norm2)))
 
 
-def run_layers(layers, prep, h, b, n, heads, hidden_act, causal, f32=True):
+def run_layers(layers, prep, h, b, n, heads, hidden_act, causal, f32=True, weights=layer_weights, keep=(), split_k=0):
     """CLIPEncoder over `layers` on the residual stream h ([b * n, C], fp32 when f32, else fp16): per layer
     layer_norm1, one stacked q|k|v GEMM that stores V transposed, self-attention (causal d_head 64, or the full
     ctrlora_attention_f16), out_proj + residual, layer_norm2, fc1, GELU (hidden_act "quick_gelu" or "gelu", in place),
-    fc2 + residual.  Returns the new residual stream."""
+    fc2 + residual.  Returns the new residual stream.
+    weights(prep, layer, i): layer i's kernel copies in layer_weights' form (default: CLIP's parameter names).
+    keep: layer indices after which the stream is handed back; when given, returns (h, [h after each kept layer]).
+    split_k: passed to every GEMM (0 lets the tile model choose)."""
+    kept = []
     dev = h.device
     c = h.shape[1]
     d = c // heads
     n_pad = (n + 7) // 8 * 8
     act = {"quick_gelu": ops.quick_gelu_, "gelu": ops.gelu_}[hidden_act]
     for i, layer in enumerate(layers):
-        (w_qkv, b_qkv), (w_out, b_out), (w_fc1, b_fc1), (w_fc2, b_fc2), ln1, ln2 = layer_weights(prep, layer, i)
+        (w_qkv, b_qkv), (w_out, b_out), (w_fc1, b_fc1), (w_fc2, b_fc2), ln1, ln2 = weights(prep, layer, i)
         x = ops.layernorm_rows(h, *ln1)
         q = torch.empty((b * n, c), device=dev, dtype=torch.float16)
         k = torch.empty_like(q)
         vt = torch.empty((b, heads, d, n_pad), device=dev, dtype=torch.float16)
         ops.gemm(x, w_qkv, bias=b_qkv, seg_outs=[q, k, vt], seg_width=c, transposed=(0, 0, 1), rows_per_img=n, head_dim=d,
-                 tok_pad=n_pad)
+                 tok_pad=n_pad, split_k=split_k)
         a = ops.causal_attention(q, k, vt, b, heads, n) if causal else ops.attention(q, k, vt, b, heads, n, n, d)
-        h = ops.gemm(a, w_out, bias=b_out, residual=h, out_f32=f32)
+        h = ops.gemm(a, w_out, bias=b_out, residual=h, out_f32=f32, split_k=split_k)
         x = ops.layernorm_rows(h, *ln2)
-        f = ops.gemm(x, w_fc1, bias=b_fc1)
+        f = ops.gemm(x, w_fc1, bias=b_fc1, split_k=split_k)
         act(f)
-        h = ops.gemm(f, w_fc2, bias=b_fc2, residual=h, out_f32=f32)
-    return h
+        h = ops.gemm(f, w_fc2, bias=b_fc2, residual=h, out_f32=f32, split_k=split_k)
+        if i in keep:
+            kept.append(h)
+    return (h, kept) if keep else h
 
 
 class FrozenCLIPEmbedder(nn.Module):

@@ -393,6 +393,12 @@ int ctrlora_layernorm_rows(const void* x, int x_f32, long long ldx, void* y, int
  * image % patch == 0, k_pad % 8 == 0. */
 int ctrlora_clip_patch_gather(const void* pixels, int pixels_f32, void* out, int batch, int channels, int image, int patch,
                               int k_pad, void* stream);
+/* The same gather over a rectangular NCHW [batch, channels, h, w] image (MiDaS' ViT-L/16 patch embedding, forward_flex in
+ * annotator/midas/midas/vit.py): a grid of gh = h / patch by gw = w / patch patches, rows and columns beyond patch * gh,
+ * patch * gw are not read (the stride-patch Conv2d ignores them); row b * gh * gw + py * gw + px.  h = w is
+ * ctrlora_clip_patch_gather, bit for bit (both run one kernel). */
+int ctrlora_patch_gather_hw(const void* pixels, int pixels_f32, void* out, int batch, int channels, int h, int w, int patch,
+                            int k_pad, void* stream);
 /* CLIPVisionEmbeddings.forward after the conv: out[b * (P+1) + t, :] = (t == 0 ? class_embedding : patch_out[b * P + t-1, :])
  * + position_embedding[t, :], fp32 throughout (patch_out row stride ldp); pre_layrnorm follows as ctrlora_layernorm_rows. */
 int ctrlora_clip_vision_embed(const float* patch_out, long long ldp, const float* class_embedding,
@@ -508,6 +514,40 @@ int ctrlora_openpose_limbs(const float* paf, int paf_ld, int h8, int w8, const i
                            const int* x_start, const double* x_w, int tx, const int* px, const int* py, const int* limbs,
                            int n_limbs, long long pairs, int img_h, double thre, double* score, unsigned char* ok,
                            void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
+ * MiDaS DPT-Large depth annotator (annotator/midas/__init__.py MidasDetector, midas/dpt_depth.py, blocks.py, vit.py).
+ * The ViT-L/16 runs on ctrlora_patch_gather_hw, ctrlora_gemm_f16, ctrlora_clip_vision_embed, ctrlora_layernorm_rows,
+ * ctrlora_attention_f16 (d_head 64) and ctrlora_gelu_f16; the reassemble and fusion convs on ctrlora_gemm_f16 and
+ * ctrlora_im2col_s2_pad_f16.
+ *
+ * ConvTranspose2d(kernel = stride = s) computed as one GEMM with N = s * s * channels (column (ky * s + kx) * channels + c)
+ * and fp32 output: dst[b, y * s + ky, x * s + kx, c] = fp16(src[b, y, x, (ky * s + kx) * channels + c] + bias[c]).
+ * src fp32 [batch, h, w, s * s * channels] dense, dst fp16 [batch, h * s, w * s, channels]; channels % 4 == 0, s <= 8. */
+int ctrlora_depth_to_space_bias(const float* src, const float* bias, void* dst, int batch, int h, int w, int channels, int s,
+                                void* stream);
+/* sum = fp16(a + b) and relu = max(sum, 0) in one pass over fp16 [n] (n % 8 == 0, 16-byte aligned): the fusion block's
+ * skip_add.add followed by its RCU's input ReLU.  b = NULL: relu = max(a, 0) only (sum must be NULL then); either output
+ * may be NULL.  The ReLU is of the rounded sum. */
+int ctrlora_add_relu_f16(const void* a, const void* b, void* sum, void* relu, long long n, void* stream);
+/* F.interpolate(scale_factor=2, mode="bilinear", align_corners=True) on fp16 NHWC [batch, h, w, channels] -> [batch, 2h,
+ * 2w, channels], fp32 weights and sums (source index ((in - 1) / (out - 1)) * dst, as torch's kernel forms it);
+ * channels % 8 == 0.  FeatureFusionBlock_custom's and the DPT head's upsample. */
+int ctrlora_upsample_bilinear2x_f16(const void* src, void* dst, int batch, int h, int w, int channels, void* stream);
+/* The DPT head's Conv2d(channels -> 1, 1) + ReLU: out[p] = max(bias[0] + sum_c weight[c] * x[p, c], 0), fp32 sums in
+ * channel order.  x fp16 [pixels, channels] dense, channels % 8 == 0, <= 64; weight fp32 [channels]; bias fp32 [1]
+ * (device); out fp32 [pixels]. */
+int ctrlora_midas_head_out_f16(const void* x, const float* weight, const float* bias, float* out, long long pixels,
+                               int channels, void* stream);
+/* MidasDetector.__call__'s post-process on fp32 depth [batch, h, w] (h, w >= 2), two launches: per image the min and max
+ * into minmax fp32 [batch, 2] (exact, so independent of the reduction order), then per pixel, in fp32 with each
+ * operation rounded on its own as numpy and cv2 compute it:
+ *   dn = (d - min) / (max - min);  depth_u8 = u8(dn * 255)
+ *   x, y = cv2.Sobel(d, CV_32F, 1, 0 / 0, 1, ksize=3), BORDER_REFLECT_101, on the raw depth; x = y = 0 where dn < bg_th
+ *   n = sqrt(x^2 + y^2 + a^2);  normal_u8[.., 0..2] = u8([x, y, a] / n * 127.5 + 127.5)
+ * u8(v) is numpy's clip(0, 255).astype(uint8).  depth_u8 uint8 [batch, h, w]; normal_u8 uint8 [batch, h, w, 3]. */
+int ctrlora_midas_maps(const float* depth, float* minmax, unsigned char* depth_u8, unsigned char* normal_u8, int batch,
+                       int h, int w, float a, float bg_th, void* stream);
 
 #ifdef __cplusplus
 }
