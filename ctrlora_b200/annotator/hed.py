@@ -18,15 +18,12 @@ parameters; forward runs:
 Activations are fp16 pixel-major with fp32 accumulation.  Inference only, on the current stream.  H and W must be at
 least 16: the fifth block sees H // 16 x W // 16 pixels.  Odd sizes work: the pools floor as max_pool2d does.
 """
-import collections
-import os
-
 import numpy as np
 import torch
 import torch.nn as nn
 
 from .. import ops, prepare
-from .lineart import TAPS3, default_ckpt_dir
+from .common import TAPS3, SizeCache, checkpoint_path, device_input, freeze, linear_src_coord
 
 MIN_SIZE = 16
 TABLE_CACHE_SIZES = 8  # output sizes whose device resize tables are kept (least recently used goes first)
@@ -37,10 +34,7 @@ def resize_tables(src, dst):
     fraction), output position i = (1 - frac) * s[idx] + frac * s[idx + 1] (the neighbour clamped to the map).  A
     restatement of OpenCV's resizeGeneric rule: scale = 1 / (dst / src) in float64, fx = (float)((i + 0.5) * scale - 0.5),
     sx = floor(fx), fx -= sx in float32, then sx < 0 -> (0, 0) and sx >= src - 1 -> (src - 1, 0)."""
-    scale = 1.0 / (dst / src)
-    f = ((np.arange(dst, dtype=np.float64) + 0.5) * scale - 0.5).astype(np.float32)
-    s = np.floor(f).astype(np.int64)
-    f = (f - s.astype(np.float32)).astype(np.float32)
+    s, f = linear_src_coord(src, dst)
     lo, hi = s < 0, s >= src - 1
     f[lo | hi] = 0.0
     s[lo] = 0
@@ -80,27 +74,18 @@ class ControlNetHED_Apache2(nn.Module):
         self.block3 = DoubleConvBlock(128, 256, 3)
         self.block4 = DoubleConvBlock(256, 512, 3)
         self.block5 = DoubleConvBlock(512, 512, 3)
-        self.split_k = 0
-        self.eval()
-        for p in self.parameters():
-            p.requires_grad = False
-        self.__dict__["_prep"] = prepare.PrepCache()
-        self.__dict__["_tables"] = collections.OrderedDict()
+        freeze(self)
+        self.__dict__["_tables"] = SizeCache(TABLE_CACHE_SIZES)
 
     def blocks(self):
         return [self.block1, self.block2, self.block3, self.block4, self.block5]
 
-    # ---- kernel-layout weights (rebuilt by the PrepCache whenever a parameter changes, e.g. after load_state_dict)
+    # ---- kernel-layout weights
     def _conv_weights(self, key, conv, flat):
-        """(fp16 weight, fp32 bias): [Cout, 9, Cin] for the implicit 3x3 GEMM, or flat [Cout, 1, 32] (tap-major,
-        channel-minor, zero-padded from 27) for block1's first conv on the tap gather"""
+        """(fp16 weight, fp32 bias): [Cout, 9, Cin] for the implicit 3x3 GEMM, or flat [Cout, 1, 32] (K zero-padded
+        from 27) for block1's first conv on the tap gather"""
         def build():
-            w = prepare.conv_weight(conv.weight)
-            if flat:
-                co, taps, ci = w.shape
-                full = torch.zeros((co, 1, 32), device=w.device, dtype=torch.float16)
-                full[:, 0, :taps * ci] = w.reshape(co, taps * ci)
-                w = full
+            w = prepare.flat_conv_weight(conv.weight, 32) if flat else prepare.conv_weight(conv.weight)
             return w, prepare.bias_f32(conv.bias)
         return self._prep.get(key, [conv.weight, conv.bias], build)
 
@@ -112,19 +97,14 @@ class ControlNetHED_Apache2(nn.Module):
     def _resize_tables(self, h, w, device):
         """device (idx, frac) pairs of levels 1..4 for an h x w output, host-built; the last TABLE_CACHE_SIZES sizes are
         kept, so a caller that runs many image sizes holds a bounded set"""
-        key = (h, w, str(device))
-        tabs = self._tables.get(key)
-        if tabs is None:
+        def build():
             tabs = []
             for lh, lw in level_sizes(h, w)[1:]:
                 (ri, rf), (ci, cf) = resize_tables(lh, h), resize_tables(lw, w)
                 tabs.append((torch.from_numpy(np.concatenate([ri, ci])).to(device),
                              torch.from_numpy(np.concatenate([rf, cf])).to(device)))
-            self._tables[key] = tabs
-            while len(self._tables) > TABLE_CACHE_SIZES:
-                self._tables.popitem(last=False)
-        self._tables.move_to_end(key)
-        return tabs
+            return tabs
+        return self._tables.fetch((h, w, str(device)), build)
 
     def _check(self, x):
         if x.dim() != 4 or x.shape[1] != 3:
@@ -133,10 +113,7 @@ class ControlNetHED_Apache2(nn.Module):
         if h < MIN_SIZE or w < MIN_SIZE:
             raise ValueError(f"{h} x {w}: H and W must be at least {MIN_SIZE} (the fifth block sees H // 16 x W // 16 "
                              "pixels)")
-        dev = self.norm.device
-        if dev.type != "cuda":
-            raise RuntimeError("ControlNetHED_Apache2 runs on the sm_90a kernels only: move the model to a CUDA device")
-        return x.to(dev, torch.float32).contiguous()
+        return device_input(self, x, self.norm)
 
     def _run(self, x, stages=None):
         """the five fp32 side maps; with `stages` (a list) also the five blocks' fp16 outputs"""
@@ -178,19 +155,12 @@ class ControlNetHED_Apache2(nn.Module):
 
 
 class HEDdetector:
-    """The reference's HEDdetector: ControlNetHED.pth from `ckpt_dir` (default: the reference's annotator_ckpts_path);
+    """The reference's HEDdetector: ControlNetHED.pth from `ckpt_dir` (default: the reference's checkpoint directory);
     __call__(HWC uint8 RGB image, safe=False) -> HW uint8 edge map.  Nothing is downloaded: a missing checkpoint raises
     FileNotFoundError with the path it was expected at."""
 
     def __init__(self, ckpt_dir=None, device="cuda"):
-        ckpt_dir = ckpt_dir if ckpt_dir is not None else default_ckpt_dir()
-        if ckpt_dir is None:
-            raise FileNotFoundError("no checkpoint directory: the reference's annotator package is not importable, so "
-                                    "pass ckpt_dir (the directory holding ControlNetHED.pth)")
-        path = os.path.join(ckpt_dir, "ControlNetHED.pth")
-        if not os.path.isfile(path):
-            raise FileNotFoundError(f"ControlNetHED.pth not found at {path}: ctrlora_b200 never downloads checkpoints; "
-                                    f"fetch lllyasviel/Annotators' ControlNetHED.pth into {ckpt_dir}")
+        path = checkpoint_path(ckpt_dir, "ControlNetHED.pth")
         self.netNetwork = ControlNetHED_Apache2()
         self.netNetwork.load_state_dict(torch.load(path, map_location="cpu", weights_only=True), strict=True)
         self.netNetwork = self.netNetwork.to(device).eval()

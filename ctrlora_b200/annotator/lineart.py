@@ -20,24 +20,21 @@ constant cancels exactly.  Activations are fp16 pixel-major with fp32 accumulati
 only, on the current stream.  H and W must be multiples of 4 (the two stride-2 convs and the two transposed convs then
 give back H x W) and at least 8 (the residual blocks' ReflectionPad2d(1) needs 2 x 2 pixels).
 """
-import os
+import functools
 
 import numpy as np
 import torch
 import torch.nn as nn
 
 from .. import ops, prepare
+from . import common
+from .common import TAPS3, checkpoint_path, device_input, freeze, phase_weights
 
 TAPS7 = [(ky - 3, kx - 3) for ky in range(7) for kx in range(7)]
-TAPS3 = [(ky - 1, kx - 1) for ky in range(3) for kx in range(3)]
 # ConvTranspose2d(3, stride 2, padding 1, output_padding 1): output row 2m + py reads input rows m + dy through kernel
 # row ky, for the (dy, ky) of PHASE_ROWS[py] (oy = 2 iy - 1 + ky); the same for columns.  Phase p = 2 py + px.
 PHASE_ROWS = (((0, 1),), ((0, 2), (1, 0)))
-
-
-def phase_taps(py, px):
-    """[(dy, dx, ky, kx)] of the sub-pixel phase (py, px)"""
-    return [(dy, dx, ky, kx) for dy, ky in PHASE_ROWS[py] for dx, kx in PHASE_ROWS[px]]
+phase_taps = functools.partial(common.phase_taps, PHASE_ROWS)  # (py, px) -> [(dy, dx, ky, kx)]
 
 
 class ResidualBlock(nn.Module):
@@ -72,41 +69,16 @@ class Generator(nn.Module):
         if sigmoid:
             out.append(nn.Sigmoid())
         self.model4 = nn.Sequential(*out)
-        self.split_k = 0
-        self.eval()
-        for p in self.parameters():
-            p.requires_grad = False
-        self.__dict__["_prep"] = prepare.PrepCache()
+        freeze(self)
 
-    # ---- kernel-layout weights (rebuilt by the PrepCache whenever a parameter changes, e.g. after load_state_dict)
+    # ---- kernel-layout weights
     def _conv_gemm_weight(self, key, conv):
-        """Conv2d weight -> fp16 [Cout, 1, k_pad]: tap-major, channel-minor columns (the tap gather's and
-        im2col_s2's order), zero-padded to a multiple of 16"""
-        def build():
-            co, ci, kh, kw = conv.weight.shape
-            k = kh * kw * ci
-            w = prepare.conv_weight(conv.weight).view(co, 1, k)
-            k_pad = (k + 15) // 16 * 16
-            if k_pad == k:
-                return w
-            full = torch.zeros((co, 1, k_pad), device=w.device, dtype=torch.float16)
-            full[:, :, :k] = w
-            return full
-        return self._prep.get(key, [conv.weight], build)
+        """Conv2d weight -> fp16 [Cout, 1, k_pad], K zero-padded to a multiple of 16"""
+        return self._prep.get(key, [conv.weight], lambda: prepare.flat_conv_weight(conv.weight, 16))
 
     def _phase_weights(self, key, convt):
         """ConvTranspose2d weight [Cin, Cout, 3, 3] -> per phase 2 py + px: (gather taps, fp16 [Cout, 1, taps * Cin])"""
-        def build():
-            wt = convt.weight.detach().float().permute(1, 2, 3, 0)  # [Cout, ky, kx, Cin]
-            res = []
-            for py in (0, 1):
-                for px in (0, 1):
-                    taps = phase_taps(py, px)
-                    sel = torch.stack([wt[:, ky, kx] for _, _, ky, kx in taps], 1)  # [Cout, taps, Cin]
-                    res.append(([(dy, dx) for dy, dx, _, _ in taps],
-                                prepare.linear_weight(sel.reshape(sel.shape[0], -1).contiguous())))
-            return res
-        return self._prep.get(key, [convt.weight], build)
+        return self._prep.get(key, [convt.weight], lambda: phase_weights(convt, PHASE_ROWS))
 
     def _out_weights(self):
         conv = self.model4[1]
@@ -130,10 +102,7 @@ class Generator(nn.Module):
                                       "the output size)")
         if h < 8 or w < 8:
             raise ValueError(f"{h} x {w}: H and W must be at least 8 (ReflectionPad2d(1) of the residual blocks)")
-        dev = self.model4[1].weight.device
-        if dev.type != "cuda":
-            raise RuntimeError("Generator runs on the sm_90a kernels only: move the model to a CUDA device")
-        return x.to(dev, torch.float32).contiguous()
+        return device_input(self, x, self.model4[1].weight)
 
     def _run(self, x, want_u8=False, stages=None):
         x = self._check(x)
@@ -186,34 +155,18 @@ class Generator(nn.Module):
         return y, [ops.nhwc_to_nchw_f32(s) for s in st]
 
 
-def default_ckpt_dir():
-    """the reference's annotator_ckpts_path when its `annotator` package is importable, else None"""
-    try:
-        from annotator.util import annotator_ckpts_path
-    except ImportError:
-        return None
-    return annotator_ckpts_path
-
-
 class LineartDetector:
     """The reference's LineartDetector: sk_model.pth (fine) and sk_model2.pth (coarse) from `ckpt_dir` (default: the
-    reference's annotator_ckpts_path); __call__(HWC uint8 image, coarse) -> HW uint8 line map.  Nothing is downloaded:
+    reference's checkpoint directory); __call__(HWC uint8 image, coarse) -> HW uint8 line map.  Nothing is downloaded:
     a missing checkpoint raises FileNotFoundError with the path it was expected at."""
 
     def __init__(self, ckpt_dir=None, device="cuda"):
-        ckpt_dir = ckpt_dir if ckpt_dir is not None else default_ckpt_dir()
-        if ckpt_dir is None:
-            raise FileNotFoundError("no checkpoint directory: the reference's annotator package is not importable, so "
-                                    "pass ckpt_dir (the directory holding sk_model.pth and sk_model2.pth)")
         self.ckpt_dir, self.device = ckpt_dir, device
         self.model = self.load_model("sk_model.pth")
         self.model_coarse = self.load_model("sk_model2.pth")
 
     def load_model(self, name):
-        path = os.path.join(self.ckpt_dir, name)
-        if not os.path.isfile(path):
-            raise FileNotFoundError(f"{name} not found at {path}: ctrlora_b200 never downloads checkpoints; fetch "
-                                    f"lllyasviel/Annotators' {name} into {self.ckpt_dir}")
+        path = checkpoint_path(self.ckpt_dir, name)
         model = Generator(3, 1, 3)
         model.load_state_dict(torch.load(path, map_location="cpu", weights_only=True), strict=True)
         return model.to(self.device).eval()

@@ -23,7 +23,6 @@ Activations are fp16 pixel-major with fp32 accumulation and fp32 statistics.  In
 H and W must be multiples of 2^num_downs (the reference's `cat` fails on any other size).
 """
 import functools
-import os
 
 import cv2
 import numpy as np
@@ -31,17 +30,14 @@ import torch
 import torch.nn as nn
 
 from .. import ops, prepare
-from .lineart import default_ckpt_dir
+from . import common
+from .common import checkpoint_path, device_input, freeze, phase_weights
 
 TAPS4 = [(ky - 1, kx - 1) for ky in range(4) for kx in range(4)]  # Conv2d(4, stride 2, padding 1): iy = 2y - 1 + ky
 # ConvTranspose2d(4, stride 2, padding 1): output row 2m + py reads input rows m + dy through kernel row ky, for the
 # (dy, ky) of PHASE_ROWS[py] (oy = 2 iy - 1 + ky); the same for columns.  Phase p = 2 py + px.
 PHASE_ROWS = (((0, 1), (-1, 3)), ((1, 0), (0, 2)))
-
-
-def phase_taps(py, px):
-    """[(dy, dx, ky, kx)] of the sub-pixel phase (py, px)"""
-    return [(dy, dx, ky, kx) for dy, ky in PHASE_ROWS[py] for dx, kx in PHASE_ROWS[px]]
+phase_taps = functools.partial(common.phase_taps, PHASE_ROWS)  # (py, px) -> [(dy, dx, ky, kx)]
 
 
 def _is_instance_norm(norm_layer):
@@ -114,11 +110,7 @@ class UnetGenerator(nn.Module):
         self.model = UnetSkipConnectionBlock(output_nc, ngf, input_nc=input_nc, submodule=blk, outermost=True,
                                              norm_layer=norm_layer)
         self.num_downs = num_downs
-        self.split_k = 0
-        self.eval()
-        for p in self.parameters():
-            p.requires_grad = False
-        self.__dict__["_prep"] = prepare.PrepCache()
+        freeze(self)
 
     def blocks(self):
         """the UnetSkipConnectionBlocks from the outermost (0) to the innermost (num_downs - 1)"""
@@ -128,41 +120,15 @@ class UnetGenerator(nn.Module):
             blk = next((m for m in blk.model if isinstance(m, UnetSkipConnectionBlock)), None)
         return res
 
-    # ---- kernel-layout weights (rebuilt by the PrepCache whenever a parameter changes, e.g. after load_state_dict)
+    # ---- kernel-layout weights
     def _down_weight(self, i, conv):
-        """Conv2d weight -> fp16 [Cout, 1, k_pad]: tap-major, channel-minor columns (the gather's order), zero-padded to
-        a multiple of 64 (block 0: K = 48)"""
-        def build():
-            co, ci, kh, kw = conv.weight.shape
-            k = kh * kw * ci
-            w = prepare.conv_weight(conv.weight).view(co, 1, k)
-            k_pad = (k + 63) // 64 * 64
-            if k_pad == k:
-                return w
-            full = torch.zeros((co, 1, k_pad), device=w.device, dtype=torch.float16)
-            full[:, :, :k] = w
-            return full
-        return self._prep.get(f"down{i}", [conv.weight], build)
+        """Conv2d weight -> fp16 [Cout, 1, k_pad], K zero-padded to a multiple of 64 (block 0: K = 48)"""
+        return self._prep.get(f"down{i}", [conv.weight], lambda: prepare.flat_conv_weight(conv.weight, 64))
 
     def _phase_weights(self, i, convt, split):
-        """ConvTranspose2d weight [Cin, Cout, 4, 4] -> per phase 2 py + px: (gather taps, fp16 [Cout, 1, 4 * Cin]) or,
-        with split, (taps, fp16 [Cout, 1, 4 * Cin / 2] over the first half of the input channels, fp16 [Cout, 4 * Cin / 2]
-        over the second) -- the skip and the submodule halves of the concatenation"""
-        def build():
-            wt = convt.weight.detach().float().permute(1, 2, 3, 0)  # [Cout, ky, kx, Cin]
-            cin = wt.shape[-1]
-            res = []
-            for py in (0, 1):
-                for px in (0, 1):
-                    taps = phase_taps(py, px)
-                    sel = torch.stack([wt[:, ky, kx] for _, _, ky, kx in taps], 1)  # [Cout, taps, Cin]
-                    halves = (sel[..., :cin // 2], sel[..., cin // 2:]) if split else (sel,)
-                    ws = [prepare.linear_weight(h.reshape(h.shape[0], -1).contiguous()) for h in halves]
-                    if split:
-                        ws[1] = ws[1].view(ws[1].shape[0], -1)
-                    res.append(([(dy, dx) for dy, dx, _, _ in taps], *ws))
-            return res
-        return self._prep.get(f"up{i}", [convt.weight], build)
+        """common.phase_weights of a ConvTranspose2d(4, stride 2, padding 1); split: its input is the concatenation of
+        the skip and the submodule halves"""
+        return self._prep.get(f"up{i}", [convt.weight], lambda: phase_weights(convt, PHASE_ROWS, split))
 
     def _out_weights(self, convt):
         def build():
@@ -177,10 +143,7 @@ class UnetGenerator(nn.Module):
         if h % m or w % m:
             raise NotImplementedError(f"{h} x {w}: H and W must be multiples of {m} (2^num_downs: the U-Net's skip "
                                       "concatenations need every level to halve exactly)")
-        dev = self.model.model[0].weight.device
-        if dev.type != "cuda":
-            raise RuntimeError("UnetGenerator runs on the sm_90a kernels only: move the model to a CUDA device")
-        return x.to(dev, torch.float32).contiguous()
+        return device_input(self, x, self.model.model[0].weight)
 
     def _gather(self, x, taps, act, stride=1):
         c = x.shape[1] if x.dtype == torch.float32 else x.shape[-1]
@@ -259,19 +222,12 @@ def load_netg(path):
 
 
 class LineartAnimeDetector:
-    """The reference's LineartAnimeDetector: netG.pth from `ckpt_dir` (default: the reference's annotator_ckpts_path);
+    """The reference's LineartAnimeDetector: netG.pth from `ckpt_dir` (default: the reference's checkpoint directory);
     __call__(HWC uint8 image) -> HW uint8 line map.  Nothing is downloaded: a missing checkpoint raises
     FileNotFoundError with the path it was expected at."""
 
     def __init__(self, ckpt_dir=None, device="cuda"):
-        ckpt_dir = ckpt_dir if ckpt_dir is not None else default_ckpt_dir()
-        if ckpt_dir is None:
-            raise FileNotFoundError("no checkpoint directory: the reference's annotator package is not importable, so "
-                                    "pass ckpt_dir (the directory holding netG.pth)")
-        path = os.path.join(ckpt_dir, "netG.pth")
-        if not os.path.isfile(path):
-            raise FileNotFoundError(f"netG.pth not found at {path}: ctrlora_b200 never downloads checkpoints; fetch "
-                                    f"lllyasviel/Annotators' netG.pth into {ckpt_dir}")
+        path = checkpoint_path(ckpt_dir, "netG.pth")
         norm_layer = functools.partial(nn.InstanceNorm2d, affine=False, track_running_stats=False)
         net = UnetGenerator(3, 1, 8, 64, norm_layer=norm_layer, use_dropout=False)
         net.load_state_dict(load_netg(path), strict=True)

@@ -26,9 +26,7 @@ Activations are fp16 pixel-major with fp32 accumulation.  Inference only, on the
 and gw = W // 16 must be even and >= 2 (otherwise the reference's stride-2 branch and x2 upsample disagree in size);
 rows and columns beyond 16 gh, 16 gw are ignored, as the reference's patch conv ignores them.
 """
-import collections
 import math
-import os
 
 import numpy as np
 import torch
@@ -37,7 +35,7 @@ import torch.nn.functional as F
 
 from .. import ops, prepare
 from ..text_encoder import run_layers
-from .lineart import default_ckpt_dir
+from .common import SizeCache, checkpoint_path, device_input, freeze
 
 HOOKS = (5, 11, 17, 23)             # vitl16_384's hooked blocks
 FEATURES = (256, 512, 1024, 1024)   # reassemble widths
@@ -185,28 +183,22 @@ class DPTDepthModel(nn.Module):
                                       "non_negative=True, features=256, readout='project', use_bn=False")
         self.pretrained = _Pretrained()
         self.scratch = _Scratch(features)
-        self.split_k = 0
-        self.eval()
-        for p in self.parameters():
-            p.requires_grad = False
-        self.__dict__["_prep"] = prepare.PrepCache()
-        self.__dict__["_pos"] = collections.OrderedDict()
+        freeze(self)
+        self.__dict__["_pos"] = SizeCache(POS_CACHE_SIZES)
         if path is not None:
             self.load(path)
 
     def load(self, path):
         self.load_state_dict(load_checkpoint(path), strict=True)
 
-    # ---- kernel-layout weights (rebuilt by the PrepCache whenever a parameter changes, e.g. after load_state_dict)
+    # ---- kernel-layout weights
     def _lin(self, key, m):
         return self._prep.get(key, [m.weight, m.bias], lambda: (prepare.linear_weight(m.weight), prepare.bias_f32(m.bias)))
 
     def _conv(self, key, conv):
         """Conv2d -> (fp16 [Cout, 1, taps * Cin] tap-major, fp32 bias or None); 3x3 stride-1 convs keep [Cout, 9, Cin]"""
         def build():
-            w = prepare.conv_weight(conv.weight)
-            if conv.stride != (1, 1):
-                w = w.view(w.shape[0], 1, -1)
+            w = prepare.flat_conv_weight(conv.weight) if conv.stride != (1, 1) else prepare.conv_weight(conv.weight)
             return w, prepare.bias_f32(conv.bias)
         return self._prep.get(key, [conv.weight, conv.bias], build)
 
@@ -251,23 +243,16 @@ class DPTDepthModel(nn.Module):
         """fp32 [gh * gw + 1, C]: the reference's _resize_pos_embed (bilinear, align_corners=False) on the device; the last
         POS_CACHE_SIZES grid sizes are kept, and every entry is rebuilt when pos_embed changes"""
         pe = self.pretrained.model.pos_embed
-        key = (gh, gw)
-        ver = (pe.data_ptr(), pe._version)
-        hit = self._pos.get(key)
-        if hit is None or hit[0] != ver:
-            with torch.no_grad():
-                posemb = pe.detach().float()
-                tok, grid = posemb[:, :1], posemb[0, 1:]
-                g = int(math.sqrt(len(grid)))
-                grid = grid.reshape(1, g, g, -1).permute(0, 3, 1, 2)
-                grid = F.interpolate(grid, size=(gh, gw), mode="bilinear")
-                grid = grid.permute(0, 2, 3, 1).reshape(1, gh * gw, -1)
-                hit = (ver, torch.cat([tok, grid], dim=1)[0].contiguous())
-            self._pos[key] = hit
-            while len(self._pos) > POS_CACHE_SIZES:
-                self._pos.popitem(last=False)
-        self._pos.move_to_end(key)
-        return hit[1]
+
+        def build():
+            posemb = pe.detach().float()
+            tok, grid = posemb[:, :1], posemb[0, 1:]
+            g = int(math.sqrt(len(grid)))
+            grid = grid.reshape(1, g, g, -1).permute(0, 3, 1, 2)
+            grid = F.interpolate(grid, size=(gh, gw), mode="bilinear")
+            grid = grid.permute(0, 2, 3, 1).reshape(1, gh * gw, -1)
+            return torch.cat([tok, grid], dim=1)[0].contiguous()
+        return self._pos.fetch((gh, gw), build, [pe])
 
     # ---- forward
     def grid(self, x):
@@ -282,10 +267,7 @@ class DPTDepthModel(nn.Module):
 
     def _check(self, x):
         gh, gw = self.grid(x)
-        dev = self.pretrained.model.cls_token.device
-        if dev.type != "cuda":
-            raise RuntimeError("DPTDepthModel runs on the sm_90a kernels only: move the model to a CUDA device")
-        return x.to(dev, torch.float32).contiguous(), gh, gw
+        return device_input(self, x, self.pretrained.model.cls_token), gh, gw
 
     def _vit(self, x, gh, gw):
         """the residual stream after the hooked blocks: four fp32 [B * (P + 1), C]"""
@@ -382,7 +364,7 @@ MODEL_TYPES = ("dpt_large", "dpt_hybrid", "midas_v21", "midas_v21_small")
 
 class MiDaSInference(nn.Module):
     """The reference's MiDaSInference: `model` is the DPTDepthModel loaded from dpt_large_384.pt in `ckpt_dir` (default:
-    the reference's annotator_ckpts_path).  Only "dpt_large" is implemented; nothing is downloaded."""
+    the reference's checkpoint directory).  Only "dpt_large" is implemented; nothing is downloaded."""
 
     def __init__(self, model_type="dpt_large", ckpt_dir=None):
         super().__init__()
@@ -390,14 +372,7 @@ class MiDaSInference(nn.Module):
             raise ValueError(f"model_type {model_type!r} is not one of {MODEL_TYPES}")
         if model_type != "dpt_large":
             raise NotImplementedError(f"model_type {model_type!r}: only 'dpt_large' runs on the sm_90a kernels")
-        ckpt_dir = ckpt_dir if ckpt_dir is not None else default_ckpt_dir()
-        if ckpt_dir is None:
-            raise FileNotFoundError("no checkpoint directory: the reference's annotator package is not importable, so "
-                                    f"pass ckpt_dir (the directory holding {CKPT_NAME})")
-        path = os.path.join(ckpt_dir, CKPT_NAME)
-        if not os.path.isfile(path):
-            raise FileNotFoundError(f"{CKPT_NAME} not found at {path}: ctrlora_b200 never downloads checkpoints; fetch "
-                                    f"it into {ckpt_dir}")
+        path = checkpoint_path(ckpt_dir, CKPT_NAME)
         self.model = DPTDepthModel(path=path, backbone="vitl16_384", non_negative=True)
 
     def forward(self, x):

@@ -35,7 +35,7 @@ import torch
 import torch.nn as nn
 
 from .. import ops, prepare
-from .lineart import TAPS3, default_ckpt_dir
+from .common import TAPS3, SizeCache, checkpoint_path, device_input, freeze, linear_src_coord
 
 BOXSIZE, STRIDE, PAD_VALUE = 368, 8, 128
 SCALE_SEARCH = 0.5          # the reference's single scale
@@ -118,28 +118,23 @@ class bodypose_model(nn.Module):
         for b in (1, 2):  # the reference's registration order: model1_1 ... model6_1, then model1_2 ... model6_2
             for s in range(1, 7):
                 setattr(self, f"model{s}_{b}", _sequential(_stage_spec(s, b), no_relu))
-        self.split_k = 0
-        self.eval()
-        for p in self.parameters():
-            p.requires_grad = False
-        self.__dict__["_prep"] = prepare.PrepCache()
+        freeze(self)
         self.__dict__["_no_relu"] = no_relu
 
     def branch(self, stage, b):
         return getattr(self, f"model{stage}_{b}")
 
-    # ---- kernel-layout weights (rebuilt by the PrepCache whenever a parameter changes, e.g. after load_state_dict)
+    # ---- kernel-layout weights
     def _conv(self, name, conv, pad_out=None):
-        """(fp16 [Cout(pad), taps, Cin], fp32 bias [Cout(pad)]); conv1_1 flat [64, 1, 32] for the tap gather"""
+        """(fp16 [Cout(pad), taps, Cin], fp32 bias [Cout(pad)]); conv1_1 flat [64, 1, 32] (K zero-padded from 27) for
+        the tap gather"""
         def build():
-            w = prepare.conv_weight(conv.weight, pad_out=pad_out)
+            if name == "conv1_1":
+                w = prepare.flat_conv_weight(conv.weight, 32)
+            else:
+                w = prepare.conv_weight(conv.weight, pad_out=pad_out)
             bias = torch.zeros(w.shape[0], device=w.device, dtype=torch.float32)
             bias[:conv.out_channels] = conv.bias.detach().float()
-            if name == "conv1_1":
-                co, taps, ci = w.shape
-                flat = torch.zeros((co, 1, 32), device=w.device, dtype=torch.float16)
-                flat[:, 0, :taps * ci] = w.reshape(co, taps * ci)
-                w = flat
             return w, bias
         return self._prep.get(name, [conv.weight, conv.bias], build)
 
@@ -169,10 +164,7 @@ class bodypose_model(nn.Module):
         h, w = x.shape[2], x.shape[3]
         if h % STRIDE or w % STRIDE or h < STRIDE or w < STRIDE:
             raise ValueError(f"{h} x {w}: H and W must be positive multiples of {STRIDE} (Body pads the image so)")
-        dev = self.model0.conv1_1.weight.device
-        if dev.type != "cuda":
-            raise RuntimeError("bodypose_model runs on the sm_90a kernels only: move the model to a CUDA device")
-        return x.to(dev, torch.float32).contiguous()
+        return device_input(self, x, self.model0.conv1_1.weight)
 
     def _gemm(self, x, conv, name, out=None, out_f32=False, pad_out=None):
         w, b = self._conv(name, conv, pad_out)
@@ -224,20 +216,18 @@ class bodypose_model(nn.Module):
 
 # ------------------------------------------------------------------------------------------------ resampling tables
 def _src_coord(dst, src, area_linear):
-    """cv2.resize's (sx, fx) per output index along one axis: the generic rule fx = (float)((d + 0.5) * scale - 0.5), or
-    INTER_AREA's rule when it does not shrink both axes: sx = floor(d * scale), fx = (float)((d + 1) - (sx + 1) / scale)
-    wrapped to [0, 1).  scale = 1 / (dst / src) in float64."""
+    """cv2.resize's (sx, fx) per output index along one axis: the generic rule (common.linear_src_coord), or INTER_AREA's
+    rule when it does not shrink both axes: sx = floor(d * scale), fx = (float)((d + 1) - (sx + 1) / scale) wrapped to
+    [0, 1).  scale = 1 / (dst / src) in float64."""
+    if not area_linear:
+        return linear_src_coord(src, dst)
     inv = dst / src
     scale = 1.0 / inv
     d = np.arange(dst, dtype=np.float64)
-    if area_linear:
-        sx = np.floor(d * scale).astype(np.int64)
-        fx = ((d + 1) - (sx + 1) * inv).astype(np.float32)
-        fx = np.where(fx <= 0, np.float32(0), fx - np.floor(fx)).astype(np.float32)
-        return sx, fx
-    f = ((d + 0.5) * scale - 0.5).astype(np.float32)
-    sx = np.floor(f).astype(np.int64)
-    return sx, (f - sx.astype(np.float32)).astype(np.float32)
+    sx = np.floor(d * scale).astype(np.int64)
+    fx = ((d + 1) - (sx + 1) * inv).astype(np.float32)
+    fx = np.where(fx <= 0, np.float32(0), fx - np.floor(fx)).astype(np.float32)
+    return sx, fx
 
 
 def _lanczos4_coeffs(fx):
@@ -475,20 +465,14 @@ class PostProcess:
     TABLE_CACHE_SIZES image sizes"""
 
     def __init__(self):
-        self._tables = collections.OrderedDict()
+        self._tables = SizeCache(TABLE_CACHE_SIZES)
         self._gauss = gaussian_weights()
 
     def tables(self, h, w, device):
-        key = (h, w, str(device))
-        tabs = self._tables.get(key)
-        if tabs is None:
+        def build():
             (ys, yw), (xs, xw) = [band(m) for m in axis_matrices(h, w)]
-            tabs = tuple(torch.from_numpy(np.ascontiguousarray(t)).to(device) for t in (ys, yw, xs, xw))
-            self._tables[key] = tabs
-            while len(self._tables) > TABLE_CACHE_SIZES:
-                self._tables.popitem(last=False)
-        self._tables.move_to_end(key)
-        return tabs
+            return tuple(torch.from_numpy(np.ascontiguousarray(t)).to(device) for t in (ys, yw, xs, xw))
+        return self._tables.fetch((h, w, str(device)), build)
 
     def peaks(self, heat_px, h, w):
         """(heatmaps fp32 [18, h, w], smoothed float64 [18, h, w], device peaks (x, y, part, score))"""
@@ -528,9 +512,7 @@ class Body:
     (x, y, score, id) or the empty 1-D array, subset float64 [n, 20])"""
 
     def __init__(self, model_path, device="cuda"):
-        if not os.path.isfile(model_path):
-            raise FileNotFoundError(f"body_pose_model.pth not found at {model_path}: ctrlora_b200 never downloads "
-                                    "checkpoints; fetch lllyasviel/Annotators' body_pose_model.pth there")
+        checkpoint_path(*os.path.split(model_path))
         self.model = bodypose_model()
         ckpt = torch.load(model_path, map_location="cpu", weights_only=True)
         self.model.load_state_dict(checkpoint_state_dict(self.model, ckpt), strict=True)
@@ -547,17 +529,13 @@ class Body:
 
 class OpenposeDetector:
     """The reference's OpenposeDetector for bodies: body_pose_model.pth from `ckpt_dir` (default: the reference's
-    annotator_ckpts_path); __call__(HWC uint8 RGB image, hand_and_face=False, return_is_index=False) -> the drawn
+    checkpoint directory); __call__(HWC uint8 RGB image, hand_and_face=False, return_is_index=False) -> the drawn
     uint8 canvas, or the pose dict with return_is_index.  Nothing is downloaded: a missing checkpoint raises
     FileNotFoundError with the path it was expected at.  The hand and face estimators are not provided:
     hand_and_face=True raises NotImplementedError."""
 
     def __init__(self, ckpt_dir=None, device="cuda"):
-        ckpt_dir = ckpt_dir if ckpt_dir is not None else default_ckpt_dir()
-        if ckpt_dir is None:
-            raise FileNotFoundError("no checkpoint directory: the reference's annotator package is not importable, so "
-                                    "pass ckpt_dir (the directory holding body_pose_model.pth)")
-        self.body_estimation = Body(os.path.join(ckpt_dir, "body_pose_model.pth"), device=device)
+        self.body_estimation = Body(checkpoint_path(ckpt_dir, "body_pose_model.pth"), device=device)
 
     def __call__(self, oriImg, hand_and_face=False, return_is_index=False):
         if hand_and_face:

@@ -13,9 +13,6 @@ struct TapList {
     signed char dy[kMaxTaps], dx[kMaxTaps];
 };
 
-// nn.ReflectionPad2d's index map: the border pixel is not repeated (needs |offset| < n)
-__device__ __forceinline__ int reflect_idx(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }
-
 // ------------------------------------------------------------------------------------------ tap gather
 // dst[b, y, x, t * C + c] = act(src[b, Y(s y + dy_t), X(s x + dx_t), c]) for output pixels (y, x) of [b, h / s, w / s]
 // (h, w: the source's size, s: stride 1 or 2), Y / X reflecting or (zero) masking outside the image; columns
@@ -48,7 +45,7 @@ tap_gather_kernel(const void* __restrict__ src_, long long ld, __half* __restric
                 const int t = col0 / channels, c = col0 - t * channels;
                 int yy = y + taps.dy[t], xx = x + taps.dx[t];
                 bool in = true;
-                if (reflect) { yy = reflect_idx(yy, h); xx = reflect_idx(xx, w); }
+                if (reflect) { yy = reflect101(yy, h); xx = reflect101(xx, w); }
                 else in = yy >= 0 && yy < h && xx >= 0 && xx < w;
                 if (in) {
                     const __half* s = static_cast<const __half*>(src_) + (((long long)b * h + yy) * w + xx) * ld + c;
@@ -73,7 +70,7 @@ tap_gather_kernel(const void* __restrict__ src_, long long ld, __half* __restric
                 if (t < n_taps) {
                     int yy = y + taps.dy[t], xx = x + taps.dx[t];
                     bool in = true;
-                    if (reflect) { yy = reflect_idx(yy, h); xx = reflect_idx(xx, w); }
+                    if (reflect) { yy = reflect101(yy, h); xx = reflect101(xx, w); }
                     else in = yy >= 0 && yy < h && xx >= 0 && xx < w;
                     if (in) {
                         if (F32)
@@ -249,7 +246,7 @@ lineart_out_kernel(const __half* __restrict__ x, const float* __restrict__ wt, c
         __syncthreads();
         for (int i = threadIdx.x; i < kOW * kOW * (kOC / 2); i += 256) {
             const int cp = i % (kOC / 2), px = (i / (kOC / 2)) % kOW, py = i / (kOC / 2 * kOW);
-            const int yy = reflect_idx(min(y0 + py - kOP, h - 1 + kOP), h), xx = reflect_idx(min(x0 + px - kOP, w - 1 + kOP), w);
+            const int yy = reflect101(min(y0 + py - kOP, h - 1 + kOP), h), xx = reflect101(min(x0 + px - kOP, w - 1 + kOP), w);
             tile[cp][py][px] = reinterpret_cast<const __half2*>(xb + ((long long)yy * w + xx) * channels + c0)[cp];
         }
         for (int i = threadIdx.x; i < kOK * kOK * kOC; i += 256) wsm[i / kOC][i % kOC] = wt[(i / kOC) * channels + c0 + i % kOC];
@@ -338,16 +335,6 @@ lineart_anime_out_kernel(const __half* __restrict__ skip, const __half* __restri
     out[((long long)b * 2 * h + oy) * (2LL * w) + ox] = __fadd_rn(__fmul_rn(t, scale), shift);
 }
 
-static int launched_annot(cudaError_t e) {
-    if (e != cudaSuccess) return CTRLORA_ERR_CUDA;
-    return cudaGetLastError() == cudaSuccess ? CTRLORA_OK : CTRLORA_ERR_CUDA;
-}
-
-static unsigned grid_annot(long long items) {
-    const long long blocks = (items + 255) / 256;
-    return static_cast<unsigned>(blocks > 8192 ? 8192 : (blocks < 1 ? 1 : blocks));
-}
-
 // rows per statistics chunk: at most 1024 chunks per image, at least 64 rows each (a function of the image alone, so a
 // batch of B gives each image the statistics a batch of 1 gives it)
 constexpr int kNormMaxChunks = 1024;
@@ -384,12 +371,12 @@ static int tap_gather_launch(const void* src, int src_f32_nchw, long long ld, vo
     __half* d = static_cast<__half*>(dst);
     const bool vec = !src_f32_nchw && channels % 8 == 0 && ld % 8 == 0 && !(reinterpret_cast<uintptr_t>(src) & 15);
     if (vec)
-        return launched_annot(launch_pdl(tap_gather_kernel<true, false>, dim3(grid_annot(vecs)), dim3(256), (size_t)0, stream,
+        return launched(launch_pdl(tap_gather_kernel<true, false>, dim3(grid_blocks(vecs, 256, 8192)), dim3(256), (size_t)0, stream,
                                          src, ld, d, (int)vecs, h, w, channels, tl, n_taps, reflect, k_pad, stride, act));
     if (src_f32_nchw)
-        return launched_annot(launch_pdl(tap_gather_kernel<false, true>, dim3(grid_annot(vecs)), dim3(256), (size_t)0, stream,
+        return launched(launch_pdl(tap_gather_kernel<false, true>, dim3(grid_blocks(vecs, 256, 8192)), dim3(256), (size_t)0, stream,
                                          src, ld, d, (int)vecs, h, w, channels, tl, n_taps, reflect, k_pad, stride, act));
-    return launched_annot(launch_pdl(tap_gather_kernel<false, false>, dim3(grid_annot(vecs)), dim3(256), (size_t)0, stream,
+    return launched(launch_pdl(tap_gather_kernel<false, false>, dim3(grid_blocks(vecs, 256, 8192)), dim3(256), (size_t)0, stream,
                                      src, ld, d, (int)vecs, h, w, channels, tl, n_taps, reflect, k_pad, stride, act));
 }
 
@@ -422,13 +409,13 @@ extern "C" int ctrlora_instance_norm_f16(const void* x, const void* residual, vo
     float2* part = reinterpret_cast<float2*>(ws);
     float2* stats = part + (long long)batch * chunks * channels;
     const __half* xh = static_cast<const __half*>(x);
-    int rc = launched_annot(launch_pdl(inorm_partial_kernel, dim3(chunks, batch), dim3(256), (size_t)0, stream, xh, part,
+    int rc = launched(launch_pdl(inorm_partial_kernel, dim3(chunks, batch), dim3(256), (size_t)0, stream, xh, part,
                                        batch, hw, channels, phases, rows, chunk_rows, chunks));
     if (rc) return rc;
-    rc = launched_annot(launch_pdl(inorm_finalize_kernel, dim3((batch * channels + 7) / 8), dim3(256), (size_t)0, stream,
+    rc = launched(launch_pdl(inorm_finalize_kernel, dim3((batch * channels + 7) / 8), dim3(256), (size_t)0, stream,
                                    xh, (const float2*)part, stats, batch, hw, channels, phases, rows, chunks, eps));
     if (rc) return rc;
-    return launched_annot(launch_pdl(inorm_apply_kernel, dim3(grid_annot((long long)batch * rows * (channels / 8))), dim3(256),
+    return launched(launch_pdl(inorm_apply_kernel, dim3(grid_blocks((long long)batch * rows * (channels / 8), 256, 8192)), dim3(256),
                                      (size_t)0, stream, xh, static_cast<const __half*>(residual), static_cast<__half*>(y),
                                      (const float2*)stats, batch, hw, w, channels, phases, rows, relu));
 }
@@ -442,7 +429,7 @@ extern "C" int ctrlora_lineart_out_f16(const void* x, const float* weight, const
     if (batch == 0) return CTRLORA_OK;
     if (batch > 65535) return CTRLORA_ERR_UNSUPPORTED;
     const dim3 grid((w + kOT - 1) / kOT, (h + kOT - 1) / kOT, batch);
-    return launched_annot(launch_pdl(lineart_out_kernel, grid, dim3(256), (size_t)0, stream, static_cast<const __half*>(x),
+    return launched(launch_pdl(lineart_out_kernel, grid, dim3(256), (size_t)0, stream, static_cast<const __half*>(x),
                                      weight, bias, out, out_u8, h, w, channels));
 }
 
@@ -456,7 +443,7 @@ extern "C" int ctrlora_lineart_anime_out_f16(const void* skip, const void* up, c
     if (batch == 0) return CTRLORA_OK;
     if (batch > 65535) return CTRLORA_ERR_UNSUPPORTED;
     const dim3 grid((2 * w + kAT - 1) / kAT, (2 * h + kAT - 1) / kAT, batch);
-    return launched_annot(launch_pdl(lineart_anime_out_kernel, grid, dim3(256), (size_t)0, stream,
+    return launched(launch_pdl(lineart_anime_out_kernel, grid, dim3(256), (size_t)0, stream,
                                      static_cast<const __half*>(skip), static_cast<const __half*>(up), weight, bias, out, h,
                                      w, channels, scale, shift));
 }

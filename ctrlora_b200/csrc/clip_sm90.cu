@@ -245,11 +245,6 @@ layernorm_rows_kernel(const void* __restrict__ x, int x_f32, long long ldx, void
     }
 }
 
-static int launched(cudaError_t e) {
-    if (e != cudaSuccess) return CTRLORA_ERR_CUDA;
-    return cudaGetLastError() == cudaSuccess ? CTRLORA_OK : CTRLORA_ERR_CUDA;
-}
-
 }  // namespace ctrl
 
 using namespace ctrl;

@@ -79,16 +79,6 @@ __global__ void __launch_bounds__(256) gelu_erf_kernel(__half* __restrict__ x, l
     }
 }
 
-static int launched_vision(cudaError_t e) {
-    if (e != cudaSuccess) return CTRLORA_ERR_CUDA;
-    return cudaGetLastError() == cudaSuccess ? CTRLORA_OK : CTRLORA_ERR_CUDA;
-}
-
-static unsigned grid_for(long long vecs) {
-    const long long blocks = (vecs + 255) / 256;
-    return static_cast<unsigned>(blocks > 4096 ? 4096 : blocks);
-}
-
 }  // namespace ctrl
 
 using namespace ctrl;
@@ -103,10 +93,10 @@ static int patch_gather_launch(const void* pixels, int pixels_f32, void* out, in
     if (vecs == 0) return CTRLORA_OK;
     __half* o = static_cast<__half*>(out);
     if (pixels_f32)
-        return launched_vision(launch_pdl(patch_gather_kernel<float>, dim3(grid_for(vecs)), dim3(256), (size_t)0, stream,
+        return launched(launch_pdl(patch_gather_kernel<float>, dim3(grid_blocks(vecs, 256, 4096)), dim3(256), (size_t)0, stream,
                                           static_cast<const float*>(pixels), o, vecs, channels, img_h, img_w, grid_h, grid_w,
                                           patch, k_pad));
-    return launched_vision(launch_pdl(patch_gather_kernel<__half>, dim3(grid_for(vecs)), dim3(256), (size_t)0, stream,
+    return launched(launch_pdl(patch_gather_kernel<__half>, dim3(grid_blocks(vecs, 256, 4096)), dim3(256), (size_t)0, stream,
                                       static_cast<const __half*>(pixels), o, vecs, channels, img_h, img_w, grid_h, grid_w,
                                       patch, k_pad));
 }
@@ -133,7 +123,7 @@ extern "C" int ctrlora_clip_vision_embed(const float* patch_out, long long ldp, 
         return CTRLORA_ERR_ARG;
     const int rows = batch * (patches + 1);
     if (rows == 0) return CTRLORA_OK;
-    return launched_vision(launch_pdl(vision_embed_kernel, dim3((rows + 7) / 8), dim3(256), (size_t)0, stream, patch_out, ldp,
+    return launched(launch_pdl(vision_embed_kernel, dim3((rows + 7) / 8), dim3(256), (size_t)0, stream, patch_out, ldp,
                                       class_embedding, position_embedding, out, rows, patches, cols));
 }
 
@@ -142,6 +132,6 @@ extern "C" int ctrlora_gelu_f16(void* x, long long n, void* stream_) {
     if (!x || n < 0 || n % 8) return CTRLORA_ERR_ARG;
     const long long vecs = n / 8;
     if (vecs == 0) return CTRLORA_OK;
-    return launched_vision(launch_pdl(gelu_erf_kernel, dim3(grid_for(vecs)), dim3(256), (size_t)0, stream,
+    return launched(launch_pdl(gelu_erf_kernel, dim3(grid_blocks(vecs, 256, 4096)), dim3(256), (size_t)0, stream,
                                       static_cast<__half*>(x), vecs));
 }

@@ -379,4 +379,18 @@ __device__ __forceinline__ float exp2_poly4(float x) {
     p = fmaf(p, f, 0.99999928f);
     return __int_as_float(__float_as_int(p) + (__float_as_int(t) << 23));
 }
+// nn.ReflectionPad2d's and cv2's BORDER_REFLECT_101 index map: the border pixel is not repeated (needs |offset| < n)
+__device__ __forceinline__ int reflect101(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }
+
+// ---------------------------------------------------------------- host-side launch helpers
+// an entry point's status after a launch: the launch's own error, else any error pending from earlier work
+inline int launched(cudaError_t e) {
+    if (e != cudaSuccess) return CTRLORA_ERR_CUDA;
+    return cudaGetLastError() == cudaSuccess ? CTRLORA_OK : CTRLORA_ERR_CUDA;
+}
+// blocks of a grid-stride kernel over `items` at `per_block` per block, clamped to [1, cap]
+inline unsigned grid_blocks(long long items, int per_block, long long cap) {
+    const long long blocks = (items + per_block - 1) / per_block;
+    return static_cast<unsigned>(blocks > cap ? cap : (blocks < 1 ? 1 : blocks));
+}
 }  // namespace ctrl

@@ -133,16 +133,6 @@ hed_fuse_kernel(const __grid_constant__ HedFuseMaps m, float* __restrict__ mean,
     }
 }
 
-static int launched_hed(cudaError_t e) {
-    if (e != cudaSuccess) return CTRLORA_ERR_CUDA;
-    return cudaGetLastError() == cudaSuccess ? CTRLORA_OK : CTRLORA_ERR_CUDA;
-}
-
-static unsigned grid_hed(long long items, int per_block) {
-    const long long blocks = (items + per_block - 1) / per_block;
-    return static_cast<unsigned>(blocks > 8192 ? 8192 : (blocks < 1 ? 1 : blocks));
-}
-
 }  // namespace ctrl
 
 using namespace ctrl;
@@ -163,18 +153,18 @@ extern "C" int ctrlora_hed_side_pool_f16(const void* x, const float* weight, con
     const int per_block = 8 * (32 / (channels / (8 * nv)));  // quads of one 256-thread block
     const __half* xh = static_cast<const __half*>(x);
     __half* ph = static_cast<__half*>(pooled);
-    const dim3 grid(grid_hed(quads, per_block));
+    const dim3 grid(grid_blocks(quads, per_block, 8192));
     if (!with_side) {
         if (nv == 2)
-            return launched_hed(launch_pdl(hed_side_pool_kernel<2, false>, grid, dim3(256), (size_t)0, stream, xh, weight,
+            return launched(launch_pdl(hed_side_pool_kernel<2, false>, grid, dim3(256), (size_t)0, stream, xh, weight,
                                            bias, side, ph, h, w, channels, quads, qh, qw));
-        return launched_hed(launch_pdl(hed_side_pool_kernel<1, false>, grid, dim3(256), (size_t)0, stream, xh, weight, bias,
+        return launched(launch_pdl(hed_side_pool_kernel<1, false>, grid, dim3(256), (size_t)0, stream, xh, weight, bias,
                                        side, ph, h, w, channels, quads, qh, qw));
     }
     if (nv == 2)
-        return launched_hed(launch_pdl(hed_side_pool_kernel<2, true>, grid, dim3(256), (size_t)0, stream, xh, weight, bias,
+        return launched(launch_pdl(hed_side_pool_kernel<2, true>, grid, dim3(256), (size_t)0, stream, xh, weight, bias,
                                        side, ph, h, w, channels, quads, qh, qw));
-    return launched_hed(launch_pdl(hed_side_pool_kernel<1, true>, grid, dim3(256), (size_t)0, stream, xh, weight, bias,
+    return launched(launch_pdl(hed_side_pool_kernel<1, true>, grid, dim3(256), (size_t)0, stream, xh, weight, bias,
                                    side, ph, h, w, channels, quads, qh, qw));
 }
 
@@ -200,6 +190,6 @@ extern "C" int ctrlora_hed_fuse(const float* const* sides, const int* side_hw, c
     }
     const long long n = (long long)batch * h * w;
     if (n == 0) return CTRLORA_OK;
-    return launched_hed(launch_pdl(hed_fuse_kernel, dim3(grid_hed(n, 256)), dim3(256), (size_t)0, stream, m, mean, out_u8,
+    return launched(launch_pdl(hed_fuse_kernel, dim3(grid_blocks(n, 256, 8192)), dim3(256), (size_t)0, stream, m, mean, out_u8,
                                    batch, h, w, safe));
 }

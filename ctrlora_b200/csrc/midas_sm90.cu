@@ -12,16 +12,6 @@
 
 namespace ctrl {
 
-static int launched_midas(cudaError_t e) {
-    if (e != cudaSuccess) return CTRLORA_ERR_CUDA;
-    return cudaGetLastError() == cudaSuccess ? CTRLORA_OK : CTRLORA_ERR_CUDA;
-}
-
-static unsigned grid_midas(long long items) {
-    const long long blocks = (items + 255) / 256;
-    return static_cast<unsigned>(blocks > 8192 ? 8192 : blocks);
-}
-
 static bool misaligned(const void* p, int bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) != 0; }
 
 // ------------------------------------------------------------------------------------------ depth to space + bias
@@ -194,8 +184,6 @@ __device__ __forceinline__ unsigned char to_u8(float v) {
     return static_cast<unsigned char>(static_cast<int>(fminf(fmaxf(v, 0.f), 255.f)));
 }
 
-__device__ __forceinline__ int reflect101(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }
-
 // MidasDetector.__call__ after the network, restated in fp32 with every product and sum rounded on its own (no FMA
 // contraction), as numpy and cv2 compute them:
 //   depth_pt = (d - min) / (max - min);  depth_u8 = u8(depth_pt * 255)
@@ -249,7 +237,7 @@ extern "C" int ctrlora_depth_to_space_bias(const float* src, const float* bias, 
         return CTRLORA_ERR_ARG;
     const long long items = (long long)batch * h * s * w * s * (channels / 4);
     if (items == 0) return CTRLORA_OK;
-    return launched_midas(launch_pdl(depth_to_space_kernel, dim3(grid_midas(items)), dim3(256), (size_t)0, stream, src, bias,
+    return launched(launch_pdl(depth_to_space_kernel, dim3(grid_blocks(items, 256, 8192)), dim3(256), (size_t)0, stream, src, bias,
                                      static_cast<__half*>(dst), items, h, w, channels, s));
 }
 
@@ -260,7 +248,7 @@ extern "C" int ctrlora_add_relu_f16(const void* a, const void* b, void* sum, voi
         return CTRLORA_ERR_ARG;
     const long long vecs = n / 8;
     if (vecs == 0) return CTRLORA_OK;
-    return launched_midas(launch_pdl(add_relu_kernel, dim3(grid_midas(vecs)), dim3(256), (size_t)0, stream,
+    return launched(launch_pdl(add_relu_kernel, dim3(grid_blocks(vecs, 256, 8192)), dim3(256), (size_t)0, stream,
                                      static_cast<const __half*>(a), static_cast<const __half*>(b), static_cast<__half*>(sum),
                                      static_cast<__half*>(relu), vecs));
 }
@@ -273,7 +261,7 @@ extern "C" int ctrlora_upsample_bilinear2x_f16(const void* src, void* dst, int b
         return CTRLORA_ERR_ARG;
     const long long items = (long long)batch * 2 * h * 2 * w * (channels / 8);
     if (items == 0) return CTRLORA_OK;
-    return launched_midas(launch_pdl(upsample_bilinear2x_kernel, dim3(grid_midas(items)), dim3(256), (size_t)0, stream,
+    return launched(launch_pdl(upsample_bilinear2x_kernel, dim3(grid_blocks(items, 256, 8192)), dim3(256), (size_t)0, stream,
                                      static_cast<const __half*>(src), static_cast<__half*>(dst), items, h, w, channels));
 }
 
@@ -284,7 +272,7 @@ extern "C" int ctrlora_midas_head_out_f16(const void* x, const float* weight, co
         misaligned(x, 16))
         return CTRLORA_ERR_ARG;
     if (pixels == 0) return CTRLORA_OK;
-    return launched_midas(launch_pdl(midas_head_out_kernel, dim3(grid_midas(pixels)), dim3(256), (size_t)0, stream,
+    return launched(launch_pdl(midas_head_out_kernel, dim3(grid_blocks(pixels, 256, 8192)), dim3(256), (size_t)0, stream,
                                      static_cast<const __half*>(x), weight, bias, out, pixels, channels));
 }
 
@@ -295,9 +283,9 @@ extern "C" int ctrlora_midas_maps(const float* depth, float* minmax, unsigned ch
         return CTRLORA_ERR_ARG;
     if (batch == 0) return CTRLORA_OK;
     const long long hw = (long long)h * w;
-    const int rc = launched_midas(launch_pdl(midas_minmax_kernel, dim3(batch), dim3(1024), (size_t)0, stream, depth, minmax,
+    const int rc = launched(launch_pdl(midas_minmax_kernel, dim3(batch), dim3(1024), (size_t)0, stream, depth, minmax,
                                              hw));
     if (rc) return rc;
-    return launched_midas(launch_pdl(midas_maps_kernel, dim3(grid_midas(batch * hw)), dim3(256), (size_t)0, stream, depth,
+    return launched(launch_pdl(midas_maps_kernel, dim3(grid_blocks(batch * hw, 256, 8192)), dim3(256), (size_t)0, stream, depth,
                                      (const float*)minmax, depth_u8, normal_u8, batch * hw, h, w, a, bg_th));
 }

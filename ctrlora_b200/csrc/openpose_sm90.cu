@@ -227,16 +227,6 @@ openpose_limb_kernel(const float* __restrict__ paf, int ld, int w8, const Resamp
     }
 }
 
-static int launched_op(cudaError_t e) {
-    if (e != cudaSuccess) return CTRLORA_ERR_CUDA;
-    return cudaGetLastError() == cudaSuccess ? CTRLORA_OK : CTRLORA_ERR_CUDA;
-}
-
-static unsigned grid_op(long long items, int per_block) {
-    const long long blocks = (items + per_block - 1) / per_block;
-    return static_cast<unsigned>(blocks > 8192 ? 8192 : (blocks < 1 ? 1 : blocks));
-}
-
 static bool tabs_ok(const ResampleTabs& t) { return t.y_start && t.y_w && t.x_start && t.x_w && t.ty >= 1 && t.tx >= 1; }
 
 }  // namespace ctrl
@@ -251,9 +241,9 @@ extern "C" int ctrlora_openpose_resample(const float* maps, int map_ld, int h8, 
     const ResampleTabs t{y_start, y_w, x_start, x_w, ty, tx};
     if (!tabs_ok(t)) return CTRLORA_ERR_ARG;
     const long long n = (long long)channels * h * w;
-    openpose_resample_kernel<<<grid_op(n, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(maps, map_ld, w8,
+    openpose_resample_kernel<<<grid_blocks(n, 256, 8192), 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(maps, map_ld, w8,
                                                                                                       channels, t, out, h, w);
-    return launched_op(cudaSuccess);
+    return launched(cudaSuccess);
 }
 
 extern "C" int ctrlora_openpose_smooth(const float* in, double* tmp, double* out, int maps, int h, int w,
@@ -267,9 +257,9 @@ extern "C" int ctrlora_openpose_smooth(const float* in, double* tmp, double* out
     const long long n = (long long)maps * h * w;
     if (n == 0) return CTRLORA_OK;
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    openpose_smooth_kernel<float, true><<<grid_op(n, 256), 256, 0, stream>>>(in, tmp, maps, h, w, g);
-    openpose_smooth_kernel<double, false><<<grid_op(n, 256), 256, 0, stream>>>(tmp, out, maps, h, w, g);
-    return launched_op(cudaSuccess);
+    openpose_smooth_kernel<float, true><<<grid_blocks(n, 256, 8192), 256, 0, stream>>>(in, tmp, maps, h, w, g);
+    openpose_smooth_kernel<double, false><<<grid_blocks(n, 256, 8192), 256, 0, stream>>>(tmp, out, maps, h, w, g);
+    return launched(cudaSuccess);
 }
 
 extern "C" int ctrlora_openpose_peaks(const double* smoothed, const float* heat, int maps, int h, int w, double thre,
@@ -287,7 +277,7 @@ extern "C" int ctrlora_openpose_peaks(const double* smoothed, const float* heat,
     openpose_peak_scan_kernel<<<1, kPeakThreads, 0, stream>>>(ws, static_cast<int>(blocks));
     openpose_peak_write_kernel<<<nb, kPeakThreads, 0, stream>>>(smoothed, heat, n, h, w, thre, ws, px, py, part, score,
                                                                 capacity);
-    return launched_op(cudaSuccess);
+    return launched(cudaSuccess);
 }
 
 extern "C" int ctrlora_openpose_limbs(const float* paf, int paf_ld, int h8, int w8, const int* y_start, const double* y_w,
@@ -313,7 +303,7 @@ extern "C" int ctrlora_openpose_limbs(const float* paf, int paf_ld, int h8, int 
         next += (long long)L.d[k][2] * L.d[k][4];
     }
     if (next != pairs) return CTRLORA_ERR_ARG;
-    openpose_limb_kernel<<<grid_op(pairs, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
+    openpose_limb_kernel<<<grid_blocks(pairs, 256, 8192), 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
         paf, paf_ld, w8, t, px, py, L, pairs, img_h, thre, score, ok);
-    return launched_op(cudaSuccess);
+    return launched(cudaSuccess);
 }

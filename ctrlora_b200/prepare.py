@@ -106,6 +106,21 @@ def conv_weight(weight, pad_in=None, pad_out=None):
     return w
 
 
+def flat_conv_weight(weight, k_multiple=1):
+    """nn.Conv2d weight fp32 [Cout, Cin, kh, kw] -> fp16 [Cout, 1, K]: conv_weight's tap-major, channel-minor order as
+    one row per output channel (the order of the tap gather and im2col_s2), zero-padded to a multiple of k_multiple."""
+    w = conv_weight(weight)
+    co, taps, ci = w.shape
+    k = taps * ci
+    w = w.view(co, 1, k)
+    k_pad = (k + k_multiple - 1) // k_multiple * k_multiple
+    if k_pad == k:
+        return w
+    full = torch.zeros((co, 1, k_pad), device=w.device, dtype=torch.float16)
+    full[:, :, :k] = w
+    return full
+
+
 def lora_folded_weight(weight, down, up, scale=1.0, out=None):
     """W' = W + scale * up @ down as fp16 [N, 1, K]  (cldm/lora.py:250 `_fuse_lora`, evaluated in fp32 accumulate).
 

@@ -39,3 +39,13 @@ def synth_state_dict(shapes, seed=0, prefix=""):
 
 def synth_input(name, shape, seed=0, scale=1.0):
     return torch.from_numpy(_rs("input." + name, seed).standard_normal(tuple(shape)).astype(np.float32) * scale)
+
+
+def noise_image(name, seed, h, w, block, amp):
+    """uint8 HWC [h, w, 3] test image: block x block squares of coarse noise (edges for a detector) plus fine noise in
+    [-amp, amp)"""
+    rs = _rs(name, seed)
+    nh, nw = (h + block - 1) // block, (w + block - 1) // block
+    coarse = rs.uniform(0, 1, (nh, nw, 3)).repeat(block, 0).repeat(block, 1)[:h, :w]
+    fine = rs.uniform(-amp, amp, (h, w, 3))
+    return np.clip((coarse + fine) * 255.0, 0, 255).astype(np.uint8)

@@ -1,10 +1,16 @@
 """Golden fixtures larger than PART_BYTES are stored as <stem>.pt plus <stem>.part<i>.pt: every file stays small enough
-for the repository, the content is unchanged.  load_golden() reassembles the dict that save_golden() was given."""
+for the repository, the content is unchanged.  load_golden() reassembles the dict that save_golden() was given.
+
+Large activations are stored at a sample of pixel positions (stage_positions, sample_stage) and full-size maps in bands
+of rows (bands, unband): the part splitter moves whole entries, so each band is an entry of its own."""
 import glob
 import io
 import os
 
+import numpy as np
 import torch
+
+from oracle import synth
 
 PART_BYTES = 900 * 1024
 
@@ -48,6 +54,29 @@ def save_golden(g, path):
     torch.save(pack(parts[0]), path)
     for i, its in enumerate(parts[1:], 1):
         torch.save(pack(its), f"{stem}.part{i}.pt")
+
+
+def stage_positions(prefix, seed, floats, h, w, channels):
+    """sorted flat pixel indices (row-major over h x w) at which a stage of `channels` channels is stored: about
+    `floats` values, at least one position"""
+    n = min(h * w, max(1, floats // channels))
+    rs = synth._rs(f"{prefix}.positions.{h}x{w}x{channels}", seed)
+    return np.sort(rs.choice(h * w, n, replace=False))
+
+
+def sample_stage(t, idx):
+    """fp32 [1, C, h, w] stage -> [C, len(idx)] at the given flat pixel indices"""
+    return t[0].reshape(t.shape[1], -1)[:, torch.as_tensor(idx, device=t.device)].float().cpu().contiguous()
+
+
+def bands(t, rows):
+    """[H, ...] -> {band name: `rows` rows}"""
+    return {f"rows{r:05d}": t[r:r + rows].clone() for r in range(0, t.shape[0], rows)}
+
+
+def unband(d):
+    """the tensor that `bands` split"""
+    return torch.cat([d[k] for k in sorted(d)])
 
 
 def load_golden(path):

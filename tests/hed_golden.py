@@ -8,16 +8,20 @@ the activations by 2^13), and the projections are scaled and offset so that the 
 about 2, which spreads the uint8 map and safe_step's bins.  Stage activations (the five blocks' outputs) are stored at a fixed sample
 of pixel positions with all their channels.
 """
+import functools
+
 import cv2
 import numpy as np
 import torch
 
+import golden_io
+from golden_io import sample_stage, unband  # noqa: F401 (sample_stage)
 from oracle import synth
 
 SEED = 13
 SIZES = {"512": (512, 512), "384x640": (384, 640), "200x328": (200, 328)}
 STAGE_FLOATS = 16384                                 # per stored stage: positions = STAGE_FLOATS // channels
-MAP_BAND_ROWS = 128                                  # full-size fp32 maps are stored in bands of rows (see map_bands)
+MAP_BAND_ROWS = 128                                  # full-size fp32 maps are stored in bands of rows
 PROJ_SCALE = 0.12                                    # on top of synth's fan_in ** -0.5 (see the module docstring)
 # projection biases that centre each side map of the test images near 0 (measured once at 200 x 328)
 PROJ_BIAS = (2.0, -6.9, -4.6, 0.3, -13.3)
@@ -42,34 +46,16 @@ def weights(shapes):
 def image(size, tag=""):
     """uint8 HWC [H, W, 3] test image: 16-pixel blocks of coarse noise (edges for the detector) plus fine noise"""
     h, w = SIZES[size] if size in SIZES else size
-    rs = synth._rs(f"hed.image.{h}x{w}{tag}", SEED)
-    coarse = rs.uniform(0, 1, ((h + 15) // 16, (w + 15) // 16, 3)).repeat(16, 0).repeat(16, 1)[:h, :w]
-    fine = rs.uniform(-0.15, 0.15, (h, w, 3))
-    return np.clip((coarse + fine) * 255.0, 0, 255).astype(np.uint8)
+    return synth.noise_image(f"hed.image.{h}x{w}{tag}", SEED, h, w, 16, 0.15)
 
 
-def stage_positions(h, w, channels):
-    """sorted flat pixel indices (row-major over h x w) at which a stage is stored"""
-    n = min(h * w, STAGE_FLOATS // channels)
-    rs = synth._rs(f"hed.positions.{h}x{w}x{channels}", SEED)
-    return np.sort(rs.choice(h * w, n, replace=False))
-
-
-def sample_stage(t, idx):
-    """fp32 [1, C, h, w] stage -> [C, len(idx)] at the given flat pixel indices"""
-    return t[0].reshape(t.shape[1], -1)[:, torch.as_tensor(idx, device=t.device)].float().cpu().contiguous()
-
-
-def map_bands(m):
-    """fp32 [H, W] map -> {band name: rows}: a 512 x 512 map is 1 MB, more than one fixture part file may hold, and the
-    part splitter moves whole entries, so each band is an entry of its own"""
-    return {f"rows{r:05d}": m[r:r + MAP_BAND_ROWS].clone() for r in range(0, m.shape[0], MAP_BAND_ROWS)}
+stage_positions = functools.partial(golden_io.stage_positions, "hed", SEED, STAGE_FLOATS)
+map_bands = functools.partial(golden_io.bands, rows=MAP_BAND_ROWS)  # a 512 x 512 map is 1 MB, more than a part file
 
 
 def golden_map(golden, size, name):
     """a full-size fp32 [H, W] map ("mean" or "e1") of one size, reassembled from its bands"""
-    bands = golden[f"{size}.{name}"]
-    return torch.cat([bands[k] for k in sorted(bands)])
+    return unband(golden[f"{size}.{name}"])
 
 
 def dark(edge):

@@ -6,11 +6,13 @@ bits), so the fixture holds the reference's outputs, the state-dict keys and sha
 outputs (blocks 1 ... 7 of UnetGenerator(3, 1, 8)) are stored at a fixed sample of pixel positions with all their
 channels: whole blocks at 512 x 768 would be hundreds of MB.
 """
+import functools
 import zlib
 
-import numpy as np
 import torch
 
+import golden_io
+from golden_io import sample_stage, unband  # noqa: F401 (sample_stage)
 from oracle import synth
 
 SEED = 23
@@ -20,7 +22,7 @@ NUM_DOWNS = 8                                        # LineartAnimeDetector buil
 SIZES = {"256": (256, 256), "512": (512, 512), "512x768": (512, 768)}
 DETECTOR_SIZE = (500, 740)                           # not a multiple of 256: both cubic resizes run
 STAGE_FLOATS = 16384                                 # per stored block output: positions = STAGE_FLOATS // channels
-MAP_BAND_ROWS = 128                                  # the fp32 map is stored in bands of rows (see map_bands)
+MAP_BAND_ROWS = 128                                  # the fp32 map is stored in bands of rows
 OUT_CONV = "model.model.3.weight"                    # block 0's ConvTranspose2d(128 -> 1)
 OUT_CONV_SCALE = 0.125
 
@@ -37,10 +39,7 @@ def weights(shapes):
 def image(size, tag=""):
     """uint8 HWC [H, W, 3] test image: 16-pixel blocks of coarse noise (edges for the detector) plus fine noise"""
     h, w = SIZES[size] if size in SIZES else size
-    rs = synth._rs(f"lineart_anime.image.{h}x{w}{tag}", SEED)
-    coarse = rs.uniform(0, 1, ((h + 15) // 16, (w + 15) // 16, 3)).repeat(16, 0).repeat(16, 1)[:h, :w]
-    fine = rs.uniform(-0.15, 0.15, (h, w, 3))
-    return np.clip((coarse + fine) * 255.0, 0, 255).astype(np.uint8)
+    return synth.noise_image(f"lineart_anime.image.{h}x{w}{tag}", SEED, h, w, 16, 0.15)
 
 
 def image_tensor(img):
@@ -49,27 +48,13 @@ def image_tensor(img):
     return (torch.from_numpy(img).float() / 127.5 - 1.0).permute(2, 0, 1).unsqueeze(0).contiguous()
 
 
-def stage_positions(h, w, channels):
-    """sorted flat pixel indices (row-major over h x w) at which a block output is stored"""
-    n = min(h * w, max(1, STAGE_FLOATS // channels))
-    rs = synth._rs(f"lineart_anime.positions.{h}x{w}x{channels}", SEED)
-    return np.sort(rs.choice(h * w, n, replace=False))
-
-
-def sample_stage(t, idx):
-    """fp32 [1, C, h, w] block output -> [C, len(idx)] at the given flat pixel indices"""
-    return t[0].reshape(t.shape[1], -1)[:, torch.as_tensor(idx, device=t.device)].float().cpu().contiguous()
-
-
-def map_bands(line):
-    """fp32 [H, W] map -> {band name: rows}: the part splitter moves whole entries, so each band is an entry of its own"""
-    return {f"rows{r:05d}": line[r:r + MAP_BAND_ROWS].clone() for r in range(0, line.shape[0], MAP_BAND_ROWS)}
+stage_positions = functools.partial(golden_io.stage_positions, "lineart_anime", SEED, STAGE_FLOATS)
+map_bands = functools.partial(golden_io.bands, rows=MAP_BAND_ROWS)
 
 
 def golden_map(golden, size):
     """the fp32 [H, W] network output of one size, reassembled from its bands"""
-    bands = golden[f"{size}.map"]
-    return torch.cat([bands[k] for k in sorted(bands)])
+    return unband(golden[f"{size}.map"])
 
 
 # ---- the line-art kernels' existing calls, recorded from the library before 512-channel norms and strided gathers

@@ -11,9 +11,12 @@ activations, and scales the ViT's residual-branch output projections (attn.proj,
 24 blocks do not grow the stream's norm by orders of magnitude.  The normal map then has structure: the depth has
 edges at the image's 16-pixel blocks.
 """
-import numpy as np
+import functools
+
 import torch
 
+import golden_io
+from golden_io import unband  # noqa: F401
 from oracle import synth
 
 SEED = 31
@@ -39,10 +42,7 @@ def weights(shapes):
 def image(size, tag=""):
     """uint8 HWC [H, W, 3] test image: 16-pixel blocks of coarse noise plus fine noise"""
     h, w = SIZES[size] if size in SIZES else size
-    rs = synth._rs(f"midas.image.{h}x{w}{tag}", SEED)
-    coarse = rs.uniform(0, 1, ((h + 15) // 16, (w + 15) // 16, 3)).repeat(16, 0).repeat(16, 1)[:h, :w]
-    fine = rs.uniform(-0.15, 0.15, (h, w, 3))
-    return np.clip((coarse + fine) * 255.0, 0, 255).astype(np.uint8)
+    return synth.noise_image(f"midas.image.{h}x{w}{tag}", SEED, h, w, 16, 0.15)
 
 
 def image_tensor(img):
@@ -50,10 +50,4 @@ def image_tensor(img):
     return (torch.from_numpy(img).float() / 127.5 - 1.0).permute(2, 0, 1).unsqueeze(0).contiguous()
 
 
-def bands(t):
-    """[H, ...] -> {band name: rows}: the part splitter moves whole entries, so each band is an entry of its own"""
-    return {f"rows{r:05d}": t[r:r + MAP_BAND_ROWS].clone() for r in range(0, t.shape[0], MAP_BAND_ROWS)}
-
-
-def unband(d):
-    return torch.cat([d[k] for k in sorted(d)])
+bands = functools.partial(golden_io.bands, rows=MAP_BAND_ROWS)

@@ -55,10 +55,7 @@ def weights(shapes):
 def image(size, tag=""):
     """uint8 HWC [H, W, 3] test image: 8-pixel blocks of coarse noise plus fine noise"""
     h, w = NET_SIZES[size] if size in NET_SIZES else size
-    rs = synth._rs(f"openpose.image.{h}x{w}{tag}", SEED)
-    coarse = rs.uniform(0, 1, ((h + 7) // 8, (w + 7) // 8, 3)).repeat(8, 0).repeat(8, 1)[:h, :w]
-    fine = rs.uniform(-0.2, 0.2, (h, w, 3))
-    return np.clip((coarse + fine) * 255.0, 0, 255).astype(np.uint8)
+    return synth.noise_image(f"openpose.image.{h}x{w}{tag}", SEED, h, w, 8, 0.2)
 
 
 def _blob(h8, w8, cx, cy, amp=1.0):
