@@ -146,6 +146,10 @@ _ARGTYPES = {
     "ctrlora_upsample_bilinear2x_f16": [_P, _P, _I, _I, _I, _I, _P],
     "ctrlora_midas_head_out_f16": [_P, _P, _P, _P, _L, _I, _P],
     "ctrlora_midas_maps": [_P, _P, _P, _P, _I, _I, _I, _F, _F, _P],
+    "ctrlora_dwconv_f16": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P],
+    "ctrlora_resize_bilinear_f16": [_P, _I, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P],
+    "ctrlora_adaptive_avg_pool_f16": [_P, _I, _P, _I, _I, _I, _I, _P, _I, _P],
+    "ctrlora_seg_output": [_P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P],
 }
 
 
@@ -243,4 +247,8 @@ EXPORTS = [
     "ctrlora_upsample_bilinear2x_f16",
     "ctrlora_midas_head_out_f16",
     "ctrlora_midas_maps",
+    "ctrlora_dwconv_f16",
+    "ctrlora_resize_bilinear_f16",
+    "ctrlora_adaptive_avg_pool_f16",
+    "ctrlora_seg_output",
 ]

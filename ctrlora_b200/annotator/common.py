@@ -1,5 +1,6 @@
 """What every annotator shares: the checkpoint lookup, the frozen-network setup and device check, a bounded cache of
-size-keyed tables, the 3x3 tap list, the sub-pixel split of a stride-2 ConvTranspose2d and cv2's linear resize rule."""
+size-keyed tables, the 3x3 tap list, the sub-pixel split of a stride-2 ConvTranspose2d, cv2's linear resize rule and
+the kernel copies of a ViT-style block's weights."""
 import collections
 import os
 
@@ -109,3 +110,24 @@ def linear_src_coord(src, dst):
     f = ((np.arange(dst, dtype=np.float64) + 0.5) * scale - 0.5).astype(np.float32)
     sx = np.floor(f).astype(np.int64)
     return sx, (f - sx.astype(np.float32)).astype(np.float32)
+
+
+def vit_block_weights(prep, blk, i):
+    """text_encoder.layer_weights for a timm-style pre-norm block (norm1, attn.qkv, attn.proj, norm2, mlp.fc1, mlp.fc2;
+    MiDaS's ViT, UniFormer's SABlock): the fused qkv Linear is already the stacked q | k | v weight.  i keys the
+    block's entries in the PrepCache."""
+    at, mlp = blk.attn, blk.mlp
+
+    def lin(m):
+        return lambda: (prepare.linear_weight(m.weight), prepare.bias_f32(m.bias))
+
+    def ln(m):
+        return lambda: (prepare.bias_f32(m.weight), prepare.bias_f32(m.bias), m.eps)
+
+    get = prep.get
+    return (get(("qkv", i), [at.qkv.weight, at.qkv.bias], lin(at.qkv)),
+            get(("proj", i), [at.proj.weight, at.proj.bias], lin(at.proj)),
+            get(("fc1", i), [mlp.fc1.weight, mlp.fc1.bias], lin(mlp.fc1)),
+            get(("fc2", i), [mlp.fc2.weight, mlp.fc2.bias], lin(mlp.fc2)),
+            get(("ln1", i), [blk.norm1.weight, blk.norm1.bias], ln(blk.norm1)),
+            get(("ln2", i), [blk.norm2.weight, blk.norm2.bias], ln(blk.norm2)))

@@ -35,7 +35,7 @@ import torch.nn.functional as F
 
 from .. import ops, prepare
 from ..text_encoder import run_layers
-from .common import SizeCache, checkpoint_path, device_input, freeze
+from .common import SizeCache, checkpoint_path, device_input, freeze, vit_block_weights
 
 HOOKS = (5, 11, 17, 23)             # vitl16_384's hooked blocks
 FEATURES = (256, 512, 1024, 1024)   # reassemble widths
@@ -150,25 +150,6 @@ def load_checkpoint(path):
     return params
 
 
-def _block_weights(prep, blk, i):
-    """text_encoder.layer_weights for a timm Block: the fused qkv Linear is already the stacked q | k | v weight"""
-    at, mlp = blk.attn, blk.mlp
-
-    def lin(m):
-        return lambda: (prepare.linear_weight(m.weight), prepare.bias_f32(m.bias))
-
-    def ln(m):
-        return lambda: (prepare.bias_f32(m.weight), prepare.bias_f32(m.bias), m.eps)
-
-    get = prep.get
-    return (get(("qkv", i), [at.qkv.weight, at.qkv.bias], lin(at.qkv)),
-            get(("proj", i), [at.proj.weight, at.proj.bias], lin(at.proj)),
-            get(("fc1", i), [mlp.fc1.weight, mlp.fc1.bias], lin(mlp.fc1)),
-            get(("fc2", i), [mlp.fc2.weight, mlp.fc2.bias], lin(mlp.fc2)),
-            get(("ln1", i), [blk.norm1.weight, blk.norm1.bias], ln(blk.norm1)),
-            get(("ln2", i), [blk.norm2.weight, blk.norm2.bias], ln(blk.norm2)))
-
-
 class DPTDepthModel(nn.Module):
     """The reference's DPTDepthModel(path, backbone="vitl16_384", non_negative=True) (readout "project", 256 features);
     forward(x fp32 [B, 3, H, W]) -> fp32 [B, 16 gh, 16 gw].  Other configurations raise NotImplementedError.
@@ -278,7 +259,7 @@ class DPTDepthModel(nn.Module):
         patch = ops.gemm(rows, w_patch, bias=b_patch, out_f32=True, split_k=self.split_k)
         h = ops.clip_vision_embed(patch, self._f32("cls", vit.cls_token), self.pos_table(gh, gw), b)
         _, kept = run_layers(vit.blocks[:HOOKS[-1] + 1], self._prep, h, b, gh * gw + 1, 16, "gelu", causal=False,
-                             weights=_block_weights, keep=HOOKS, split_k=self.split_k)
+                             weights=vit_block_weights, keep=HOOKS, split_k=self.split_k)
         return kept
 
     def _reassemble(self, k, h, b, gh, gw):

@@ -353,7 +353,7 @@ static int tap_gather_launch(const void* src, int src_f32_nchw, long long ld, vo
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     if (!src || !dst || !taps || batch < 0 || h < 1 || w < 1 || channels < 1 || n_taps < 1 || n_taps > kMaxTaps ||
         k_pad % 8 || k_pad < n_taps * channels || (!src_f32_nchw && ld < channels) || (stride != 1 && stride != 2) ||
-        h % stride || w % stride || act < 0 || act > 2)
+        h < stride || w < stride || act < 0 || act > 2)
         return CTRLORA_ERR_ARG;
     TapList tl;
     memset(&tl, 0, sizeof(tl));

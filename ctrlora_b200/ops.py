@@ -1046,7 +1046,7 @@ GATHER_ACTS = {None: 0, "relu": 1, "leaky": 2}  # ctrlora_tap_gather_act_f16's a
 
 
 def tap_gather_act(x, taps, *, reflect, k_pad, stride=1, act=None, channels=None, out=None):
-    """tap_gather with an output stride and an activation on load: fp16 [B, H / stride, W / stride, k_pad], column
+    """tap_gather with an output stride and an activation on load: fp16 [B, H // stride, W // stride, k_pad], column
     t * C + c of output pixel (y, x) = act(x at (stride y + dy_t, stride x + dx_t)), reflected or zero outside.
     stride 1 or 2; act None, "relu" or "leaky" (LeakyReLU(0.2)), applied in fp32 before the fp16 rounding."""
     b, h, w, c, ld, f32, flat = _gather_source(x, taps, channels)
@@ -1335,6 +1335,73 @@ def midas_maps(depth, a, bg_th):
     check(_lib.load().ctrlora_midas_maps(_dp(depth), _dp(minmax), _dp(d8), _dp(n8), b, h, w, float(a), float(bg_th), _sp()),
           "midas_maps")
     return d8, n8
+
+
+# ------------------------------------------------------------------------------------------------ UniFormer annotator
+def dwconv(x, weight, bias, k, residual=None):
+    """depthwise Conv2d(C, C, k, padding k // 2, groups=C) (k = 3 or 5) on fp16 [B, H, W, C] (contiguous), weight fp32
+    [k * k, C] tap-major, bias fp32 [C] -> fp16 [B, H, W, C] = (residual +) bias + conv, rounded once"""
+    _require_cuda(x, weight, bias, residual)
+    assert x.dtype == torch.float16 and x.is_contiguous() and x.dim() == 4
+    b, h, w, c = x.shape
+    assert weight.dtype == torch.float32 and weight.is_contiguous() and weight.shape == (k * k, c)
+    assert bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == c
+    if residual is not None:
+        assert residual.dtype == torch.float16 and residual.is_contiguous() and residual.shape == x.shape
+    out = torch.empty_like(x)
+    _count()
+    check(_lib.load().ctrlora_dwconv_f16(_dp(x), _dp(weight), _dp(bias), _dp(residual), _dp(out), b, h, w, c, k, _sp()),
+          "dwconv")
+    return out
+
+
+def resize_bilinear(x, size=None, out=None, accumulate=False):
+    """F.interpolate(x, size, mode="bilinear", align_corners=False) on fp16 [B, h, w, C] (channels may be a slice of a
+    wider buffer) -> fp16 [B, H, W, C]: into `out` (an fp16 [B, H, W, C] view, channel slices allowed) when given,
+    adding to its contents when accumulate; otherwise a new tensor of `size`"""
+    _require_cuda(x, out)
+    assert x.dtype == torch.float16 and (out is None or out.dtype == torch.float16)
+    b, hi, wi, c, ld = _as_bhwc(x)
+    if out is None:
+        assert not accumulate
+        out = torch.empty((b, size[0], size[1], c), device=x.device, dtype=torch.float16)
+    bo, ho, wo, co, ldo = _as_bhwc(out)
+    assert (bo, co) == (b, c) and (size is None or tuple(size) == (ho, wo))
+    _count()
+    check(_lib.load().ctrlora_resize_bilinear_f16(_dp(x), ld, _dp(out), ldo, b, hi, wi, ho, wo, c, int(bool(accumulate)),
+                                                  _sp()), "resize_bilinear")
+    return out
+
+
+def adaptive_avg_pool(x, sizes):
+    """AdaptiveAvgPool2d(s) for every s in sizes (<= 4) in one launch on fp16 [B, H, W, C] (channels may be a slice of a
+    wider buffer) -> [fp16 [B * s * s, C] rows (b, i, j) per size], views of one buffer"""
+    _require_cuda(x)
+    assert x.dtype == torch.float16
+    b, h, w, c, ld = _as_bhwc(x)
+    rows = [b * s * s for s in sizes]
+    out = torch.empty((sum(rows), c), device=x.device, dtype=torch.float16)
+    arr = (C.c_int * len(sizes))(*[int(s) for s in sizes])
+    _count()
+    check(_lib.load().ctrlora_adaptive_avg_pool_f16(_dp(x), ld, _dp(out), b, h, w, c, C.cast(arr, C.c_void_p), len(sizes),
+                                                    _sp()), "adaptive_avg_pool")
+    return list(torch.split(out, rows))
+
+
+def seg_output(logits, classes, net_size, out_size, palette, want_labels=False):
+    """logits fp32 [B, h4, w4, ld] (ld % 4 == 0) -> uint8 [B, H, W, 3] = palette[argmax over the first `classes`
+    channels of the logits resized to net_size and then to out_size = (H, W)] (and the int32 labels [B, H, W])"""
+    _require_cuda(logits, palette)
+    assert logits.dtype == torch.float32 and logits.is_contiguous() and logits.dim() == 4
+    assert palette.dtype == torch.uint8 and palette.is_contiguous() and palette.shape == (classes, 3)
+    b, h4, w4, ld = logits.shape
+    ho, wo = out_size
+    rgb = torch.empty((b, ho, wo, 3), device=logits.device, dtype=torch.uint8)
+    labels = torch.empty((b, ho, wo), device=logits.device, dtype=torch.int32) if want_labels else None
+    _count()
+    check(_lib.load().ctrlora_seg_output(_dp(logits), ld, classes, b, h4, w4, net_size[0], net_size[1], ho, wo,
+                                         _dp(palette), _dp(rgb), _dp(labels), _sp()), "seg_output")
+    return (rgb, labels) if want_labels else rgb
 
 
 def set_sm_limit(limit):

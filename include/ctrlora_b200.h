@@ -422,7 +422,8 @@ int ctrlora_tap_gather_f16(const void* src, int src_f32_nchw, long long ld, void
                            const int* taps, int n_taps, int reflect, int k_pad, void* stream);
 /* ctrlora_tap_gather_f16 with an output stride and an activation on load (Anime2Sketch's UnetGenerator,
  * annotator/lineart_anime/__init__.py:73-99): dst is [batch, h / stride, w / stride, k_pad] and output pixel (y, x)
- * reads (stride y + dy, stride x + dx); stride 1 or 2, h and w multiples of it.  act: 0 none, 1 ReLU (uprelu), 2
+ * reads (stride y + dy, stride x + dx); stride 1 or 2, h / stride and w / stride rounded down (a stride-2 Conv2d's
+ * truncation of odd sizes), at least 1.  act: 0 none, 1 ReLU (uprelu), 2
  * LeakyReLU(0.2) (downrelu), applied in fp32 to each gathered value before the fp16 rounding (zero-masked taps stay
  * 0).  stride = 1, act = 0 is ctrlora_tap_gather_f16, bit for bit. */
 int ctrlora_tap_gather_act_f16(const void* src, int src_f32_nchw, long long ld, void* dst, int batch, int h, int w,
@@ -548,6 +549,38 @@ int ctrlora_midas_head_out_f16(const void* x, const float* weight, const float* 
  * u8(v) is numpy's clip(0, 255).astype(uint8).  depth_u8 uint8 [batch, h, w]; normal_u8 uint8 [batch, h, w, 3]. */
 int ctrlora_midas_maps(const float* depth, float* minmax, unsigned char* depth_u8, unsigned char* normal_u8, int batch,
                        int h, int w, float a, float bg_th, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
+ * UniFormer-S + UPerNet segmentation annotator (annotator/uniformer: mmseg's EncoderDecoder, UniFormer backbone,
+ * UPerHead).  The patch embeds, 1x1 and 3x3 convs and linears run on ctrlora_patch_gather_hw, ctrlora_tap_gather_act_f16
+ * and ctrlora_gemm_f16, the attention on ctrlora_attention_f16 (d_head 64), the norms on ctrlora_layernorm_rows.
+ *
+ * Depthwise Conv2d(channels, channels, k, padding k / 2, groups=channels), k = 3 or 5, on fp16 NHWC x [batch, h, w,
+ * channels] (dense): out = fp16(residual + bias + sum over the taps of weight[ky * k + kx, c] * x), zero padding, fp32
+ * sums.  weight fp32 [k * k, channels] (tap-major), bias fp32 [channels]; residual NULL or fp16 like out (it may be x:
+ * x + dw(x) in one launch); out must not be x.  channels % 8 == 0. */
+int ctrlora_dwconv_f16(const void* x, const float* weight, const float* bias, const void* residual, void* out, int batch,
+                       int h, int w, int channels, int k, void* stream);
+/* F.interpolate(size=(ho, wo), mode="bilinear", align_corners=False) on fp16 NHWC: src [batch, hi, wi] with pixel stride
+ * src_ld (halves), dst [batch, ho, wo] with pixel stride dst_ld, `channels` channels from each pointer (so dst may be a
+ * channel slice of a wider buffer).  torch's source rule (scale = in / out in fp32, r = max(scale (d + 0.5) - 0.5, 0)),
+ * fp32 weights and sums; accumulate != 0: dst = fp16(dst + resized), one rounding.  channels, src_ld, dst_ld % 8 == 0;
+ * dst must not overlap src. */
+int ctrlora_resize_bilinear_f16(const void* src, int src_ld, void* dst, int dst_ld, int batch, int hi, int wi, int ho,
+                                int wo, int channels, int accumulate, void* stream);
+/* AdaptiveAvgPool2d(s) for each of n_sizes (<= 4) sizes (host array) in one launch, torch's bins (rows floor(i h / s) ..
+ * ceil((i + 1) h / s) - 1, the same for columns), fp32 sums: src fp16 [batch, h, w] with pixel stride src_ld, dst fp16
+ * rows of `channels`: size k's block starts at row batch * (sum of the squares of the sizes before it), row
+ * (b * s + i) * s + j within it.  channels, src_ld % 8 == 0. */
+int ctrlora_adaptive_avg_pool_f16(const void* src, int src_ld, void* dst, int batch, int h, int w, int channels,
+                                  const int* sizes, int n_sizes, void* stream);
+/* The segmentor's output from fp32 logits [batch, h4, w4, ld] (ld % 4 == 0, ld >= classes rounded up to 4): per pixel
+ * of [batch, ho, wo], the logits resized to the network size [hn, wn] and then to [ho, wo] (two bilinear steps with
+ * align_corners=False, as ctrlora_resize_bilinear_f16 computes them, in fp32; the network-size logits are evaluated
+ * where the second step reads them and never stored), the first class with the largest value, rgb uint8 [batch, ho,
+ * wo, 3] = palette[label] (uint8 [classes, 3], device) and, unless NULL, labels int32 [batch, ho, wo]. */
+int ctrlora_seg_output(const float* logits, int ld, int classes, int batch, int h4, int w4, int hn, int wn, int ho, int wo,
+                       const unsigned char* palette, unsigned char* rgb, int* labels, void* stream);
 
 #ifdef __cplusplus
 }

@@ -224,3 +224,102 @@ def install_timm_shim():
     m = types.ModuleType("timm")
     m.create_model, m.VisionTransformer = create_model, VisionTransformer
     sys.modules["timm"] = m
+
+
+def install_uniformer_shims():
+    """Stand-ins for what the reference's annotator.uniformer (its vendored mmcv and mmseg) imports and is not
+    installed: addict.Dict (mmcv.Config's attribute dict), yapf's FormatCode (Config.pretty_text only), prettytable
+    (mmseg's evaluation tables, never printed here), timm.models.layers' DropPath, to_2tuple and trunc_normal_ (the
+    UniFormer backbone; DropPath is the identity in eval mode) and an import-only matplotlib"""
+    install_openpose_shims()
+    if "addict" not in sys.modules:
+        m = types.ModuleType("addict")
+
+        class Dict(dict):
+            """addict.Dict's behaviour as mmcv.Config uses it: attribute access, nested dicts converted on
+            construction, a missing key raises (mmcv's ConfigDict overrides __missing__ to raise as well)"""
+
+            def __init__(self, *args, **kwargs):
+                super().__init__()
+                for arg in args:
+                    if isinstance(arg, dict):
+                        for k, v in arg.items():
+                            self[k] = self._hook(v)
+                    elif isinstance(arg, tuple) and not isinstance(arg[0], tuple):
+                        self[arg[0]] = self._hook(arg[1])
+                    elif arg is not None:
+                        for k, v in iter(arg):
+                            self[k] = self._hook(v)
+                for k, v in kwargs.items():
+                    self[k] = self._hook(v)
+
+            @classmethod
+            def _hook(cls, item):
+                if isinstance(item, dict):
+                    return cls(item)
+                if isinstance(item, (list, tuple)):
+                    return type(item)(cls._hook(e) for e in item)
+                return item
+
+            def __getattr__(self, k):
+                return self.__getitem__(k)
+
+            def __setattr__(self, k, v):
+                self[k] = v
+
+            def __missing__(self, k):
+                raise KeyError(k)
+
+            def to_dict(self):
+                return {k: v.to_dict() if isinstance(v, Dict) else v for k, v in self.items()}
+
+            def __deepcopy__(self, memo):
+                import copy
+                other = self.__class__()
+                memo[id(self)] = other
+                for k, v in self.items():
+                    other[copy.deepcopy(k, memo)] = copy.deepcopy(v, memo)
+                return other
+
+        m.Dict = Dict
+        sys.modules["addict"] = m
+    if "yapf" not in sys.modules:
+        names = ("yapf", "yapf.yapflib", "yapf.yapflib.yapf_api")
+        mods = {n: types.ModuleType(n) for n in names}
+        for n in names[:2]:
+            mods[n].__path__ = []
+        mods["yapf.yapflib.yapf_api"].FormatCode = lambda text, **k: (text, False)
+        sys.modules.update(mods)
+    if "prettytable" not in sys.modules:
+        m = types.ModuleType("prettytable")
+
+        class PrettyTable:
+            def __init__(self, *a, **k):
+                raise RuntimeError("prettytable is an import-only stand-in")
+
+        m.PrettyTable = PrettyTable
+        sys.modules["prettytable"] = m
+    if "timm.models.layers" not in sys.modules:
+        timm = sys.modules.get("timm") or types.ModuleType("timm")
+        timm.__path__ = []
+        models = types.ModuleType("timm.models")
+        models.__path__ = []
+        layers = types.ModuleType("timm.models.layers")
+
+        class DropPath(nn.Module):
+            def __init__(self, drop_prob=0.0):
+                super().__init__()
+                self.drop_prob = drop_prob
+
+            def forward(self, x):
+                if self.drop_prob == 0.0 or not self.training:
+                    return x
+                keep = 1 - self.drop_prob
+                mask = x.new_empty((x.shape[0],) + (1,) * (x.dim() - 1)).bernoulli_(keep)
+                return x * mask / keep
+
+        layers.DropPath = DropPath
+        layers.to_2tuple = lambda x: tuple(x) if isinstance(x, (list, tuple)) else (x, x)
+        layers.trunc_normal_ = lambda t, mean=0.0, std=1.0, a=-2.0, b=2.0: nn.init.trunc_normal_(t, mean, std, a, b)
+        timm.models, models.layers = models, layers
+        sys.modules.update({"timm": timm, "timm.models": models, "timm.models.layers": layers})
