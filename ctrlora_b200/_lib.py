@@ -150,6 +150,9 @@ _ARGTYPES = {
     "ctrlora_resize_bilinear_f16": [_P, _I, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P],
     "ctrlora_adaptive_avg_pool_f16": [_P, _I, _P, _I, _I, _I, _I, _P, _I, _P],
     "ctrlora_seg_output": [_P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P],
+    "ctrlora_dwconv_act_f16": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P],
+    "ctrlora_upsample_bilinear2x_ld_f16": [_P, _I, _P, _I, _I, _I, _I, _I, _P],
+    "ctrlora_mlsd_decode": [_P, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P],
 }
 
 
@@ -251,4 +254,7 @@ EXPORTS = [
     "ctrlora_resize_bilinear_f16",
     "ctrlora_adaptive_avg_pool_f16",
     "ctrlora_seg_output",
+    "ctrlora_dwconv_act_f16",
+    "ctrlora_upsample_bilinear2x_ld_f16",
+    "ctrlora_mlsd_decode",
 ]

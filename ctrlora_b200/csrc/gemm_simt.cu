@@ -42,9 +42,11 @@ __global__ void gemm_simt_kernel(ctrlora_gemm_args a, int M, int rows_per_img) {
     const int img = static_cast<int>(m / rows_per_img), tok = static_cast<int>(m % rows_per_img);
     if (a.rowbias) v += a.rowbias[static_cast<long long>(img) * (a.rowbias_ld > 0 ? a.rowbias_ld : a.n) + n];
     v *= a.out_scale;
+    if (a.relu == 3) v = fmaxf(v, 0.f);
     if (a.residual) v += a.residual_f32 ? reinterpret_cast<const float*>(a.residual)[m * a.ldr + n]
                                          : __half2float(reinterpret_cast<const __half*>(a.residual)[m * a.ldr + n]);
-    if (a.relu) v = fmaxf(v, 0.f);
+    if (a.relu == 1) v = fmaxf(v, 0.f);
+    if (a.relu == 2) v = fminf(fmaxf(v, 0.f), 6.f);
     int seg = 0, nloc = n;
     if (a.seg_width > 0) { seg = n / a.seg_width; nloc = n % a.seg_width; }
     if (a.transposed[seg]) {

@@ -21,6 +21,11 @@
 namespace ctrl {
 
 __device__ __forceinline__ bool aligned16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; }
+// The last step of the epilogue for relu = 1 (ReLU) and 2 (ReLU6); relu = 3 (ReLU before the residual) is applied
+// before the residual add instead.
+__device__ __forceinline__ float act_last(int relu, float v) {
+    return relu == 2 ? fminf(fmaxf(v, 0.f), 6.f) : fmaxf(v, 0.f);
+}
 __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
     __half2 h = __floats2half2_rn(a, b);
     return *reinterpret_cast<uint32_t*>(&h);
@@ -52,6 +57,10 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, float* v, i
     if (p.out_scale != 1.0f) {
 #pragma unroll
         for (int j = 0; j < CW; ++j) v[j] *= p.out_scale;
+    }
+    if (p.relu == 3) {
+#pragma unroll
+        for (int j = 0; j < CW; ++j) v[j] = fmaxf(v[j], 0.f);
     }
     if (p.residual && p.residual_f32) {
         const float* rp = reinterpret_cast<const float*>(p.residual) + m * p.ldr + nbase;
@@ -88,9 +97,9 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, float* v, i
                 if (c + j < bn_out && nbase + j < p.N) v[j] += __half2float(rp[j]);
         }
     }
-    if (p.relu) {
+    if (p.relu == 1 || p.relu == 2) {
 #pragma unroll
-        for (int j = 0; j < CW; ++j) v[j] = fmaxf(v[j], 0.f);
+        for (int j = 0; j < CW; ++j) v[j] = act_last(p.relu, v[j]);
     }
     int seg = 0, nloc = nbase;
     if (p.seg_width > 0) { seg = nbase / p.seg_width; nloc = nbase - seg * p.seg_width; }
@@ -334,14 +343,18 @@ __device__ __forceinline__ void gemm_pingpong_consumers(const GemmKParams& p, ui
                     }
                     const uint32_t a0 = sb + ((static_cast<uint32_t>(c) ^ row_x) << 4);
                     const uint32_t a1 = a0 + 8 * SW * 2;
+                    if (p.relu == 3) {
+                        v00 = fmaxf(v00, 0.f); v01 = fmaxf(v01, 0.f);
+                        v10 = fmaxf(v10, 0.f); v11 = fmaxf(v11, 0.f);
+                    }
                     if (p.residual) {
                         const float2 r0 = h2_to_f2(lds32(a0)), r1 = h2_to_f2(lds32(a1));
                         v00 = __fadd_rn(v00, r0.x); v01 = __fadd_rn(v01, r0.y);
                         v10 = __fadd_rn(v10, r1.x); v11 = __fadd_rn(v11, r1.y);
                     }
-                    if (p.relu) {
-                        v00 = fmaxf(v00, 0.f); v01 = fmaxf(v01, 0.f);
-                        v10 = fmaxf(v10, 0.f); v11 = fmaxf(v11, 0.f);
+                    if (p.relu == 1 || p.relu == 2) {
+                        v00 = act_last(p.relu, v00); v01 = act_last(p.relu, v01);
+                        v10 = act_last(p.relu, v10); v11 = act_last(p.relu, v11);
                     }
                     sts32(a0, pack_h2(v00, v01));
                     sts32(a1, pack_h2(v10, v11));
@@ -638,14 +651,18 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     }
                     const uint32_t a0 = sb + ((static_cast<uint32_t>(c) ^ row_x) << 4);
                     const uint32_t a1 = a0 + 8 * SW * 2;
+                    if (p.relu == 3) {
+                        v00 = fmaxf(v00, 0.f); v01 = fmaxf(v01, 0.f);
+                        v10 = fmaxf(v10, 0.f); v11 = fmaxf(v11, 0.f);
+                    }
                     if (p.residual) {
                         const float2 r0 = h2_to_f2(lds32(a0)), r1 = h2_to_f2(lds32(a1));
                         v00 = __fadd_rn(v00, r0.x); v01 = __fadd_rn(v01, r0.y);
                         v10 = __fadd_rn(v10, r1.x); v11 = __fadd_rn(v11, r1.y);
                     }
-                    if (p.relu) {
-                        v00 = fmaxf(v00, 0.f); v01 = fmaxf(v01, 0.f);
-                        v10 = fmaxf(v10, 0.f); v11 = fmaxf(v11, 0.f);
+                    if (p.relu == 1 || p.relu == 2) {
+                        v00 = act_last(p.relu, v00); v01 = act_last(p.relu, v01);
+                        v10 = act_last(p.relu, v10); v11 = act_last(p.relu, v11);
                     }
                     sts32(a0, pack_h2(v00, v01));
                     sts32(a1, pack_h2(v10, v11));
@@ -808,6 +825,7 @@ extern "C" int ctrlora_gemm_f16(const ctrlora_gemm_args* a, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     if (!a || !a->a || !a->w || !a->out[0]) return CTRLORA_ERR_ARG;
     if (a->a_c % 8 != 0 || a->a_ld % 8 != 0) return CTRLORA_ERR_ARG;
+    if (a->relu < 0 || a->relu > 3) return CTRLORA_ERR_ARG;
     // square 1x1, 3x3 and 7x7 taps (7x7: OpenPose's CPM stages); the box origin goes down to -pad, which the tensor
     // map's out-of-bounds fill reads as zero padding
     if (a->kh != a->kw || (a->kh != 1 && a->kh != 3 && a->kh != 7)) return CTRLORA_ERR_UNSUPPORTED;

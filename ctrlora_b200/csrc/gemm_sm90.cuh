@@ -71,7 +71,7 @@ struct GemmKParams {
     int rb_img_off;
     const float* bias_g[2];
     const float* rowbias_g[2];
-    int relu;                       // max(v, 0) just before the output rounding
+    int relu;                       // 1: max(v, 0), 2: min(max(v, 0), 6) last; 3: max(v, 0) before the residual
 };
 
 }  // namespace ctrl

@@ -4,7 +4,8 @@
 // - the depth-to-space + bias step that follows a kernel = stride ConvTranspose2d computed as one GEMM;
 // - s = a (+ b), relu(s) in one pass: the RCU's input ReLU and the fusion block's skip sum, which the implicit GEMM
 //   cannot apply on load (it reads A by TMA);
-// - the bilinear x2 upsample with align_corners = True of FeatureFusionBlock_custom and the head's Interpolate;
+// - the bilinear x2 upsample with align_corners = True of FeatureFusionBlock_custom and the head's Interpolate (also
+//   M-LSD's BlockTypeA, which writes it into a channel slice);
 // - the head's last Conv2d(32 -> 1, 1) + bias + ReLU, writing the fp32 depth;
 // - MidasDetector's post-process: the min / max normalisation and uint8 depth map, and cv2.Sobel's normal map.
 #include "common.cuh"
@@ -71,10 +72,11 @@ add_relu_kernel(const __half* __restrict__ a, const __half* __restrict__ b, __ha
 
 // ------------------------------------------------------------------------------------------ bilinear x2
 // F.interpolate(scale_factor=2, mode="bilinear", align_corners=True) on fp16 [B, h, w, C], fp32 weights and sums as
-// torch's CUDA kernel forms them: source index = ((in - 1) / (out - 1)) * dst, lambda = index - floor.
+// torch's CUDA kernel forms them: source index = ((in - 1) / (out - 1)) * dst, lambda = index - floor.  src and dst
+// pixel strides src_ld, dst_ld (halves), so either may be a channel slice of a wider buffer.
 __global__ void __launch_bounds__(256)
-upsample_bilinear2x_kernel(const __half* __restrict__ src, __half* __restrict__ dst, long long items, int h, int w,
-                           int channels) {
+upsample_bilinear2x_kernel(const __half* __restrict__ src, int src_ld, __half* __restrict__ dst, int dst_ld,
+                           long long items, int h, int w, int channels) {
     pdl_launch_dependents();
     pdl_wait();
     const int c8 = channels >> 3, oh = 2 * h, ow = 2 * w;
@@ -91,12 +93,12 @@ upsample_bilinear2x_kernel(const __half* __restrict__ src, __half* __restrict__ 
         const int y0 = static_cast<int>(fy), x0 = static_cast<int>(fx);
         const int y1 = y0 + (y0 < h - 1), x1 = x0 + (x0 < w - 1);
         const float ly1 = fy - y0, ly0 = 1.f - ly1, lx1 = fx - x0, lx0 = 1.f - lx1;
-        const __half* base = src + b * h * (long long)w * channels + c;
+        const __half* base = src + b * h * (long long)w * src_ld + c;
         uint4 q[4];
-        q[0] = *reinterpret_cast<const uint4*>(base + ((long long)y0 * w + x0) * channels);
-        q[1] = *reinterpret_cast<const uint4*>(base + ((long long)y0 * w + x1) * channels);
-        q[2] = *reinterpret_cast<const uint4*>(base + ((long long)y1 * w + x0) * channels);
-        q[3] = *reinterpret_cast<const uint4*>(base + ((long long)y1 * w + x1) * channels);
+        q[0] = *reinterpret_cast<const uint4*>(base + ((long long)y0 * w + x0) * src_ld);
+        q[1] = *reinterpret_cast<const uint4*>(base + ((long long)y0 * w + x1) * src_ld);
+        q[2] = *reinterpret_cast<const uint4*>(base + ((long long)y1 * w + x0) * src_ld);
+        q[3] = *reinterpret_cast<const uint4*>(base + ((long long)y1 * w + x1) * src_ld);
         const __half2* h00 = reinterpret_cast<const __half2*>(&q[0]);
         const __half2* h01 = reinterpret_cast<const __half2*>(&q[1]);
         const __half2* h10 = reinterpret_cast<const __half2*>(&q[2]);
@@ -111,7 +113,7 @@ upsample_bilinear2x_kernel(const __half* __restrict__ src, __half* __restrict__ 
             const float vy = ly0 * (lx0 * a.y + lx1 * bq.y) + ly1 * (lx0 * cq.y + lx1 * d.y);
             ho[e] = __floats2half2_rn(vx, vy);
         }
-        *reinterpret_cast<uint4*>(dst + i * 8) = o;
+        *reinterpret_cast<uint4*>(dst + ((b * oh + oy) * (long long)ow + ox) * dst_ld + c) = o;
     }
 }
 
@@ -253,16 +255,22 @@ extern "C" int ctrlora_add_relu_f16(const void* a, const void* b, void* sum, voi
                                      static_cast<__half*>(relu), vecs));
 }
 
-extern "C" int ctrlora_upsample_bilinear2x_f16(const void* src, void* dst, int batch, int h, int w, int channels,
-                                               void* stream_) {
+extern "C" int ctrlora_upsample_bilinear2x_ld_f16(const void* src, int src_ld, void* dst, int dst_ld, int batch, int h,
+                                                  int w, int channels, void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    if (!src || !dst || batch < 0 || h < 1 || w < 1 || channels < 8 || channels % 8 || misaligned(src, 16) ||
-        misaligned(dst, 16))
+    if (!src || !dst || batch < 0 || h < 1 || w < 1 || channels < 8 || channels % 8 || src_ld < channels ||
+        dst_ld < channels || src_ld % 8 || dst_ld % 8 || misaligned(src, 16) || misaligned(dst, 16))
         return CTRLORA_ERR_ARG;
     const long long items = (long long)batch * 2 * h * 2 * w * (channels / 8);
     if (items == 0) return CTRLORA_OK;
     return launched(launch_pdl(upsample_bilinear2x_kernel, dim3(grid_blocks(items, 256, 8192)), dim3(256), (size_t)0, stream,
-                                     static_cast<const __half*>(src), static_cast<__half*>(dst), items, h, w, channels));
+                                     static_cast<const __half*>(src), src_ld, static_cast<__half*>(dst), dst_ld, items, h,
+                                     w, channels));
+}
+
+extern "C" int ctrlora_upsample_bilinear2x_f16(const void* src, void* dst, int batch, int h, int w, int channels,
+                                               void* stream_) {
+    return ctrlora_upsample_bilinear2x_ld_f16(src, channels, dst, channels, batch, h, w, channels, stream_);
 }
 
 extern "C" int ctrlora_midas_head_out_f16(const void* x, const float* weight, const float* bias, float* out,

@@ -2,7 +2,8 @@
 // EncoderDecoder with the UniFormer backbone and UPerHead).  The patch embeds, every 1x1 and 3x3 conv, the linears,
 // the attention, LayerNorm and GELU run on the existing entry points; what is left is here:
 // - the depthwise k x k conv (k = 3, 5) with bias and an optional residual: CBlock's and SABlock's pos_embed
-//   (x + dw3x3(x) in one launch) and CBlock's dw5x5 `attn`;
+//   (x + dw3x3(x) in one launch) and CBlock's dw5x5 `attn`; its stride-2 (TFLite padding) and ReLU / ReLU6 variants
+//   serve M-LSD's MobileNetV2 (annotator/mlsd/models/mbv2_mlsd_large.py);
 // - the bilinear resize with align_corners = False between any two sizes, optionally accumulating into its destination
 //   and writing a channel slice of a wider pixel-major buffer: the PPM and FPN resizes and the top-down adds;
 // - the adaptive average pool of the PPM, every pool size in one launch;
@@ -53,16 +54,19 @@ __device__ __forceinline__ void store8(__half* p, const float* v) {
 }
 
 // ------------------------------------------------------------------------------------------ depthwise conv
-// out[b, y, x, c] = fp16((residual[b, y, x, c]) + bias[c] + sum_{ky, kx} weight[ky * K + kx, c] * in[b, y + ky - K/2,
-// x + kx - K/2, c]), zero outside; fp32 sums in tap order.  One thread per pixel and 8 channels.
-template <int K>
+// out[b, y, x, c] = fp16(act((residual[b, y, x, c]) + bias[c] + sum_{ky, kx} weight[ky * K + kx, c] * in[b, S y + ky - P,
+// S x + kx - P, c])), zero outside; fp32 sums in tap order.  S = 1: P = K / 2, the output is hi x wi; S = 2: P = 0 (the
+// TFLite padding: F.pad(x, (0, 1, 0, 1)) then a padding-0 conv), the output is floor(hi / 2) x floor(wi / 2).  ACT 0
+// none, 1 ReLU, 2 ReLU6.  One thread per output pixel and 8 channels.
+template <int K, int S, int ACT>
 __global__ void __launch_bounds__(256)
 dwconv_kernel(const __half* __restrict__ x, const float* __restrict__ weight, const float* __restrict__ bias,
-              const __half* __restrict__ residual, __half* __restrict__ out, long long items, int h, int w, int channels) {
+              const __half* __restrict__ residual, __half* __restrict__ out, long long items, int hi, int wi, int h, int w,
+              int channels) {
     pdl_launch_dependents();
     pdl_wait();
     const int c8 = channels >> 3;
-    constexpr int R = K / 2;
+    constexpr int R = S == 1 ? K / 2 : 0;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < items; i += (long long)gridDim.x * blockDim.x) {
         const int c = static_cast<int>(i % c8) * 8;
         long long r = i / c8;
@@ -70,20 +74,20 @@ dwconv_kernel(const __half* __restrict__ x, const float* __restrict__ weight, co
         r /= w;
         const int py = static_cast<int>(r % h);
         const long long b = r / h;
-        const __half* img = x + b * h * (long long)w * channels + c;
+        const __half* img = x + b * hi * (long long)wi * channels + c;
         float acc[8];
 #pragma unroll
         for (int e = 0; e < 8; ++e) acc[e] = 0.f;
 #pragma unroll
         for (int ky = 0; ky < K; ++ky) {
-            const int iy = py + ky - R;
-            if (iy < 0 || iy >= h) continue;
+            const int iy = S * py + ky - R;
+            if (iy < 0 || iy >= hi) continue;
 #pragma unroll
             for (int kx = 0; kx < K; ++kx) {
-                const int ix = px + kx - R;
-                if (ix < 0 || ix >= w) continue;
+                const int ix = S * px + kx - R;
+                if (ix < 0 || ix >= wi) continue;
                 float v[8];
-                load8(img + ((long long)iy * w + ix) * channels, v);
+                load8(img + ((long long)iy * wi + ix) * channels, v);
                 const float4 w0 = *reinterpret_cast<const float4*>(weight + (ky * K + kx) * channels + c);
                 const float4 w1 = *reinterpret_cast<const float4*>(weight + (ky * K + kx) * channels + c + 4);
                 acc[0] = fmaf(w0.x, v[0], acc[0]);
@@ -105,6 +109,10 @@ dwconv_kernel(const __half* __restrict__ x, const float* __restrict__ weight, co
             load8(residual + i * 8, res);
 #pragma unroll
             for (int e = 0; e < 8; ++e) acc[e] += res[e];
+        }
+        if (ACT) {
+#pragma unroll
+            for (int e = 0; e < 8; ++e) acc[e] = ACT == 2 ? fminf(fmaxf(acc[e], 0.f), 6.f) : fmaxf(acc[e], 0.f);
         }
         store8(out + i * 8, acc);
     }
@@ -266,24 +274,47 @@ seg_output_kernel(const float* __restrict__ logits, int ld, int classes, int h4,
 
 using namespace ctrl;
 
-extern "C" int ctrlora_dwconv_f16(const void* x, const float* weight, const float* bias, const void* residual, void* out,
-                                  int batch, int h, int w, int channels, int k, void* stream_) {
+template <int S>
+static int launch_dwconv3(int act, dim3 grid, cudaStream_t stream, const __half* x, const float* weight, const float* bias,
+                          const __half* residual, __half* out, long long items, int hi, int wi, int h, int w,
+                          int channels) {
+    if (act == 0)
+        return launched(launch_pdl(dwconv_kernel<3, S, 0>, grid, dim3(256), (size_t)0, stream, x, weight, bias, residual,
+                                   out, items, hi, wi, h, w, channels));
+    if (act == 1)
+        return launched(launch_pdl(dwconv_kernel<3, S, 1>, grid, dim3(256), (size_t)0, stream, x, weight, bias, residual,
+                                   out, items, hi, wi, h, w, channels));
+    return launched(launch_pdl(dwconv_kernel<3, S, 2>, grid, dim3(256), (size_t)0, stream, x, weight, bias, residual, out,
+                               items, hi, wi, h, w, channels));
+}
+
+extern "C" int ctrlora_dwconv_act_f16(const void* x, const float* weight, const float* bias, const void* residual,
+                                      void* out, int batch, int h, int w, int channels, int k, int stride, int act,
+                                      void* stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    // k = 5 (UniFormer's CBlock attn) runs at stride 1 without activation only
     if (!x || !weight || !bias || !out || batch < 0 || h < 1 || w < 1 || channels < 8 || channels % 8 ||
-        (k != 3 && k != 5) || misaligned_u(x, 16) || misaligned_u(weight, 16) || misaligned_u(bias, 16) ||
-        misaligned_u(residual, 16) || misaligned_u(out, 16) || out == x)
+        (k != 3 && k != 5) || (stride != 1 && stride != 2) || act < 0 || act > 2 || (k == 5 && (stride != 1 || act)) ||
+        misaligned_u(x, 16) || misaligned_u(weight, 16) || misaligned_u(bias, 16) || misaligned_u(residual, 16) ||
+        misaligned_u(out, 16) || out == x)
         return CTRLORA_ERR_ARG;
-    const long long items = (long long)batch * h * w * (channels / 8);
+    const int ho = h / stride, wo = w / stride;
+    const long long items = (long long)batch * ho * wo * (channels / 8);
     if (items == 0) return CTRLORA_OK;
     const dim3 grid(grid_blocks(items, 256, 8192));
     const __half* xs = static_cast<const __half*>(x);
     const __half* rs = static_cast<const __half*>(residual);
     __half* o = static_cast<__half*>(out);
-    if (k == 3)
-        return launched(launch_pdl(dwconv_kernel<3>, grid, dim3(256), (size_t)0, stream, xs, weight, bias, rs, o, items, h,
-                                   w, channels));
-    return launched(launch_pdl(dwconv_kernel<5>, grid, dim3(256), (size_t)0, stream, xs, weight, bias, rs, o, items, h, w,
-                               channels));
+    if (k == 5)
+        return launched(launch_pdl(dwconv_kernel<5, 1, 0>, grid, dim3(256), (size_t)0, stream, xs, weight, bias, rs, o,
+                                   items, h, w, ho, wo, channels));
+    if (stride == 1) return launch_dwconv3<1>(act, grid, stream, xs, weight, bias, rs, o, items, h, w, ho, wo, channels);
+    return launch_dwconv3<2>(act, grid, stream, xs, weight, bias, rs, o, items, h, w, ho, wo, channels);
+}
+
+extern "C" int ctrlora_dwconv_f16(const void* x, const float* weight, const float* bias, const void* residual, void* out,
+                                  int batch, int h, int w, int channels, int k, void* stream_) {
+    return ctrlora_dwconv_act_f16(x, weight, bias, residual, out, batch, h, w, channels, k, 1, 0, stream_);
 }
 
 extern "C" int ctrlora_resize_bilinear_f16(const void* src, int src_ld, void* dst, int dst_ld, int batch, int hi, int wi,

@@ -158,6 +158,18 @@ def gemm_relu(a, w, **kwargs):
     return _gemm(a, w, relu=True, **kwargs)
 
 
+def gemm_relu6(a, w, **kwargs):
+    """ops.gemm (same arguments) with min(max(., 0), 6) as the epilogue's last step, before the output rounding: a conv
+    + BatchNorm + ReLU6 (MobileNetV2's ConvBNReLU) in one launch"""
+    return _gemm(a, w, relu=2, **kwargs)
+
+
+def gemm_relu_residual(a, w, *, residual, **kwargs):
+    """ops.gemm (same arguments) with max(., 0) taken before the residual add: relu(conv(a)) + residual in one launch
+    (M-LSD's BlockTypeB conv1)"""
+    return _gemm(a, w, relu=3, residual=residual, **kwargs)
+
+
 def _gemm(a, w, *, ksize=1, bias=None, rowbias=None, rows_per_img=0, rowbias_ld=0, residual=None, out_scale=1.0, a2=None,
           w2=None, geglu=False, out=None, out_f32=False, seg_outs=None, seg_width=0, transposed=(0, 0, 0), head_dim=0,
           tok_pad=0, block_n=0, split_k=0, dup_out=None, single_cta=False, simt=False, hi=None, relu=False):
@@ -213,7 +225,7 @@ def _gemm(a, w, *, ksize=1, bias=None, rowbias=None, rows_per_img=0, rowbias_ld=
     if dup_out is not None:
         args.dup_out, args.dup_ld = dup_out.data_ptr(), dup_out.stride(0)
     args.force_single_cta = int(single_cta)
-    args.relu = int(bool(relu))
+    args.relu = int(relu)
     if hi is not None:
         if hi.get("rowbias") is not None:  # the kernel reads both halves' row terms with the lower half's row stride
             assert rowbias is not None and hi["rowbias"].stride(0) == rowbias.stride(0) and \
@@ -1309,6 +1321,20 @@ def upsample_bilinear2x(x):
     return y
 
 
+def upsample_bilinear2x_into(x, out):
+    """upsample_bilinear2x from fp16 [B, h, w, C] into `out`, an fp16 [B, 2h, 2w, C] view; either may be a channel slice
+    of a wider pixel-major buffer"""
+    _require_cuda(x, out)
+    assert x.dtype == torch.float16 and out.dtype == torch.float16
+    b, h, w, c, ld = _as_bhwc(x)
+    bo, ho, wo, co, ldo = _as_bhwc(out)
+    assert (bo, ho, wo, co) == (b, 2 * h, 2 * w, c), (tuple(x.shape), tuple(out.shape))
+    _count()
+    check(_lib.load().ctrlora_upsample_bilinear2x_ld_f16(_dp(x), ld, _dp(out), ldo, b, h, w, c, _sp()),
+          "upsample_bilinear2x_into")
+    return out
+
+
 def midas_head_out(x, weight, bias):
     """the DPT head's Conv2d(C -> 1, 1) + ReLU: x fp16 [B, H, W, C], weight fp32 [C], bias fp32 [1] -> fp32 [B, H, W]"""
     _require_cuda(x, weight, bias)
@@ -1352,6 +1378,28 @@ def dwconv(x, weight, bias, k, residual=None):
     _count()
     check(_lib.load().ctrlora_dwconv_f16(_dp(x), _dp(weight), _dp(bias), _dp(residual), _dp(out), b, h, w, c, k, _sp()),
           "dwconv")
+    return out
+
+
+DWCONV_ACTS = {None: 0, "relu": 1, "relu6": 2}  # ctrlora_dwconv_act_f16's act codes
+
+
+def dwconv_act(x, weight, bias, k, *, stride=1, act=None, residual=None):
+    """dwconv with a stride and an activation: stride 1 pads k // 2 -> fp16 [B, H, W, C]; stride 2 uses the TFLite
+    padding (output pixel (y, x) reads rows 2y .. 2y + k - 1 and the same columns, zero outside) -> fp16 [B, H // 2,
+    W // 2, C].  act None, "relu" or "relu6", applied after bias and residual (shaped like the output).  Stride 2 and
+    an activation take k = 3 only."""
+    _require_cuda(x, weight, bias, residual)
+    assert x.dtype == torch.float16 and x.is_contiguous() and x.dim() == 4
+    b, h, w, c = x.shape
+    assert weight.dtype == torch.float32 and weight.is_contiguous() and weight.shape == (k * k, c)
+    assert bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == c
+    out = torch.empty((b, h // stride, w // stride, c), device=x.device, dtype=torch.float16)
+    if residual is not None:
+        assert residual.dtype == torch.float16 and residual.is_contiguous() and residual.shape == out.shape
+    _count()
+    check(_lib.load().ctrlora_dwconv_act_f16(_dp(x), _dp(weight), _dp(bias), _dp(residual), _dp(out), b, h, w, c, k,
+                                             stride, DWCONV_ACTS[act], _sp()), "dwconv_act")
     return out
 
 
@@ -1402,6 +1450,26 @@ def seg_output(logits, classes, net_size, out_size, palette, want_labels=False):
     check(_lib.load().ctrlora_seg_output(_dp(logits), ld, classes, b, h4, w4, net_size[0], net_size[1], ho, wo,
                                          _dp(palette), _dp(rgb), _dp(labels), _sp()), "seg_output")
     return (rgb, labels) if want_labels else rgb
+
+
+# ------------------------------------------------------------------------------------------------ M-LSD annotator
+MLSD_TOPK = 200  # CTRLORA_MLSD_TOPK
+
+
+def mlsd_decode(tp, c_center, c_disp):
+    """M-LSD's line decode on the head's fp32 map [B, h, w, ld] (contiguous): per image the MLSD_TOPK largest of
+    sigmoid(centre) * (3 x 3 peak mask), descending, ties by the lower flat index -> (int32 [B, TOPK] flat indices
+    y * w + x, fp32 [B, TOPK, 6] (score, segment length, the four displacements)).  h * w >= MLSD_TOPK."""
+    _require_cuda(tp)
+    assert tp.dtype == torch.float32 and tp.is_contiguous() and tp.dim() == 4
+    b, h, w, ld = tp.shape
+    ws = torch.empty((b, h, w), device=tp.device, dtype=torch.float32)
+    idx = torch.empty((b, MLSD_TOPK), device=tp.device, dtype=torch.int32)
+    val = torch.empty((b, MLSD_TOPK, 6), device=tp.device, dtype=torch.float32)
+    _count(2)
+    check(_lib.load().ctrlora_mlsd_decode(_dp(tp), ld, c_center, c_disp, b, h, w, _dp(ws), _dp(idx), _dp(val), _sp()),
+          "mlsd_decode")
+    return idx, val
 
 
 def set_sm_limit(limit):

@@ -89,7 +89,10 @@ typedef struct ctrlora_gemm_args {
     const float* rowbias_hi;
     const void* w2_hi;
     /* relu = 1: max(v, 0) as the last step before the output rounding, after bias, row term, scale and residual (split
-     * tiles: after the split-K sum).  The ReLU of HED's conv + ReLU pairs (annotator/hed/__init__.py:30-31). */
+     * tiles: after the split-K sum).  The ReLU of HED's conv + ReLU pairs (annotator/hed/__init__.py:30-31).
+     * relu = 2: min(max(v, 0), 6) as that last step: the ReLU6 of M-LSD's ConvBNReLU (annotator/mlsd/models/
+     * mbv2_mlsd_large.py:107).  relu = 3: max((acc + bias + row term) * scale, 0) + residual, the ReLU before the
+     * residual add: BlockTypeB's relu(bn(conv1(x))) + x (mbv2_mlsd_large.py:47).  Other values are rejected. */
     int relu;
 } ctrlora_gemm_args;
 
@@ -535,6 +538,11 @@ int ctrlora_add_relu_f16(const void* a, const void* b, void* sum, void* relu, lo
  * 2w, channels], fp32 weights and sums (source index ((in - 1) / (out - 1)) * dst, as torch's kernel forms it);
  * channels % 8 == 0.  FeatureFusionBlock_custom's and the DPT head's upsample. */
 int ctrlora_upsample_bilinear2x_f16(const void* src, void* dst, int batch, int h, int w, int channels, void* stream);
+/* ctrlora_upsample_bilinear2x_f16 with pixel strides src_ld and dst_ld (halves, % 8 == 0, >= channels), so that either
+ * side may be a channel slice of a wider buffer: M-LSD's BlockTypeA upsamples into its half of the concatenation
+ * (annotator/mlsd/models/mbv2_mlsd_large.py:27-29).  ld = channels on both sides is ctrlora_upsample_bilinear2x_f16. */
+int ctrlora_upsample_bilinear2x_ld_f16(const void* src, int src_ld, void* dst, int dst_ld, int batch, int h, int w,
+                                       int channels, void* stream);
 /* The DPT head's Conv2d(channels -> 1, 1) + ReLU: out[p] = max(bias[0] + sum_c weight[c] * x[p, c], 0), fp32 sums in
  * channel order.  x fp16 [pixels, channels] dense, channels % 8 == 0, <= 64; weight fp32 [channels]; bias fp32 [1]
  * (device); out fp32 [pixels]. */
@@ -561,6 +569,14 @@ int ctrlora_midas_maps(const float* depth, float* minmax, unsigned char* depth_u
  * x + dw(x) in one launch); out must not be x.  channels % 8 == 0. */
 int ctrlora_dwconv_f16(const void* x, const float* weight, const float* bias, const void* residual, void* out, int batch,
                        int h, int w, int channels, int k, void* stream);
+/* ctrlora_dwconv_f16 with a stride and an activation; stride 2 and act != 0 take k = 3 only (k = 5 with either returns
+ * CTRLORA_STATUS_BAD_ARGUMENT).  stride 1: padding k / 2, the output is h x w (stride 1, act 0 is ctrlora_dwconv_f16).
+ * stride 2: the TFLite padding of M-LSD's ConvBNReLU (F.pad(x, (0, 1, 0, 1)) then padding 0,
+ * annotator/mlsd/models/mbv2_mlsd_large.py:98-100, 113-115): output pixel (y, x) reads rows 2y .. 2y + 2 and the same
+ * columns, zero outside, and the output is floor(h / 2) x floor(w / 2).  act 0 none, 1 ReLU, 2 ReLU6
+ * (min(max(v, 0), 6)), applied after bias and residual, before the one fp16 rounding; residual is shaped like out. */
+int ctrlora_dwconv_act_f16(const void* x, const float* weight, const float* bias, const void* residual, void* out,
+                           int batch, int h, int w, int channels, int k, int stride, int act, void* stream);
 /* F.interpolate(size=(ho, wo), mode="bilinear", align_corners=False) on fp16 NHWC: src [batch, hi, wi] with pixel stride
  * src_ld (halves), dst [batch, ho, wo] with pixel stride dst_ld, `channels` channels from each pointer (so dst may be a
  * channel slice of a wider buffer).  torch's source rule (scale = in / out in fp32, r = max(scale (d + 0.5) - 0.5, 0)),
@@ -581,6 +597,25 @@ int ctrlora_adaptive_avg_pool_f16(const void* src, int src_ld, void* dst, int ba
  * wo, 3] = palette[label] (uint8 [classes, 3], device) and, unless NULL, labels int32 [batch, ho, wo]. */
 int ctrlora_seg_output(const float* logits, int ld, int classes, int batch, int h4, int w4, int hn, int wn, int ho, int wo,
                        const unsigned char* palette, unsigned char* rgb, int* labels, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
+ * M-LSD line detector (annotator/mlsd/__init__.py MLSDdetector, models/mbv2_mlsd_large.py, utils.py pred_lines).  The
+ * MobileNetV2 backbone and the decoder run on ctrlora_tap_gather_act_f16, ctrlora_gemm_f16 (relu = 2, 3),
+ * ctrlora_dwconv_act_f16 and ctrlora_upsample_bilinear2x_ld_f16.
+ *
+ * The line decode (utils.py:19-41, deccode_output_score_and_ptss with ksize 3 and topk_n = CTRLORA_MLSD_TOPK): on the
+ * head's fp32 map tp [batch, h, w, ld] (centre at column c_center, the four displacements at c_disp .. c_disp + 3),
+ * per image: heat = sigmoid(centre) in fp32; score = heat where it equals the maximum of its 3 x 3 window (pixels
+ * outside the map skipped, max_pool2d's -inf padding), else 0; the CTRLORA_MLSD_TOPK largest scores in descending
+ * order, ties broken by the lower flat index y * w + x (so zero scores fill the slots left over, lowest indices first).
+ * Per candidate: out_idx int32 [batch, TOPK] the flat index, out_val fp32 [batch, TOPK, 6] = (score, dist, d0, d1, d2,
+ * d3) with d the displacements and dist = sqrt((d0 - d2)^2 + (d1 - d3)^2), each step rounded to fp32 as numpy does
+ * (utils.py:66).  score_ws: fp32 [batch, h, w] workspace.  Two launches: the scores, then one CTA per image (a radix
+ * select on the scores' bits and a rank sort, no atomics), so the result is deterministic and does not depend on the
+ * batch.  h * w < TOPK returns CTRLORA_STATUS_BAD_ARGUMENT (torch.topk fails there too). */
+#define CTRLORA_MLSD_TOPK 200
+int ctrlora_mlsd_decode(const float* tp, int ld, int c_center, int c_disp, int batch, int h, int w, float* score_ws,
+                        int* out_idx, float* out_val, void* stream);
 
 #ifdef __cplusplus
 }

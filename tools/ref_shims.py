@@ -3,8 +3,10 @@ third-party packages that are not installed (omegaconf, pytorch_lightning, open_
 (needs the HF hub).  Used only by tools/make_golden.py to generate tests/golden/*; never by the product or the
 GPU-side tests (the reference tree does not exist on the GPU box).
 """
+import contextlib
 import os
 import sys
+import tempfile
 import types
 
 import torch
@@ -323,3 +325,25 @@ def install_uniformer_shims():
         layers.trunc_normal_ = lambda t, mean=0.0, std=1.0, a=-2.0, b=2.0: nn.init.trunc_normal_(t, mean, std, a, b)
         timm.models, models.layers = models, layers
         sys.modules.update({"timm": timm, "timm.models": models, "timm.models.layers": layers})
+
+
+@contextlib.contextmanager
+def mlsd_on_cpu(state_dict):
+    """The unmodified reference annotator.mlsd, importable and runnable on the CPU for the duration of the block: yields
+    the module.  Tensor.cuda and Module.cuda are no-ops inside (its MLSDdetector and pred_lines call them), and its
+    annotator_ckpts_path points at a temporary directory holding `state_dict` as mlsd_large_512_fp32.pth, so the
+    detector loads it instead of downloading."""
+    if REFERENCE_ROOT not in sys.path:
+        sys.path.insert(0, REFERENCE_ROOT)
+    import importlib
+    mod = importlib.import_module("annotator.mlsd")
+    saved = (torch.Tensor.cuda, nn.Module.cuda, mod.annotator_ckpts_path)
+    with tempfile.TemporaryDirectory() as d:
+        torch.save(state_dict, os.path.join(d, "mlsd_large_512_fp32.pth"))
+        torch.Tensor.cuda = lambda self, *a, **k: self
+        nn.Module.cuda = lambda self, *a, **k: self
+        mod.annotator_ckpts_path = d
+        try:
+            yield mod
+        finally:
+            torch.Tensor.cuda, nn.Module.cuda, mod.annotator_ckpts_path = saved
