@@ -153,6 +153,8 @@ _ARGTYPES = {
     "ctrlora_dwconv_act_f16": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P],
     "ctrlora_upsample_bilinear2x_ld_f16": [_P, _I, _P, _I, _I, _I, _I, _I, _P],
     "ctrlora_mlsd_decode": [_P, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P],
+    "ctrlora_canny_classify": [_P, _L, _I, _I, _I, _I, _I, _P, _P],
+    "ctrlora_canny_hysteresis": [_P, _I, _I, _I, _P, _P, _P],
 }
 
 
@@ -257,4 +259,6 @@ EXPORTS = [
     "ctrlora_dwconv_act_f16",
     "ctrlora_upsample_bilinear2x_ld_f16",
     "ctrlora_mlsd_decode",
+    "ctrlora_canny_classify",
+    "ctrlora_canny_hysteresis",
 ]

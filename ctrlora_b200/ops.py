@@ -1472,6 +1472,42 @@ def mlsd_decode(tp, c_center, c_disp):
     return idx, val
 
 
+# ------------------------------------------------------------------------------------------------ Canny annotator
+CANNY_MAX_MAG = 2040  # the largest L1 Sobel magnitude of uint8 input: 4 * 255 + 4 * 255
+
+
+def canny_classify(x, lo, hi):
+    """cv2.Canny's gradient, non-maximum suppression and thresholds on uint8 [B, H, W, 3] (rows may be strided, pixels
+    and channels packed) with integer thresholds lo <= hi -> uint8 [B, H, W] classes: 0 none, 1 candidate (kept by the
+    suppression and m > lo), 2 strong (also m > hi).  Thresholds beyond the magnitudes' range [0, 2040] act as -1 or
+    2040, so they are clamped there before they cross the int32 ABI."""
+    _require_cuda(x)
+    assert x.dtype == torch.uint8 and x.dim() == 4 and x.shape[3] == 3
+    assert x.stride(3) == 1 and x.stride(2) == 3 and x.stride(0) == x.shape[1] * x.stride(1), "packed pixels required"
+    lo, hi = int(lo), int(hi)
+    assert lo <= hi, (lo, hi)
+    b, h, w, _ = x.shape
+    cls = torch.empty((b, h, w), device=x.device, dtype=torch.uint8)
+    clamp = lambda t: max(-1, min(t, CANNY_MAX_MAG))  # noqa: E731
+    _count()
+    check(_lib.load().ctrlora_canny_classify(_dp(x), x.stride(1), b, h, w, clamp(lo), clamp(hi), _dp(cls), _sp()),
+          "canny_classify")
+    return cls
+
+
+def canny_hysteresis(cls):
+    """cv2.Canny's hysteresis on the classes of canny_classify (uint8 [B, H, W], contiguous) -> uint8 [B, H, W]: 255 at
+    every candidate 8-connected through candidates to a strong pixel, else 0.  Four launches whatever the content."""
+    _require_cuda(cls)
+    assert cls.dtype == torch.uint8 and cls.is_contiguous() and cls.dim() == 3
+    b, h, w = cls.shape
+    ws = torch.empty((b, h, w), device=cls.device, dtype=torch.int32)
+    out = torch.empty_like(cls)
+    _count(4)
+    check(_lib.load().ctrlora_canny_hysteresis(_dp(cls), b, h, w, _dp(ws), _dp(out), _sp()), "canny_hysteresis")
+    return out
+
+
 def set_sm_limit(limit):
     """persistent GEMM grids use at most `limit` SMs (0 = all); baked into CUDA graphs at capture"""
     check(_lib.load().ctrlora_set_sm_limit(int(limit)), "set_sm_limit")

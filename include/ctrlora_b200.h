@@ -617,6 +617,31 @@ int ctrlora_seg_output(const float* logits, int ld, int classes, int batch, int 
 int ctrlora_mlsd_decode(const float* tp, int ld, int c_center, int c_disp, int batch, int h, int w, float* score_ws,
                         int* out_idx, float* out_val, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * Canny edges (annotator/canny/__init__.py CannyDetector: cv2.Canny(img, low, high) with apertureSize 3 and the L1
+ * gradient), bit for bit, in integer arithmetic.
+ *
+ * Classification: img uint8 [batch, h, w, 3] with row stride ld bytes (image stride h * ld, pixel stride 3) -> cls
+ * uint8 [batch, h, w]: 0 none, 1 candidate, 2 strong.  Per channel the 3 x 3 Sobel dx, dy with the border replicated
+ * and m = |dx| + |dy|; per pixel the (dx, dy, m) of the channel with the largest m (ties keep the lower channel).  With
+ * x = |dx|, y = |dy| << 15 and TG22 = 13573 the direction is horizontal if y < x TG22, vertical if y > x TG22 +
+ * (x << 16), else diagonal; magnitudes outside the image are 0 and a pixel is kept when m > m[left] && m >= m[right]
+ * (horizontal), m > m[up] && m >= m[down] (vertical), m > m[up-right] && m > m[down-left] (diagonal, dx and dy of
+ * opposite sign) or m > m[up-left] && m > m[down-right] (the other diagonal).  Candidate: kept and m > lo; strong:
+ * candidate and m > hi.  lo <= hi, both already floored (and swapped) on the host.  One launch.
+ *
+ * Hysteresis: cls as above -> out uint8 [batch, h, w], 255 at every candidate 8-connected through candidates to a
+ * strong pixel, else 0.  Union-find labelling in labels_ws (int32 [batch * h * w]) in four launches whatever the
+ * content (tile-local union, union across tile borders, flatten and flag the roots with a strong member, output), no
+ * host synchronisation, so the pair can be captured in a CUDA graph.  The atomics may link components in any order;
+ * the output does not depend on it.
+ *
+ * Both: batch * h * w < 2^31, batch <= 65535, else CTRLORA_STATUS_BAD_ARGUMENT. */
+int ctrlora_canny_classify(const unsigned char* img, long long ld, int batch, int h, int w, int lo, int hi,
+                           unsigned char* cls, void* stream);
+int ctrlora_canny_hysteresis(const unsigned char* cls, int batch, int h, int w, int* labels_ws, unsigned char* out,
+                             void* stream);
+
 #ifdef __cplusplus
 }
 #endif
